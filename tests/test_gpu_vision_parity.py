@@ -88,9 +88,9 @@ def test_lm_solve_matches_oracle(models):
 
 @pytest.mark.parametrize("inertial", [False, True])
 def test_eight_cameras_match_oracle(inertial):
-    """The maximum rig vcgpu_set_cameras accepts (8 cameras; 8 x poly3: G = 104, + IMU 119): the global block is 87 / 113 KB,
+    """Eight cameras, the most vcgpu_set_cameras accepts (8 x poly3: G = 104, + IMU 119): the global block is 87 / 113 KB,
     more than the 48 KB a kernel gets without the dynamic shared-memory opt-in; the persistent kernels do not fit and the
-    multi-launch engine runs the solve."""
+    multi-launch engine runs the solve.  Not the largest rig: 8 x kb4 + IMU has G = 127 (test_gpu_imu_engines.py)."""
     from oracle.binding import Oracle
     from vicalib_b200.capi import Calibrator
 

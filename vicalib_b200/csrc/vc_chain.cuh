@@ -62,6 +62,16 @@ __global__ void chain_init_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl
   if (tid == 0) L.orig[f] = f;
 }
 
+// dynamic shared memory of chain_eliminate_kernel<FD> with chunks of c nodes:
+// Sacc [G^2 + G] | Al [FD^2] | El [FD G] | gl [FD] | Ap [FD^2] | Uc [FD^2] | V [(c - 1) FD][FD + 2 FD + G + 1]
+template <int FD>
+__host__ inline size_t chain_eliminate_smem_bytes(int G, int c) {
+  const size_t g = static_cast<size_t>(G), w = 2 * FD + g + 1;
+  return (g * g + g + 3 * FD * FD + FD * g + FD + static_cast<size_t>(c - 1) * FD * (FD + w)) * sizeof(double);
+}
+// dynamic shared memory of dense_solve_kernel when it factors (modes 0 and 2): S [N^2] | rhs [N]
+__host__ inline size_t chain_dense_smem_bytes(int N) { return (static_cast<size_t>(N) * N + N) * sizeof(double); }
+
 struct ElimArgs {
   int G, c;
   const Ctl* ctl;

@@ -209,6 +209,7 @@ struct vcgpu_handle {
   unsigned long long* d_csync = nullptr;  // persistent inertial solve: two {barrier counter, weights queue} pairs
   unsigned cs_launches = 0;
   bool smem_optin_done = false;   // dynamic shared-memory opt-ins of the multi-launch engine's kernels (per device)
+  size_t elim_smem_max = 0, dense_smem_max = 0;  // ... what chain_eliminate_kernel / dense_solve_kernel may then ask for
   double* d_dsys = nullptr;       // persistent sharded inertial solve: the summed dense system in block form
   unsigned xchg_tag_dense = 0, xchg_tag_eval = 0;  // exchange numbers of the persistent inertial kernels (vc_xchg.cuh)
   double* d_dense = nullptr;      // [N*N+N] all-reduced dense system, N = G + 9*nranks
