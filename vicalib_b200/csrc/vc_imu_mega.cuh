@@ -37,6 +37,8 @@ constexpr int kCsGroups = kCsThreads / kCsGroup;
 // every kCsChunk-th node of a level is a separator; a level of at most kCsTop nodes joins the dense solve
 constexpr int kCsChunk = 8;
 constexpr int kCsTop = 4;
+constexpr int kCsBsItem = 16;  // level-0 back-substitution nodes a CTA takes at a time in the closing phase (two per warp)
+constexpr int kCsSyncWords = 8;  // counters of one launch (ChainSolveArgs::sync)
 // phase clock slots: elimination levels [0, 10), reduce 10, dense 11, back-substitution levels [12, 22), update 22
 enum { kCsProfElim = 0, kCsProfReduce = kMaxChainLevels, kCsProfDense, kCsProfBacksub, kCsProfUpdate = kCsProfBacksub + kMaxChainLevels,
        kCsProfWeights, kCsProfCount };
@@ -72,8 +74,9 @@ struct ChainSolveArgs {
   const double* ftime;
   double* wsqrt;
   double sigma_g, sigma_a;
-  unsigned long long* sync;     // {barrier counter, weights queue, barrier counter of the closing phases} of this launch
-  unsigned long long* sync_next;  // ... of the next launch (the host alternates two pairs): zeroed here
+  unsigned long long* sync;     // [kCsSyncWords] {barrier counter, weights queue, CTAs ready for level 0, level-0 items
+                                //  handed out, level-0 items done} of this launch
+  unsigned long long* sync_next;  // ... of the next launch (the host alternates two sets): zeroed here
 };
 
 // the Schur accumulator of a group: lower triangle of S packed row by row (row r at r (r + 1) / 2), then the right-hand
@@ -101,6 +104,15 @@ __host__ __device__ inline size_t chain_solve_smem_doubles(int G, int nranks = 1
   const size_t wts = (kCsThreads / wts::kTeam) * (sizeof(wts::Work) / sizeof(double) + 1);
   const size_t m = grp > dense ? grp : dense;
   return (m > wts ? m : wts) + 16;
+}
+
+// wait (one thread) until a grid-wide counter reaches target; what the arrivals wrote before their increment is visible
+__device__ __forceinline__ void spin_until(unsigned long long* c, unsigned long long target) {
+  unsigned long long v;
+  do {
+    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(c) : "memory");
+  } while (v < target);
+  __threadfence();
 }
 
 __device__ __forceinline__ void group_sync(int grp) {
@@ -501,49 +513,55 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
   tick(9);
 }
 
-// Back-substitution of one level: x_p = -Z_g - Z_L x_left - Z_R x_right - Z_E dc for every interior node p, one warp each
-// (warp gw of nw)
+// Back-substitution of one level: x_p = -Z_g - Z_L x_left - Z_R x_right - Z_E dc for every interior node p, one warp each.
+// Node slot t (interior node t mod (c - 1) of chunk t / (c - 1)) of a level's n_chunks * (c - 1) slots.
 template <int FD>
-__device__ __forceinline__ void chain_backsub_level(const ChainLevel cur, int l, double* delta, int64_t nfp, int G, int gw, int nw, int lane) {
+__device__ __forceinline__ void chain_backsub_node(const ChainLevel& cur, int l, double* delta, int64_t nfp, int G, int t, int lane) {
   const int w = 2 * FD + G + 1, c = kCsChunk;
   const double* dc = delta + nfp;
   const int n_eff = cur.n - cur.ghost;
-  const int n_chunks = (n_eff + c - 1) / c;
   int cl = 1;  // c^l
   for (int k = 0; k < l; ++k) cl *= c;
   // interior node q (0..c-2) of chunk j: p = j*c + 1 + q
-  for (int t = gw; t < n_chunks * (c - 1); t += nw) {
-    const int jc = t / (c - 1), p = jc * c + 1 + (t - jc * (c - 1));
-    if (p >= n_eff) continue;
-    const int s = jc * c;
-    const int r = s + c < n_eff ? s + c : (cur.ghost ? cur.n - 1 : cur.n);
-    // original frame of node p of level l: p * c^l (no ghost node on one GPU); a table lookup otherwise
-    const int os = cur.ghost ? (l > 0 ? cur.orig[s] : s) : s * cl, op = cur.ghost ? (l > 0 ? cur.orig[p] : p) : p * cl;
-    const double* xl = delta + static_cast<int64_t>(os) * FD;
-    const double* xr = r < cur.n ? delta + static_cast<int64_t>(cur.ghost ? (l > 0 ? cur.orig[r] : r) : r * cl) * FD : nullptr;
-    const double* Z = cur.Z + static_cast<int64_t>(p) * FD * w;
-    double* out = delta + static_cast<int64_t>(op) * FD;
-    double d[FD];
+  const int jc = t / (c - 1), p = jc * c + 1 + (t - jc * (c - 1));
+  if (p >= n_eff) return;
+  const int s = jc * c;
+  const int r = s + c < n_eff ? s + c : (cur.ghost ? cur.n - 1 : cur.n);
+  // original frame of node p of level l: p * c^l (no ghost node on one GPU); a table lookup otherwise
+  const int os = cur.ghost ? (l > 0 ? cur.orig[s] : s) : s * cl, op = cur.ghost ? (l > 0 ? cur.orig[p] : p) : p * cl;
+  const double* xl = delta + static_cast<int64_t>(os) * FD;
+  const double* xr = r < cur.n ? delta + static_cast<int64_t>(cur.ghost ? (l > 0 ? cur.orig[r] : r) : r * cl) * FD : nullptr;
+  const double* Z = cur.Z + static_cast<int64_t>(p) * FD * w;
+  double* out = delta + static_cast<int64_t>(op) * FD;
+  double d[FD];
 #pragma unroll
-    for (int rr = 0; rr < FD; ++rr) d[rr] = 0.0;
-    for (int q = lane; q < w - 1; q += 32) {
-      const double x = q < FD ? __ldcg(xl + q) : q < 2 * FD ? (xr ? __ldcg(xr + q - FD) : 0.0) : __ldcg(dc + q - 2 * FD);
+  for (int rr = 0; rr < FD; ++rr) d[rr] = 0.0;
+  for (int q = lane; q < w - 1; q += 32) {
+    const double x = q < FD ? __ldcg(xl + q) : q < 2 * FD ? (xr ? __ldcg(xr + q - FD) : 0.0) : __ldcg(dc + q - 2 * FD);
 #pragma unroll
-      for (int rr = 0; rr < FD; ++rr) d[rr] += __ldcg(Z + rr * w + q) * x;
-    }
-#pragma unroll
-    for (int rr = 0; rr < FD; ++rr) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) d[rr] += __shfl_xor_sync(0xffffffffu, d[rr], o);
-      d[rr] = -__ldcg(Z + rr * w + w - 1) - d[rr];
-    }
-    if (lane < FD) {
-      double v = d[0];
-#pragma unroll
-      for (int rr = 1; rr < FD; ++rr) v = lane == rr ? d[rr] : v;
-      out[lane] = v;
-    }
+    for (int rr = 0; rr < FD; ++rr) d[rr] += __ldcg(Z + rr * w + q) * x;
   }
+#pragma unroll
+  for (int rr = 0; rr < FD; ++rr) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) d[rr] += __shfl_xor_sync(0xffffffffu, d[rr], o);
+    d[rr] = -__ldcg(Z + rr * w + w - 1) - d[rr];
+  }
+  if (lane < FD) {
+    double v = d[0];
+#pragma unroll
+    for (int rr = 1; rr < FD; ++rr) v = lane == rr ? d[rr] : v;
+    out[lane] = v;
+  }
+}
+__host__ __device__ inline int chain_backsub_slots(const ChainLevel& cur) {
+  return (cur.n - cur.ghost + kCsChunk - 1) / kCsChunk * (kCsChunk - 1);
+}
+// all of a level, warp gw of nw
+template <int FD>
+__device__ __forceinline__ void chain_backsub_level(const ChainLevel cur, int l, double* delta, int64_t nfp, int G, int gw, int nw, int lane) {
+  const int n_slots = chain_backsub_slots(cur);
+  for (int t = gw; t < n_slots; t += nw) chain_backsub_node<FD>(cur, l, delta, nfp, G, t, lane);
 }
 
 // x (+) step of one frame into the trial state, and the frame's share of the step statistics
@@ -741,7 +759,8 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
   __shared__ unsigned long long wtask;
   __shared__ unsigned long long* xbufs[kMaxRanks];
   xchg_stage(a.x, xbufs);  // (visible after the first barrier below)
-  if (bid == 0 && tid == 0) { a.sync_next[0] = 0ull; a.sync_next[1] = 0ull; a.sync_next[2] = 0ull; }
+  if (bid == 0 && tid == 0)
+    for (int k = 0; k < kCsSyncWords; ++k) a.sync_next[k] = 0ull;
   if (a.ctl->done) return;  // uniform over the grid: written before this launch
   const Blocks& b = a.b[a.ctl->cur];
   const double rinv = 1.0 / a.ctl->radius;
@@ -1146,14 +1165,46 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
       if (step == 2) mark(kCsProfWeights);
       continue;
     }
-    bar = a.sync + 2;  // the closing phases: the whole grid again, on their own counter
-    bar_target = 0;
-    n_act = nb;
-    barrier(nb);
+    // ---------------------------------------------------------- closing phases.  The CTAs that stayed with the solve
+    // get here when the levels above level 0 are back-substituted, the CTAs that left when the weights queue is empty.
+    // Nobody waits for everybody: level 0 is handed out in items of kCsBsItem nodes, off a counter, to whoever is here
+    // once the levels above are done — a CTA still busy with its last weights task holds up neither the
+    // back-substitution nor the update of the others (the queue used to keep them all at a grid barrier).  Which warp
+    // does a node changes nothing in its result, and the update keeps its fixed frames per CTA.
+    unsigned long long* ready = a.sync + 2;  // CTAs that stayed with the solve and are done with the levels above
+    unsigned long long* items = a.sync + 3;  // level-0 items handed out
+    unsigned long long* done = a.sync + 4;   // level-0 items finished
+    if (!left) {
+      __syncthreads();
+      if (tid == 0) {
+        __threadfence();
+        atomicAdd(ready, 1ull);
+      }
+    }
     if (a.n_levels >= 2) {
-      chain_backsub_level<FD>(a.lev[0], 0, a.delta, nfp, G, bid * (kCsThreads / 32) + warp, nb * (kCsThreads / 32), lane);
+      const ChainLevel L0 = a.lev[0];
+      const int n_items = (chain_backsub_slots(L0) + kCsBsItem - 1) / kCsBsItem;
+      if (tid == 0) spin_until(ready, static_cast<unsigned long long>(ns));
+      __syncthreads();
+      for (;;) {
+        if (tid == 0) wtask = atomicAdd(items, 1ull);
+        __syncthreads();
+        const long long it = static_cast<long long>(wtask);
+        if (it >= n_items) break;
+#pragma unroll
+        for (int u = 0; u < kCsBsItem / (kCsThreads / 32); ++u)
+          chain_backsub_node<FD>(L0, 0, a.delta, nfp, G, static_cast<int>(it) * kCsBsItem + u * (kCsThreads / 32) + warp, lane);
+        __syncthreads();
+        if (tid == 0) {
+          __threadfence();
+          atomicAdd(done, 1ull);
+        }
+      }
       mark(kCsProfBacksub + (a.n_levels - 2));
-      barrier(nb);
+      if (a.do_update) {  // the update reads every frame's step
+        if (tid == 0) spin_until(done, static_cast<unsigned long long>(n_items));
+        __syncthreads();
+      }
     }
     if (!a.do_update) continue;
     // ---------------------------------------------------------- x (+) step of every frame, one thread each (the top

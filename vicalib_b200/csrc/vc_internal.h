@@ -206,7 +206,7 @@ struct vcgpu_handle {
   int rank = 0, nranks = 1;
   double* d_mg = nullptr;         // all-reduce buffer [G*G+G+6+nranks (+ 18*nranks)]
   double* d_sep = nullptr;        // [2][nranks*9]: summed diag(B) and g of the separator frames (sharded inertial runs)
-  unsigned long long* d_csync = nullptr;  // persistent inertial solve: two {barrier counter, weights queue} pairs
+  unsigned long long* d_csync = nullptr;  // persistent inertial solve: two sets of kCsSyncWords counters (ChainSolveArgs::sync)
   unsigned cs_launches = 0;
   bool smem_optin_done = false;   // dynamic shared-memory opt-ins of the multi-launch engine's kernels (per device)
   size_t elim_smem_max = 0, dense_smem_max = 0;  // ... what chain_eliminate_kernel / dense_solve_kernel may then ask for
