@@ -3,13 +3,16 @@
 It restates what the host and the kernels decide from the problem's shape alone: the level table of `imu_prepare`
 (vc_imu_host.inl), the per-level dispatch of `chain_solve_kernel` (narrow or wide, rounds of chunks, which CTAs leave
 for the deferred weight update), the dense solve's tile count, the persistent-fit decision of `imu_mega_prepare`
-(vc_engine.inl) and the dynamic shared memory every chain kernel asks for.  The tests use it to pick frame counts and
-rigs that land on a given branch, and to check that branch is the one the numbers say.
+(vc_engine.inl) and the dynamic shared memory every chain kernel asks for, and the loop shapes of the DOGLEG kernels
+(vc_dogleg.cuh).  The tests use it to pick frame counts and rigs that land on a given branch, and to check that branch
+is the one the numbers say.  Its plain reference (`arrow_matvec`, `backward_error`) works on the block normal equations
+in long double.
 
 The shape constants (`kCsChunk`, `kCsTop`, ...) are read from the CUDA sources, so a change of chunk length moves the
 test cases with it.
 """
 import ctypes
+import itertools
 import math
 import os
 import re
@@ -41,7 +44,7 @@ def _constants():
     """Every `constexpr int NAME = <integer arithmetic>;` of the headers the plan depends on, evaluated."""
     raw = {}
     for name in ("vc_internal.h", "vc_kernels.cuh", "vc_fused.cuh", "vc_mega.cuh", "vc_imu_weights.cuh", "vc_imu_mega.cuh",
-                 "vc_imu_eval_mega.cuh"):
+                 "vc_imu_eval_mega.cuh", "vc_dogleg.cuh"):
         for k, expr in _CONST.findall(_read(name)):
             raw.setdefault(k, re.sub(r"//.*", "", expr).strip())
     vals, busy = {}, set()
@@ -285,6 +288,30 @@ def rig_globals(models, inertial=True):
     return sum(6 + MODEL_K[m] for m in models) + (IMU_GLOBALS if inertial else 0)
 
 
+def rig_with_globals(G, inertial=True):
+    """The first rig (fewest cameras, then models in MODEL_K order) with G globals."""
+    for n in range(1, MAX_CAMS + 1):
+        for models in itertools.combinations_with_replacement(MODEL_K, n):
+            if rig_globals(models, inertial) == G:
+                return models
+    raise ValueError(f"no rig of at most {MAX_CAMS} cameras has {G} globals")
+
+
+# ------------------------------------------------------------------------------------------------ the DOGLEG kernels
+DL_BLOCKS, MV_WARPS = K["kDlBlocks"], K["kMvWarps"]
+
+
+def matvec_parts(n_frames):
+    """Per-CTA partials of E^T w_f that arrow_matvec_globals_kernel sums (one warp per frame)."""
+    return (n_frames + MV_WARPS - 1) // MV_WARPS
+
+
+def dot_passes(n):
+    """Passes of dl_dots_kernel's 256-thread loop over the largest of its DL_BLOCKS slices of n entries."""
+    width = max((n * (b + 1)) // DL_BLOCKS - (n * b) // DL_BLOCKS for b in range(DL_BLOCKS))
+    return (width + 255) // 256
+
+
 def engine_smem_optin(device_optin=H100_SMEM_OPTIN):
     """The dynamic shared memory the multi-launch engine opts its chain kernels in to (kernel_smem_optin): the device's
     per-block opt-in less the kernel's static shared memory, unless the source names a fixed size."""
@@ -297,25 +324,46 @@ def engine_smem_optin(device_optin=H100_SMEM_OPTIN):
 
 
 # ------------------------------------------------------------------------------------------------ plain reference
+def scaled_blocks(ne, scale):
+    """The blocks of S H S and S g in long double.  H is block tridiagonal + arrow: B[f] on the diagonal,
+    U[f] = H[f-1, f], E[f] = H[f, globals], C = H[globals, globals]; returns U[k] = H[k, k+1], k = 0 .. nf-2."""
+    ld = np.longdouble
+    nf, fd, _ = ne["B"].shape
+    nfp = nf * fd
+    sf, sc = scale[:nfp].reshape(nf, fd).astype(ld), scale[nfp:].astype(ld)
+    return dict(B=ne["B"].astype(ld) * sf[:, :, None] * sf[:, None, :],
+                U=ne["U"][1:].astype(ld) * sf[:-1, :, None] * sf[1:, None, :],
+                E=ne["E"].astype(ld) * sf[:, :, None] * sc[None, None, :],
+                C=ne["C"].astype(ld) * sc[:, None] * sc[None, :],
+                gf=ne["gf"].astype(ld) * sf, gc=ne["gc"].astype(ld) * sc)
+
+
+def arrow_matvec(ne, scale, x):
+    """y = S H S x in long double, x and y of length nf fd + G (frames first, then the globals)."""
+    sb = scaled_blocks(ne, scale)
+    nf, fd, _ = ne["B"].shape
+    nfp = nf * fd
+    x = np.asarray(x)
+    xf, xc = x[:nfp].reshape(nf, fd).astype(np.longdouble), x[nfp:].astype(np.longdouble)
+    yf = np.einsum("fij,fj->fi", sb["B"], xf) + np.einsum("fij,j->fi", sb["E"], xc)
+    yf[:-1] += np.einsum("kij,kj->ki", sb["U"], xf[1:])
+    yf[1:] += np.einsum("kji,kj->ki", sb["U"], xf[:-1])
+    yc = sb["C"] @ xc + np.einsum("fij,fi->j", sb["E"], xf)
+    return np.concatenate([yf.ravel(), yc])
+
+
 def backward_error(ne, scale, D2, x):
-    """Normwise backward error of x as a solution of (S H S + diag(D2)) x = -S g, in long double.  H is block
-    tridiagonal + arrow: B[f] on the diagonal, U[f] = H[f-1, f], E[f] = H[f, globals], C = H[globals, globals]."""
+    """Normwise backward error of x as a solution of (S H S + diag(D2)) x = -S g, in long double."""
     ld = np.longdouble
     nf, fd, _ = ne["B"].shape
     G = ne["C"].shape[0]
     nfp = nf * fd
-    sf, sc = scale[:nfp].reshape(nf, fd).astype(ld), scale[nfp:].astype(ld)
+    sb = scaled_blocks(ne, scale)
+    B, U, E, C, gf, gc = (sb[k] for k in ("B", "U", "E", "C", "gf", "gc"))
     df, dc = D2[:nfp].reshape(nf, fd).astype(ld), D2[nfp:].astype(ld)
     xf, xc = x[:nfp].reshape(nf, fd).astype(ld), x[nfp:].astype(ld)
-    B = ne["B"].astype(ld) * sf[:, :, None] * sf[:, None, :]
-    U = ne["U"][1:].astype(ld) * sf[:-1, :, None] * sf[1:, None, :]  # U[k] = H[k, k+1], k = 0 .. nf-2
-    E = ne["E"].astype(ld) * sf[:, :, None] * sc[None, None, :]
-    C = ne["C"].astype(ld) * sc[:, None] * sc[None, :]
-    gf, gc = ne["gf"].astype(ld) * sf, ne["gc"].astype(ld) * sc
-    rf = np.einsum("fij,fj->fi", B, xf) + df * xf + np.einsum("fij,j->fi", E, xc) + gf
-    rf[:-1] += np.einsum("kij,kj->ki", U, xf[1:])
-    rf[1:] += np.einsum("kji,kj->ki", U, xf[:-1])
-    rc = C @ xc + dc * xc + np.einsum("fij,fi->j", E, xf) + gc
+    r = arrow_matvec(ne, scale, x) + D2.astype(ld) * x.astype(ld)
+    rf, rc = r[:nfp].reshape(nf, fd) + gf, r[nfp:] + gc
     nrm_f = np.abs(B).sum(2) + np.abs(df) + np.abs(E).sum(2)
     nrm_f[:-1] += np.abs(U).sum(2)
     nrm_f[1:] += np.abs(U).sum(1)

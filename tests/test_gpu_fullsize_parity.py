@@ -23,8 +23,12 @@ def _rel(a, b, floor):
     return float(np.max(np.abs(a - b) / np.maximum(np.abs(b), floor)))
 
 
-@pytest.mark.parametrize("name", ["config2", "config3", "target"])
-def test_fullsize_normal_equations_and_converged_parameters(name):
+@pytest.mark.parametrize("name,strategy", [("config2", 0), ("config3", 0), ("target", 0), ("config2", 1), ("target", 1)],
+                         ids=["config2", "config3", "target", "config2_dogleg", "target_dogleg"])
+def test_fullsize_normal_equations_and_converged_parameters(name, strategy):
+    """LM with tight tolerances; DOGLEG with the reference's own settings (what the C++ ViCalibrator runs: function
+    tolerance 1e-6, the other options at their defaults, live weights), whose weights after the solve are compared
+    too."""
     from oracle.binding import Oracle
     from vicalib_b200.capi import Calibrator
 
@@ -42,7 +46,10 @@ def test_fullsize_normal_equations_and_converged_parameters(name):
     for k in keys:
         assert _relerr(ne_g[k], ne_o[k]) <= 1e-9, k
     # ---- to convergence, same options (Ceres' rules; live UpdateImuWeights on the inertial configs)
-    opts = dict(max_iters=60, function_tol=1e-12, gradient_tol=1e-14, param_tol=1e-14)
+    if strategy == 0:
+        opts = dict(max_iters=60, function_tol=1e-12, gradient_tol=1e-14, param_tol=1e-14)
+    else:
+        opts = dict(max_iters=200, function_tol=1e-6, gradient_tol=1e-10, param_tol=1e-8, strategy=1, update_imu_weights=1)
     o.set_options(num_threads=os.cpu_count() or 4, **opts)
     g.set_options(**opts)
     s_o, s_g = o.solve(), g.solve()
@@ -62,6 +69,9 @@ def test_fullsize_normal_equations_and_converged_parameters(name):
         assert _rel(st_g["b"], st_o["b"], 1e-3) <= 1e-6
         assert _rel(st_g["sf"], st_o["sf"], 1.0) <= 1e-6
         assert abs(st_g["ts"] - st_o["ts"]) <= 1e-6 * 1e-3
+        if strategy == 1:
+            W_o = o.imu_weights()
+            np.testing.assert_allclose(g.imu_weights(), W_o, rtol=1e-6, atol=1e-6 * np.abs(W_o).max())
 
 
 def test_lm_with_live_weights_converges_tight():

@@ -10,6 +10,8 @@
   multi-launch engine, and the same run with every CTA but one kept in the solve (bit for bit) and with the weights
   computed in the evaluation launch instead (to rounding).  The weights are compared after the solve: the update the
   last accepted step calls for must have run on every path.
+- The same without an oracle, on both strategies and engines and whatever ends the solve: one more update after the
+  solve leaves the weights as they are.
 
 Which frame counts reach which branch comes from the host model of the plan (chain_plan.py).
 """
@@ -213,3 +215,35 @@ def test_deferred_weights_queue(tmp_path):
     assert iters == WEIGHTS_ITERS and accepted == s_g["successful_steps"] and launches <= 2 * iters + 12
     assert (np.abs(W - W_g).max((1, 2)) / np.abs(W_g).max((1, 2))).max() <= 1e-10
     assert np.abs(T - st_g["T_wp"]).max() <= 1e-12 * np.abs(st_g["T_wp"]).max()
+
+
+@pytest.mark.parametrize("stop", ["max_iters", "function_tol", "gradient_tol"])
+@pytest.mark.parametrize("mode", [0, MULTI_LAUNCH], ids=["persistent", "multi_launch"])
+@pytest.mark.parametrize("strategy", [0, 1], ids=["lm", "dogleg"])
+def test_weights_are_current_after_solve(strategy, mode, stop):
+    """Whatever ends a solve with live weights, the weights it leaves are those of its last accepted state: updating
+    them once more changes them only to rounding (the update after the solve runs in imu_weights_kernel, the one in
+    the persistent solve launch in another kernel; see test_deferred_weights_queue)."""
+    p = synth.make_problem(models=("poly3",), n_frames=40, grid=(14, 10), inertial=True, seed=29)
+    base = dict(strategy=strategy, function_tol=0.0, gradient_tol=0.0, param_tol=0.0, update_imu_weights=1)
+    if stop == "max_iters":
+        opts, term = dict(base, max_iters=4), 0
+    elif stop == "function_tol":
+        opts, term = dict(base, max_iters=100, function_tol=1e-6), 1
+    else:  # a gradient tolerance between an accepted step's largest gradient entry and every earlier one
+        rows = _calibrator(p, mode, **dict(base, max_iters=8)).solve()["rows"]
+        gmax = rows[:, 3]
+        k = next(it for it in range(2, len(rows)) if rows[it, 8] == 1 and gmax[it] < 0.99 * gmax[:it].min())
+        opts, term = dict(base, max_iters=k + 4, gradient_tol=float(np.sqrt(gmax[k] * gmax[:k].min()))), 2
+    g = _calibrator(p, mode, **opts)
+    s = g.solve()
+    assert s["termination"] == term
+    if strategy == 0:
+        assert _persistent_ran(s) == (mode == 0), s["kernel_launches"]
+    if stop != "function_tol":
+        assert s["rows"][-1, 8] == 1  # the solve ends on an accepted step
+    W = g.imu_weights()
+    assert np.abs(W - 500 * np.eye(9)).max() > 1.0  # the weights did change
+    g.update_imu_weights()
+    rel = (np.abs(g.imu_weights() - W).max((1, 2)) / np.abs(W).max((1, 2))).max()
+    assert rel <= 1e-10, rel

@@ -172,7 +172,9 @@ class Calibrator:
         self._chk(self.L.vcgpu_comm_init(self.h, buf, C.c_int(rank), C.c_int(nranks)))
 
     # ---- hot path
-    def solve(self, callback=None):
+    def solve(self, callback=None, free_running=False):
+        """Solve; `rows` holds one row per iteration.  free_running: no iteration callback at all, so the device runs
+        the loop in batches without a host round trip per iteration (no rows; `callback` must be None)."""
         s = Summary()
         rows = []
 
@@ -182,7 +184,9 @@ class Calibrator:
                          it.step_norm, it.relative_decrease, it.trust_region_radius, it.step_is_successful])
             return int(callback(it)) if callback else 0
 
-        cb = ITER_CB(_cb)
+        if free_running and callback is not None:
+            raise ValueError("a free-running solve takes no callback")
+        cb = None if free_running else ITER_CB(_cb)
         self._chk(self.L.vcgpu_solve(self.h, cb, None, C.byref(s)))
         out = {f[0]: getattr(s, f[0]) for f in Summary._fields_}
         out["rows"] = np.array(rows)
