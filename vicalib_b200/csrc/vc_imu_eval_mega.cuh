@@ -218,6 +218,18 @@ __device__ inline void evm_build_frame(const EvalMegaArgs& a, const Blocks& bt, 
   if (lane == 0) a.cost_part[f] = cost;
 }
 
+// Phase W: the weights of intervals bid * 16 + k (+ grid * 16 ...), a team of 16 lanes each.  A function of its own, as
+// the solve kernel's weights queue (chain_weights_queue): inlined, its registers join the kernel's and both spill more.
+__device__ __noinline__ void eval_weights(const WeightQueueArgs w, const double* xs, double* smem) {
+  constexpr int kTeams = kEvThreads / wts::kTeam;
+  const int tid = threadIdx.x, warp = tid >> 5, team = tid / wts::kTeam, tl = tid & (wts::kTeam - 1);
+  wts::Work* work = reinterpret_cast<wts::Work*>(smem);
+  for (int base = blockIdx.x * kTeams; base < w.ni; base += gridDim.x * kTeams) {
+    if (base + (warp * (32 / wts::kTeam)) >= w.ni) break;  // whole warp past the end
+    wts::imu_weights_team(w, xs, base + team, &work[team], tl);
+  }
+}
+
 __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a) {
   extern __shared__ double smem[];
   namespace cg = cooperative_groups;
@@ -443,15 +455,10 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
   {
     const volatile Ctl* c = a.ctl;
     if (c->done || !(c->iter == 0 || c->last_accepted)) return;  // uniform: written before the barrier
-    const wts::WeightView wa{a.dp, a.buf, a.ftime, a.wsqrt, ni, a.sigma_g, a.sigma_a};
-    const double* xs = a.state[c->cur];
-    constexpr int kTeams = kEvThreads / wts::kTeam;
-    wts::Work* work = reinterpret_cast<wts::Work*>(smem);
-    const int team = tid / wts::kTeam, tl = tid & (wts::kTeam - 1);
-    for (int base = bid * kTeams; base < ni; base += nb * kTeams) {
-      if (base + (warp * (32 / wts::kTeam)) >= ni) break;  // whole warp past the end
-      wts::imu_weights_team(wa, xs, base + team, &work[team], tl);
-    }
+    WeightQueueArgs wa;
+    wa.dp.off_v = a.dp.off_v; wa.dp.off_imu = a.dp.off_imu; wa.buf = a.buf; wa.ftime = a.ftime; wa.wsqrt = a.wsqrt;
+    wa.ni = ni; wa.sigma_g = a.sigma_g; wa.sigma_a = a.sigma_a;
+    eval_weights(wa, a.state[c->cur], smem);
   }
   mark(kEvProfWeights);
 }

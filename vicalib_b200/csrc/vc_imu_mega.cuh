@@ -39,6 +39,7 @@ constexpr int kCsChunk = 8;
 constexpr int kCsTop = 4;
 constexpr int kCsBsItem = 16;  // level-0 back-substitution nodes a CTA takes at a time in the closing phase (two per warp)
 constexpr int kCsSyncWords = 8;  // counters of one launch (ChainSolveArgs::sync)
+constexpr int kCsRedLoads = 16;  // loads a thread of the Schur reduction keeps in flight
 // phase clock slots: elimination levels [0, 10), reduce 10, dense 11, back-substitution levels [12, 22), update 22
 enum { kCsProfElim = 0, kCsProfReduce = kMaxChainLevels, kCsProfDense, kCsProfBacksub, kCsProfUpdate = kCsProfBacksub + kMaxChainLevels,
        kCsProfWeights, kCsProfCount };
@@ -51,7 +52,7 @@ struct ChainSolveArgs {
   const double* D2x;            // explicit damping (inspection hook / dogleg) or null: LM rule
   const ChainLevel* lev;        // [n_levels] level descriptors (device memory)
   int n_levels;
-  double* Spart;                // [grid][G*G+G] one Schur partial per CTA
+  double* Spart;                // [grid][G*G+G] one Schur partial per CTA, packed (chain_sacc_doubles(G) entries used)
   double* Ssum;                 // [G*G+G]
   double* delta;                // scaled step [nf*9 + G]
   double* scalars;
@@ -840,10 +841,9 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
       __syncthreads();                             // accumulators added: half as many partials for the reduction)
       double* out = a.Spart + static_cast<int64_t>(bid) * NS;
       const double* g1 = smem + chain_group_doubles(G);
-      for (int e = tid, r = tid / G, q = tid % G; e < NS; e += kCsThreads, adv2(r, q, G, kCsThreads)) {  // unpacked: the square
-        const int k = r < G ? (q <= r ? r * (r + 1) / 2 + q : -1) : G * (G + 1) / 2 + q;         // (upper triangle 0),
-        out[e] = k >= 0 ? smem[k] + g1[k] : 0.0;                                                  // then the rhs
-      }
+#pragma unroll 1
+      for (int e = tid; e < chain_sacc_doubles(G); e += kCsThreads) out[e] = smem[e] + g1[e];  // packed, as accumulated
+
       if (gtid == 0 && bad_s[grp]) a.scalars[kScNotPD] = 1.0;
     }
     mark(kCsProfElim + l);
@@ -877,7 +877,28 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
     }
   }
   // ------------------------------------------------------------ Schur partials -> total (fixed order), distributed
-  mega_reduce_stage1(a.Spart, NS, nb, NS, a.Ssum, -1, -1, bid, ns);
+  // Entry e of the square total by one thread of the first ns CTAs: it adds the packed entry up over the nb partials in
+  // CTA order, kCsRedLoads loads in flight (neighbouring threads read neighbouring entries), and writes it unpacked:
+  // lower triangle, upper triangle 0, then the right-hand side.  32-bit offsets (grid x (G^2 + G) < 2^31 for G <= 127):
+  // 64-bit ones cost the kernel more spills.
+  for (int e = bid * kCsThreads + tid; e < NS; e += ns * kCsThreads) {
+    const int r = e / G, q = e - r * G;
+    const int k = r < G ? (q <= r ? r * (r + 1) / 2 + q : -1) : G * (G + 1) / 2 + q;
+    double s = 0.0;
+    if (k >= 0) {
+      const double* p = a.Spart + k;
+      int c = 0;
+      for (; c + kCsRedLoads <= nb; c += kCsRedLoads) {
+        double v[kCsRedLoads];
+#pragma unroll
+        for (int u = 0; u < kCsRedLoads; ++u) v[u] = __ldcg(p + (c + u) * NS);
+#pragma unroll
+        for (int u = 0; u < kCsRedLoads; ++u) s += v[u];
+      }
+      for (; c < nb; ++c) s += __ldcg(p + c * NS);
+    }
+    a.Ssum[e] = s;
+  }
   mark(kCsProfReduce);
   barrier(ns);
   // ------------------------------------------------------------ sharded: the ranks' partial systems meet here

@@ -318,20 +318,15 @@ struct WeightArgs {
   double sigma_g, sigma_a;
   int deferred;  // 1: the update the persistent solve kernel would have run for the last iteration (ignores `done`)
 };
-struct WeightView {  // WeightArgs' fields with the problem description by reference (persistent kernel)
-  const DevProblem& dp;
-  imu::ImuBuf buf;
-  const double* ftime;
-  double* wsqrt;
-  int ni;
-  double sigma_g, sigma_a;
-};
 constexpr int kWtWarps = 4;                              // warps per CTA
 constexpr int kWtTeams = kWtWarps * (32 / kTeam);        // intervals per CTA
 
 // The weights of one interval: everything after the covariance chain (vicalibrator.h:755-796).  Team-collective;
 // `on` team-uniform.  Writes the 9x9 weight_sqrt_ to `out` (left untouched when the information matrix is singular).
-__device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const double* X2, Work* W, int tl, bool on, double* out) {
+// `vec` holds the interval's eigenvectors from its last update (all NaN: none, start from the identity); the
+// eigen-decomposition starts from them and leaves its own there.
+__device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const double* X2, Work* W, int tl, bool on, double* out,
+                                                double* vec) {
   // t12 = T_end * T_2w, T_2w = T_w2^-1
   const Quat<double> q2i = imu::qconj(Quat<double>{X2[0], X2[1], X2[2], X2[3]});
   const Vec<double> t2 = imu::qrot(q2i, Vec<double>{X2[4], X2[5], X2[6]});
@@ -373,15 +368,38 @@ __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const dou
   // one cyclic Jacobi eigen-decomposition of the symmetrised P (no explicit inverse).  Round r of a sweep holds the
   // four disjoint pairs {i, j}, i + j = r (mod 9), i < j; their rotations are computed from the same matrix by four
   // lanes and applied together (columns of A and V, then rows of A).
+  // Warm start: W does not depend on which orthogonal V diagonalises P, so the sweeps start from the interval's
+  // eigenvectors of its last update, V_prev, with A = V_prev^T sym(P) V_prev — nearly diagonal when the state moved
+  // little.  Without them (NaN: after an upload, a weights upload, a flag change, at the start of a solve) V starts as
+  // the identity, and the products below are exact: A = sym(P) bit for bit.
+  bool cold = false;
   if (on)
+    for (int e = tl; e < 81; e += kTeam) {
+      const double v = vec[e];
+      cold = cold || v != v;
+      V[e] = v;
+    }
+  cold = ((__ballot_sync(0xffffffffu, cold) >> (threadIdx.x & 16)) & 0xffffu) != 0;  // any lane of this team
+  if (on && cold)
+    for (int e = tl; e < 81; e += kTeam) V[e] = (e % 10 == 0) ? 1.0 : 0.0;
+  __syncwarp();
+  if (on)  // t1 = sym(P) V
+    for (int e = tl; e < 81; e += kTeam) {
+      const int r = e / 9, c = e - r * 9;
+      double s = 0.0;
+      for (int k = 0; k < 9; ++k) s += 0.5 * (A[r * 9 + k] + A[k * 9 + r]) * V[k * 9 + c];
+      W->t1[e] = s;
+    }
+  __syncwarp();
+  if (on)  // A = V^T t1, its upper triangle mirrored
     for (int e = tl; e < 81; e += kTeam) {
       const int r = e / 9, c = e - r * 9;
       if (c >= r) {
-        const double v = 0.5 * (A[r * 9 + c] + A[c * 9 + r]);
-        W->t2[r * 9 + c] = v;
-        W->t2[c * 9 + r] = v;
+        double s = 0.0;
+        for (int k = 0; k < 9; ++k) s += V[k * 9 + r] * W->t1[k * 9 + c];
+        W->t2[r * 9 + c] = s;
+        W->t2[c * 9 + r] = s;
       }
-      V[e] = r == c ? 1.0 : 0.0;
     }
   __syncwarp();
   A = W->t2;
@@ -445,6 +463,7 @@ __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const dou
     }
   }
   if (!on) return;
+  for (int e = tl; e < 81; e += kTeam) vec[e] = V[e];  // the next update of this interval starts from them
   bool singular = false;
 #pragma unroll
   for (int k = 0; k < 9; ++k) singular = singular || !(A[k * 9 + k] > 0.0);
@@ -492,7 +511,7 @@ __device__ __forceinline__ void imu_weights_team(const A& a, const double* state
     y = integrate_imu_cov(y, prev, cur, bg, ba, sf, g, sg2, sa2, W, tl, step);
     if (step) prev = cur;
   }
-  weight_from_cov(y, X2, W, tl, on, a.wsqrt + static_cast<int64_t>(ki) * 81);
+  weight_from_cov(y, X2, W, tl, on, a.wsqrt + static_cast<int64_t>(ki) * 81, a.wsqrt + static_cast<int64_t>(a.ni + ki) * 81);
 }
 
 __global__ void __launch_bounds__(32 * kWtWarps, 2) imu_weights_kernel(WeightArgs a) {

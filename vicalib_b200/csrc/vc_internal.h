@@ -192,7 +192,9 @@ struct vcgpu_handle {
   // IMU
   double* d_imu = nullptr;        // [7][n_imu]: t w3 a3
   int n_imu = 0;
-  double* d_wsqrt = nullptr;      // [(nf-1)][81]
+  double* d_wsqrt = nullptr;      // [2][(nf-1)][81]: the weights, then d_wvec
+  double* d_wvec = nullptr;       // [(nf-1)][81] eigenvectors of each interval's last weights update (all NaN: none)
+  bool wvec_cold = true;          // d_wvec is to be reset (prepare) before the next weights update
   double* d_imu_r = nullptr;      // [(nf-1)][9]
   double* d_imu_J = nullptr;      // [(nf-1)][9*33]
   void* imu = nullptr;            // ImuDevHost (vc_imu_host.inl)

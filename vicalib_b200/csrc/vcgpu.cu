@@ -217,7 +217,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
   dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
-  dev_free(&h->d_imu); dev_free(&h->d_wsqrt); dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
+  dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
   xchg_release(h);
@@ -258,6 +258,7 @@ extern "C" int vcgpu_set_cameras(vcgpu_handle* h, int n, const int32_t* model, c
   h->h_qck.assign(q_ck, q_ck + 4 * n);
   h->h_pck.assign(p_ck, p_ck + 3 * n);
   h->state_dirty = true;
+  h->wvec_cold = true;
   return VCGPU_OK;
 }
 extern "C" int vcgpu_set_frames(vcgpu_handle* h, int n, const double* T_wp, const double* v_w, const double* time) {
@@ -269,6 +270,7 @@ extern "C" int vcgpu_set_frames(vcgpu_handle* h, int n, const double* T_wp, cons
   if (h->h_time.size() != static_cast<size_t>(n) || !std::equal(time, time + n, h->h_time.begin())) h->dirty = true;
   h->h_time.assign(time, time + n);
   h->state_dirty = true;
+  h->wvec_cold = true;
   return VCGPU_OK;
 }
 extern "C" int vcgpu_set_observations(vcgpu_handle* h, int64_t n, const int32_t* frame_id, const int32_t* cam_id,
@@ -298,6 +300,7 @@ extern "C" int vcgpu_set_imu(vcgpu_handle* h, int n, const double* t, const doub
   h->sigma_g = sigma_g;
   h->sigma_a = sigma_a;
   h->dirty = true;
+  h->wvec_cold = true;
   return VCGPU_OK;
 }
 extern "C" int vcgpu_set_imu_params(vcgpu_handle* h, const double g[2], const double b[6], const double sf[6], double ts) {
@@ -307,6 +310,7 @@ extern "C" int vcgpu_set_imu_params(vcgpu_handle* h, const double g[2], const do
   std::memcpy(h->h_sf, sf, sizeof h->h_sf);
   h->h_ts = ts;
   h->state_dirty = true;
+  h->wvec_cold = true;
   return VCGPU_OK;
 }
 extern "C" int vcgpu_set_flags(vcgpu_handle* h, const vcgpu_flags* f) {
@@ -314,6 +318,7 @@ extern "C" int vcgpu_set_flags(vcgpu_handle* h, const vcgpu_flags* f) {
   if ((f->inertial != 0) != (h->flags.inertial != 0)) h->dirty = true;
   h->flags = *f;
   h->blocks_valid = false;
+  h->wvec_cold = true;
   return VCGPU_OK;
 }
 extern "C" int vcgpu_set_options(vcgpu_handle* h, const vcgpu_options* o) {
@@ -693,6 +698,11 @@ static int prepare(vcgpu_handle* h) {
     CUDA_TRY(h, cudaMemcpyAsync(h->d_mask, mask.data(), mask.size() * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   }
   if (h->state_dirty) VC_TRY(upload_state(h));
+  // the next weights update starts its eigen-decompositions from the identity (NaN: no vectors)
+  if (h->wvec_cold && h->dp.inertial && h->d_wvec) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_wvec, 0xff, static_cast<size_t>(h->n_frames - 1) * 81 * sizeof(double), h->stream));
+    h->wvec_cold = false;
+  }
   return VCGPU_OK;
 }
 
@@ -1024,6 +1034,7 @@ extern "C" int vcgpu_get_imu_weights(vcgpu_handle* h, double* w) {
 }
 extern "C" int vcgpu_set_imu_weights(vcgpu_handle* h, const double* w) {
   if (!h || !w) return VCGPU_ERR_INVALID;
+  h->wvec_cold = true;
   VC_TRY(prepare(h));
   if (h->n_frames < 2 || !h->d_wsqrt) return VCGPU_OK;
   CUDA_TRY(h, cudaMemcpy(h->d_wsqrt, w, static_cast<size_t>(h->n_frames - 1) * 81 * sizeof(double), cudaMemcpyHostToDevice));
