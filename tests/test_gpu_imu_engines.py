@@ -3,7 +3,9 @@
 - The persistent kernels (chain_solve_kernel + eval_mega_kernel) against the multi-launch engine (vc_chain.cuh, selected
   with vcgpu_set_profiling bit 2) after a fixed number of iterations: the same accepted-step count, cost within 1e-10,
   state within 1e-8.  Shapes: G = 41; G = 67 with 256 frames (4 top nodes: N = 103 takes the 7-tile dense L D L^T); a
-  chain that needs a wide level 0 in two rounds and four elimination levels.
+  chain that needs a wide level 0 in two rounds and four elimination levels; two cameras that miss frames, and one
+  camera, with a frame no camera sees.
+- The normal equations of both engines' reprojection builds on those last two rigs, against the oracle.
 - The persistent engine's fit boundary: G = 67 runs persistent, G = 68 multi-launch; both against the oracle.
 - The largest rigs vcgpu_set_cameras accepts (G = 127 and 122), with 4 top nodes and with 1, on the multi-launch engine.
 - The deferred weights queue with more 16-interval tasks than CTAs leaving the solve, against the oracle, the
@@ -15,6 +17,7 @@
 
 Which frame counts reach which branch comes from the host model of the plan (chain_plan.py).
 """
+import dataclasses
 import os
 import subprocess
 import sys
@@ -51,15 +54,32 @@ def _calibrator(p, mode=0, **opts):
     return g
 
 
+UNSEEN_FRAME = 50
+
+
+def _missing_frames(p):
+    """test_gpu_persistent.test_cameras_missing_frames' observations: camera 1 misses every third frame, camera 0 every
+    seventh, and no camera sees frame UNSEEN_FRAME (on a one-camera rig, only that)"""
+    keep = p.obs_frame != UNSEEN_FRAME
+    if p.n_cams > 1:
+        keep &= ~((p.obs_cam == 1) & (p.obs_frame % 3 == 0)) & ~((p.obs_cam == 0) & (p.obs_frame % 7 == 2))
+    return dataclasses.replace(p, obs_frame=p.obs_frame[keep], obs_cam=p.obs_cam[keep], p_w=p.p_w[keep], p_c=p.p_c[keep],
+                               grid_idx=p.grid_idx[keep])
+
+
+MISSING_RIGS = [("poly3", "fov"), ("poly3",)]
 ENGINE_CASES = [
-    (("poly3", "poly3"), 200, (14, 10)),                                                     # G = 41
-    (("poly3",) * 4, chain_plan.TOP * chain_plan.CHUNK ** 2, (14, 10)),                      # G = 67, 4 top nodes
-    (("poly3",), chain_plan.CHUNK * SMS * chain_plan.GROUPS + 1, (4, 3)),                    # wide level 0, 2 rounds
+    (("poly3", "poly3"), 200, (14, 10), False),                                              # G = 41
+    (("poly3",) * 4, chain_plan.TOP * chain_plan.CHUNK ** 2, (14, 10), False),               # G = 67, 4 top nodes
+    (("poly3",), chain_plan.CHUNK * SMS * chain_plan.GROUPS + 1, (4, 3), False),             # wide level 0, 2 rounds
+    (MISSING_RIGS[0], 120, (14, 10), True),                                                  # cameras that miss frames
+    (MISSING_RIGS[1], 120, (14, 10), True),                                                  # one camera, a frame unseen
 ]
 
 
-@pytest.mark.parametrize("models,n_frames,grid", ENGINE_CASES, ids=["G41", "G67_top4", "wide0_rounds2"])
-def test_persistent_matches_multi_launch(models, n_frames, grid):
+@pytest.mark.parametrize("models,n_frames,grid,missing", ENGINE_CASES,
+                         ids=["G41", "G67_top4", "wide0_rounds2", "missing_frames", "unseen_frame"])
+def test_persistent_matches_multi_launch(models, n_frames, grid, missing):
     G = chain_plan.rig_globals(models)
     assert chain_plan.persistent_fits(G, n_frames, SMEM_OPTIN)
     if G == 67:
@@ -67,6 +87,8 @@ def test_persistent_matches_multi_launch(models, n_frames, grid):
     if grid == (4, 3):
         assert {"wide0_rounds2", "levels4"} <= chain_plan.branches(n_frames, SMS)
     p = synth.make_problem(models=models, n_frames=n_frames, grid=grid, inertial=True, seed=17)
+    if missing:
+        p = _missing_frames(p)
     iters = 6
     opts = dict(max_iters=iters, function_tol=0.0, gradient_tol=0.0, param_tol=0.0)
     g0, g1 = _calibrator(p, 0, **opts), _calibrator(p, MULTI_LAUNCH, **opts)
@@ -81,6 +103,30 @@ def test_persistent_matches_multi_launch(models, n_frames, grid):
     for k in STATE_KEYS:
         assert np.abs(st0[k] - st1[k]).max() <= 1e-8 * max(np.abs(st1[k]).max(), 1.0), k
     assert abs(st0["ts"] - st1["ts"]) <= 1e-8
+
+
+@pytest.mark.parametrize("mode", [0, MULTI_LAUNCH], ids=["eval_mega", "multi_launch"])
+@pytest.mark.parametrize("models", MISSING_RIGS, ids=["missing_frames", "unseen_frame"])
+def test_missing_frames_normal_equations(models, mode):
+    """The reprojection build of each inertial engine (eval_mega_kernel, fused_build_kernel<9>) on frames that a camera
+    misses or that no camera sees, against the oracle; the columns of E of a camera that misses a frame are exactly 0."""
+    from oracle.binding import Oracle
+
+    p = _missing_frames(synth.make_problem(models=models, n_frames=120, grid=(14, 10), inertial=True, seed=5))
+    o, g = Oracle(p, **ALL_ON), _calibrator(p, mode)
+    assert chain_plan.persistent_fits(g.G, p.n_frames, SMEM_OPTIN)
+    ne_o, ne_g = o.normal_equations(), g.normal_equations()
+    assert abs(ne_g["cost"] - ne_o["cost"]) <= 1e-11 * ne_o["cost"]
+    for k in ("B", "U", "E", "gf", "C", "gc"):
+        assert np.abs(ne_g[k] - ne_o[k]).max() <= 1e-10 * np.abs(ne_o[k]).max(), k
+    seen = np.zeros((p.n_cams, p.n_frames), dtype=bool)
+    seen[p.obs_cam, p.obs_frame] = True
+    assert not seen[:, UNSEEN_FRAME].any()
+    off = 0
+    for c, m in enumerate(p.models):
+        n = 6 + synth.NUM_INTR[int(m)]
+        assert not ne_g["E"][~seen[c], :, off:off + n].any(), c
+        off += n
 
 
 def _lm_against_oracle(models, n_frames, max_iters, function_tol, **opts):

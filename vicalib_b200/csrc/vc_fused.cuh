@@ -1,18 +1,22 @@
-// Fused evaluate + block-build kernel for the reprojection terms.
+// The reprojection half of the block normal equations: evaluate + Gram build, fused, for every engine.
 //
-// One CTA per frame.  For each camera that sees the frame, every thread evaluates one grid corner
-// (pose chain, camera model, analytic Jacobian, SoftLOne corrector) and parks two rows of the REDUCED
-// Jacobian  [d/dpose(6) | d/dintrinsics(K) | residual]  in a shared-memory tile, column-major over
-// corners; the CTA forms the 16 x 16 Gram matrix of those columns with FP64 tensor-core
+// Each corner (pose chain, camera model, analytic Jacobian, SoftLOne corrector) parks two rows of the
+// REDUCED Jacobian  [d/dpose(6) | d/dintrinsics(K) | residual]  in a shared-memory tile, column-major
+// over corners; the 16 x 16 Gram matrix of those columns is formed with FP64 tensor-core
 // mma.sync.m8n8k4 (DMMA), both operand fragments read straight from the tile.
 //
 // The six extrinsic (T_ck) columns never enter the tile: for one camera they are a constant linear map
 // of the pose columns,  J_ck = J_pose * A  with  A = [[0, -R_ck^T], [-I, 0]]  (right perturbation on both
 // sides, vc_math.cuh), so every block that involves them (E's extrinsic columns, the camera's global
-// block, its gradient) is A^T / A applied to the summed Gram blocks in the epilogue.  That halves the
-// DMMA work (3 instead of 6 8x8 blocks per k-step) and the tile.
+// block, its gradient) is A^T / A applied to the summed Gram matrix once per (frame, camera)
+// (expand_gram).  That halves the DMMA work (3 instead of 6 8x8 blocks per k-step) and the tile.
 //
-// The Jacobian never goes to HBM: the pass reads 44 B per corner and writes ~2 KB per (frame, camera).
+// Two layouts share the per-corner evaluation, the expansion and the frame-block store:
+//   build_frame_warp    one warp per frame, 32 corners per slab: the frame tasks of the persistent kernels
+//                       (lm_mega_kernel phase B, eval_mega_kernel phase T)
+//   fused_build_kernel  one CTA per frame, 144 corners per pass, a cross-warp reduction: the multi-launch engine
+//
+// The Jacobian never goes to HBM: a build reads 44 B per corner and writes ~2 KB per (frame, camera).
 // Replaces the residual+Jacobian evaluation and J^T J build Ceres does inside ceres::Solve
 // (vicalibrator.h:956) for the ImuReprojectionCostFunctor blocks (ceres-cost-functions.h:342-377).
 #pragma once
@@ -28,6 +32,10 @@ constexpr int kFusedLd = 2 * kFusedChunk + 4;        // tile leading dimension (
 constexpr int kFusedCols = 16;                       // 6 pose + K <= 8 intrinsics + residual, padded
 constexpr int kFusedRed = 3 * 64;                    // per-warp partial: blocks (0,0) (1,0) (1,1)
 static_assert(kFusedLd % 16 == 4, "fragment loads need ld == 4 (mod 16)");
+constexpr int kSlabLd = 64 + 4;                        // 32 corners x 2 residual rows (+4: conflict-free fragments)
+constexpr int kSlabDoubles = kFusedCols * kSlabLd;     // one warp's tile
+constexpr int kWarpDoubles = kSlabDoubles + 48;        // + frame block (36) + frame gradient (6), padded
+static_assert(kSlabLd % 16 == 4, "fragment loads need ld == 4 (mod 16)");
 
 struct FusedArgs {
   DevProblem dp;
@@ -42,7 +50,7 @@ struct FusedArgs {
   double* Cg;          // [n_groups][kCgStride]
   double* cost_part;   // [n_frames]
 };
-constexpr size_t kFusedSmemDoubles = static_cast<size_t>(kFusedCols) * kFusedLd + kFusedWarps * kFusedRed + 256 + 9 * 9 + 9 +
+constexpr size_t kFusedSmemDoubles = static_cast<size_t>(kFusedCols) * kFusedLd + kFusedWarps * kFusedRed + 256 + 36 + 6 +
                                      kFusedWarps + 9;
 
 __device__ __forceinline__ void dmma_m8n8k4(double& d0, double& d1, double a, double b) {
@@ -89,12 +97,184 @@ __device__ __forceinline__ double eval_obs_to_tile(const double* T, const double
   return 0.5 * rho0 * mult;
 }
 
+// eval_obs_to_tile for a camera model known at run time: the one device switch over the models
+template <int LD>
+__device__ __forceinline__ double eval_obs_any(int model, const double* T, const double* cam, const double* R, const double* mask, V3 pw,
+                                               double pcu, double pcv, double mult, double* tile, int k0, int k1) {
+  switch (model) {
+    case kLinear: return eval_obs_to_tile<kLinear, LD>(T, cam, R, mask, pw, pcu, pcv, mult, tile, k0, k1);
+    case kFov: return eval_obs_to_tile<kFov, LD>(T, cam, R, mask, pw, pcu, pcv, mult, tile, k0, k1);
+    case kPoly2: return eval_obs_to_tile<kPoly2, LD>(T, cam, R, mask, pw, pcu, pcv, mult, tile, k0, k1);
+    case kPoly3: return eval_obs_to_tile<kPoly3, LD>(T, cam, R, mask, pw, pcu, pcv, mult, tile, k0, k1);
+    default: return eval_obs_to_tile<kKb4, LD>(T, cam, R, mask, pw, pcu, pcv, mult, tile, k0, k1);
+  }
+}
+
 // x * A for a 6-vector x = (translation part, rotation part) of the pose columns: the matching
 // extrinsic column e (0..2 rotation w_ck, 3..5 translation p_ck)
 __device__ __forceinline__ double times_A(const double* x, int e, const double* R) {
   if (e < 3) return -x[3 + e];
   const double* r = R + 3 * (e - 3);
   return -(x[0] * r[0] + x[1] * r[1] + x[2] * r[2]);
+}
+
+// packed lower-triangle index of a camera block (at most 14 x 14: 105 entries) -> (row << 4 | col)
+__device__ __forceinline__ void fill_tri_lut(unsigned char* lut, int first, int step) {
+  for (int e = first; e < 105; e += step) {
+    int p = 0;
+    while ((p + 1) * (p + 2) / 2 <= e) ++p;
+    lut[e] = static_cast<unsigned char>((p << 4) | (e - p * (p + 1) / 2));
+  }
+}
+
+// Expands the 16 x 16 Gram matrix Gm of one (frame, camera) through A into:  Bp [6][6] += the pose block,
+// gp [6] += the pose gradient,  the camera's columns of E_f (Ec = E_f + the camera's goff, rows 0..5 of leading
+// dimension G),  and the camera's packed global block Cc (lower triangle over [w_ck p_ck intr], gradient at 105),
+// stored, or added to with kAccumulate.  Entries first, first + step, ...: a thread that passes the same (first,
+// step) for every frame owns the same entries of Cc.
+template <bool kAccumulate>
+__device__ __forceinline__ void expand_gram(const double* Gm, const double* R, const double* mask, int K, double* Bp, double* gp,
+                                            double* Ec, int G, double* Cc, const unsigned char* tri_lut, int first, int step) {
+  const int NG = 6 + K;
+  const double* Grf = Gm + (6 + K) * 16;  // residual row: [pose | intrinsics] parts of the gradient
+  const int nsym = NG * (NG + 1) / 2;
+  const int n_out = 36 + 6 + 6 * NG + nsym + NG;
+  for (int e = first; e < n_out; e += step) {
+    int o = e;
+    if (o < 36) { Bp[o] += Gm[(o / 6) * 16 + (o % 6)]; continue; }
+    o -= 36;
+    if (o < 6) { gp[o] += Grf[o]; continue; }
+    o -= 6;
+    if (o < 6 * NG) {  // E_f: row j (pose), column p of this camera's globals
+      const int j = o / NG, p = o - j * NG;
+      Ec[j * G + p] = p < 6 ? mask[p] * times_A(Gm + j * 16, p, R) : Gm[p * 16 + j];
+      continue;
+    }
+    o -= 6 * NG;
+    if (o < nsym) {
+      const int p = tri_lut[o] >> 4, q = tri_lut[o] & 15;
+      double v;
+      if (q >= 6) {
+        v = Gm[p * 16 + q];                                      // intrinsics x intrinsics
+      } else if (p >= 6) {
+        v = mask[q] * times_A(Gm + p * 16, q, R);                // intrinsics x extrinsics
+      } else {                                                   // extrinsics x extrinsics: (A^T Gff A)[p][q]
+        if (p < 3) {
+          v = -times_A(Gm + (3 + p) * 16, q, R);
+        } else {
+          const double* r = R + 3 * (p - 3);
+          v = -(r[0] * times_A(Gm, q, R) + r[1] * times_A(Gm + 16, q, R) + r[2] * times_A(Gm + 32, q, R));
+        }
+        v *= mask[p] * mask[q];
+      }
+      if (kAccumulate) Cc[o] += v;
+      else Cc[o] = v;
+      continue;
+    }
+    o -= nsym;  // gradient of the camera's globals
+    const double v = o < 6 ? mask[o] * times_A(Grf, o, R) : Grf[o];
+    if (kAccumulate) Cc[105 + o] += v;
+    else Cc[105 + o] = v;
+  }
+}
+
+// B_f [FD][FD] and g_f [FD] from the pose block Bp [6][6] and gradient gp [6]; velocity rows and columns zero
+template <int FD>
+__device__ __forceinline__ void store_frame_block(const double* Bp, const double* gp, double* Bf, double* gf, int first, int step) {
+  for (int q = first; q < FD * FD; q += step) {
+    const int i = q / FD, j = q - i * FD;
+    Bf[q] = (i < 6 && j < 6) ? Bp[i * 6 + j] : 0.0;
+  }
+  for (int q = first; q < FD; q += step) gf[q] = q < 6 ? gp[q] : 0.0;
+}
+
+// Reprojection blocks of one frame by one warp.  For every camera that sees the frame: its corners 32 at a time
+// through the warp's slab [16][kSlabLd] (the next slab's observation is loaded while this one goes through the DMMAs,
+// the accumulators stay in registers across slabs), then the three accumulator blocks mirrored into the 16 x 16 Gram
+// matrix (in the slab) and expanded by expand_gram.  cam_obs(c) -> (start, count) of camera c's observations in the
+// frame (count 0: the camera does not see it; prepare() never makes an empty group); cam_block(c) -> its packed
+// global block, asked for after the corners (no pointer held across the evaluation).  E_f (FD rows) is zeroed unless
+// the frame's only camera writes all G of its columns.  Leaves the pose block [36] and gradient [6] in the slab tail
+// (slab + kSlabDoubles) and returns cost plus the lane's share of the frame's cost.
+template <int FD, bool kAccumulate, class CamObs, class CamBlock>
+__device__ __forceinline__ double build_frame_warp(const DevProblem& dp, const double* T, const double* smCam, const double* smRc,
+                                                   const double* mask, const double* pw_all, const double* pc_all, double* Ef,
+                                                   double* slab, const unsigned char* tri_lut, int lane, double cost,
+                                                   CamObs cam_obs, CamBlock cam_block) {
+  const int G = dp.G, n_cams = dp.n_cams;
+  double* smB = slab + kSlabDoubles;  // [36] | [6]
+  double* smg = smB + 36;
+  const double* frag = slab + (lane >> 2) * kSlabLd + (lane & 3);
+  __syncwarp();
+  for (int q = lane; q < 42; q += 32) smB[q] = 0.0;
+  if (!(n_cams == 1 && G == 6 + dp.cams[0].K))
+    for (int q = lane; q < FD * G; q += 32) Ef[q] = 0.0;
+  for (int c = 0; c < n_cams; ++c) {
+    const int2 grp = cam_obs(c);
+    if (grp.y == 0) continue;
+    const CamInfo& ci = dp.cams[c];
+    const int K = ci.K, model = ci.model;
+    const int start = grp.x, cnt = grp.y;
+    const double* cam = smCam + kCamStateStride * c;
+    const double* Rc = smRc + 9 * c;
+    const double* cmask = mask + ci.goff;
+    double acc[3][2];
+#pragma unroll
+    for (int b = 0; b < 3; ++b) acc[b][0] = acc[b][1] = 0.0;
+    double nx[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+    if (lane < cnt) {
+      const int64_t i = start + lane;
+      nx[0] = pw_all[3 * i]; nx[1] = pw_all[3 * i + 1]; nx[2] = pw_all[3 * i + 2]; nx[3] = pc_all[2 * i]; nx[4] = pc_all[2 * i + 1];
+    }
+    for (int s0 = 0; s0 < cnt; s0 += 32) {
+      const int m = min(32, cnt - s0);
+      const int m4 = (m + 3) & ~3;
+      const V3 pw{nx[0], nx[1], nx[2]};
+      const double pcu = nx[3], pcv = nx[4];
+      if (s0 + 32 + lane < cnt) {
+        const int64_t i = start + s0 + 32 + lane;
+        nx[0] = pw_all[3 * i]; nx[1] = pw_all[3 * i + 1]; nx[2] = pw_all[3 * i + 2]; nx[3] = pc_all[2 * i]; nx[4] = pc_all[2 * i + 1];
+      }
+      __syncwarp();  // the previous slab's fragment loads are done
+      if (lane < m) {
+        cost += eval_obs_any<kSlabLd>(model, T, cam, Rc, cmask, pw, pcu, pcv, dp.visual_mult, slab, lane, 32 + lane);
+      } else if (lane < m4) {  // zero the padding rows of both halves
+#pragma unroll
+        for (int q = 0; q < kFusedCols; ++q) {
+          slab[q * kSlabLd + lane] = 0.0;
+          slab[q * kSlabLd + 32 + lane] = 0.0;
+        }
+      }
+      __syncwarp();
+      // SYRK over k: steps [0, m4/4) cover residual row 0, [m4/4, m4/2) residual row 1 (two accumulator sets
+      // for six independent DMMA chains measured no faster: the phase is not DMMA-latency bound)
+      const int ns = m4 >> 2;
+      for (int s = 0; s < 2 * ns; ++s) {
+        const int k0 = s < ns ? 4 * s : 32 + 4 * (s - ns);
+        const double a0 = frag[k0], a1 = frag[8 * kSlabLd + k0];
+        dmma_m8n8k4(acc[0][0], acc[0][1], a0, a0);  // (0,0)
+        dmma_m8n8k4(acc[1][0], acc[1][1], a1, a0);  // (1,0)
+        dmma_m8n8k4(acc[2][0], acc[2][1], a1, a1);  // (1,1)
+      }
+    }
+    // the three accumulator blocks -> symmetric 16 x 16 Gram matrix (in the slab)
+    __syncwarp();
+    {
+      const int rr = lane >> 2, cc = 2 * (lane & 3);
+      const double vm = dp.visual_mult;
+#pragma unroll
+      for (int b = 0; b < 3; ++b) {
+        const int i = (b == 0 ? 0 : 8) + rr, j = (b == 2 ? 8 : 0) + cc;
+        const double v0 = acc[b][0] * vm, v1 = acc[b][1] * vm;
+        // diagonal blocks: both triangles are computed (bitwise equal), keep j <= i and mirror
+        if (b == 1 || j <= i) { slab[i * 16 + j] = v0; slab[j * 16 + i] = v0; }
+        if (b == 1 || j + 1 <= i) { slab[i * 16 + j + 1] = v1; slab[(j + 1) * 16 + i] = v1; }
+      }
+    }
+    __syncwarp();
+    expand_gram<kAccumulate>(slab, Rc, cmask, K, smB, smg, Ef + ci.goff, G, cam_block(c), tri_lut, lane, 32);
+  }
+  return cost;
 }
 
 template <int FD>
@@ -107,13 +287,15 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_build_kernel(FusedArgs
   double* tile = smem;                                   // [16][kFusedLd]
   double* red = tile + kFusedCols * kFusedLd;            // [warps][3][64]
   double* Gm = red + kFusedWarps * kFusedRed;            // [16][16] Gram matrix of one (frame, camera)
-  double* smB = Gm + 256;                                // [FD*FD]
-  double* smg = smB + FD * FD;                           // [FD]
-  double* wcost = smg + FD;                              // [warps]
+  double* smB = Gm + 256;                                // [36] pose block
+  double* smg = smB + 36;                                // [6] pose gradient
+  double* wcost = smg + 6;                               // [warps]
   double* smR = wcost + kFusedWarps;                     // [9] R_ck of the current camera
+  __shared__ unsigned char tri_lut[128];
   const int f = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int G = a.dp.G, nf = a.dp.n_frames;
-  for (int k = tid; k < FD * FD + FD; k += kFusedThreads) smB[k] = 0.0;
+  fill_tri_lut(tri_lut, tid, kFusedThreads);
+  for (int k = tid; k < 42; k += kFusedThreads) smB[k] = 0.0;
   double* Ef = out.E + static_cast<int64_t>(f) * FD * G;
   for (int k = tid; k < FD * G; k += kFusedThreads) Ef[k] = 0.0;
   const double* T = state + 7 * static_cast<int64_t>(f);
@@ -123,8 +305,9 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_build_kernel(FusedArgs
     const int g = a.group_of[c * nf + f];
     if (g < 0) continue;
     const CamInfo& ci = a.dp.cams[c];
-    const int K = ci.K, NG = 6 + K;
     const int start = a.grp_start[g], cnt = a.grp_count[g];
+    double* Cgg = a.Cg + static_cast<int64_t>(g) * kCgStride;
+    double* Ec = Ef + ci.goff;
     const double* cam = camBase + kCamStateStride * c;
     const double* mask = a.mask + ci.goff;
     __syncthreads();  // the previous camera's epilogue is done with smR / Gm
@@ -146,13 +329,7 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_build_kernel(FusedArgs
         const int64_t i = start + ch + tid;
         const V3 pw{a.pw[3 * i], a.pw[3 * i + 1], a.pw[3 * i + 2]};
         const double pcu = a.pc[2 * i], pcv = a.pc[2 * i + 1];
-        switch (ci.model) {
-          case kLinear: cost += eval_obs_to_tile<kLinear>(T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid); break;
-          case kFov: cost += eval_obs_to_tile<kFov>(T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid); break;
-          case kPoly2: cost += eval_obs_to_tile<kPoly2>(T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid); break;
-          case kPoly3: cost += eval_obs_to_tile<kPoly3>(T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid); break;
-          default: cost += eval_obs_to_tile<kKb4>(T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid); break;
-        }
+        cost += eval_obs_any<kFusedLd>(ci.model, T, cam, smR, mask, pw, pcu, pcv, a.dp.visual_mult, tile, tid, kFusedChunk + tid);
       } else if (tid < m4) {  // zero the padding rows of both halves
 #pragma unroll
         for (int k = 0; k < kFusedCols; ++k) {
@@ -179,6 +356,7 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_build_kernel(FusedArgs
       for (int b = 0; b < 3; ++b) { rw[b * 64] = acc[b][0]; rw[b * 64 + 1] = acc[b][1]; }
     }
     __syncthreads();
+#pragma unroll 1  // unrolled, this loop's loads cost the kernel spills (ptxas -v)
     for (int e = tid; e < kFusedRed; e += kFusedThreads) {
       const int b = e >> 6, rr = (e >> 3) & 7, cc = e & 7;
       const int i = (b == 0 ? 0 : 8) + rr, j = (b == 2 ? 8 : 0) + cc;
@@ -191,61 +369,14 @@ __global__ void __launch_bounds__(kFusedThreads, 4) fused_build_kernel(FusedArgs
       Gm[j * 16 + i] = v;
     }
     __syncthreads();
-    // expand: frame block, frame gradient, E (extrinsic columns through A), the camera's global block
-    const double* Grf = Gm + (6 + K) * 16;  // residual row: [pose | intrinsics] parts of the gradient
-    double* Cgg = a.Cg + static_cast<int64_t>(g) * kCgStride;
-    const int nsym = NG * (NG + 1) / 2;
-    const int n_out = FD * FD + 6 + 6 * NG + nsym + NG;
-    for (int e = tid; e < n_out; e += kFusedThreads) {
-      int o = e;
-      if (o < FD * FD) {  // B_f (pose part of the frame block; velocity rows stay zero)
-        const int i = o / FD, j = o - i * FD;
-        if (i < 6 && j < 6) smB[o] += Gm[i * 16 + j];
-        continue;
-      }
-      o -= FD * FD;
-      if (o < 6) { smg[o] += Grf[o]; continue; }
-      o -= 6;
-      if (o < 6 * NG) {  // E_f: row j (pose), column p of this camera's globals
-        const int j = o / NG, p = o - j * NG;
-        Ef[j * G + ci.goff + p] = p < 6 ? mask[p] * times_A(Gm + j * 16, p, smR) : Gm[(p) * 16 + j];
-        continue;
-      }
-      o -= 6 * NG;
-      if (o < nsym) {  // global block, packed lower triangle over [w_ck p_ck intr]
-        int p = static_cast<int>((sqrt(8.0 * o + 1.0) - 1.0) * 0.5);
-        while ((p + 1) * (p + 2) / 2 <= o) ++p;
-        while (p * (p + 1) / 2 > o) --p;
-        const int q = o - p * (p + 1) / 2;
-        double v;
-        if (q >= 6) {
-          v = Gm[p * 16 + q];                                        // intrinsics x intrinsics
-        } else if (p >= 6) {
-          v = mask[q] * times_A(Gm + p * 16, q, smR);                // intrinsics x extrinsics
-        } else {                                                     // extrinsics x extrinsics: (A^T Gff A)[p][q]
-          if (p < 3) {
-            v = -times_A(Gm + (3 + p) * 16, q, smR);
-          } else {
-            const double* r = smR + 3 * (p - 3);
-            v = -(r[0] * times_A(Gm, q, smR) + r[1] * times_A(Gm + 16, q, smR) + r[2] * times_A(Gm + 32, q, smR));
-          }
-          v *= mask[p] * mask[q];
-        }
-        Cgg[o] = v;
-        continue;
-      }
-      o -= nsym;  // gradient of the camera's globals
-      Cgg[105 + o] = o < 6 ? mask[o] * times_A(Grf, o, smR) : Grf[o];
-    }
+    expand_gram<false>(Gm, smR, mask, ci.K, smB, smg, Ec, G, Cgg, tri_lut, tid, kFusedThreads);
   }
   // block cost
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) cost += __shfl_down_sync(0xffffffffu, cost, o);
   if (lane == 0) wcost[warp] = cost;
   __syncthreads();
-  double* Bf = out.B + static_cast<int64_t>(f) * FD * FD;
-  for (int k = tid; k < FD * FD; k += kFusedThreads) Bf[k] = smB[k];
-  for (int k = tid; k < FD; k += kFusedThreads) out.gf[static_cast<int64_t>(f) * FD + k] = smg[k];
+  store_frame_block<FD>(smB, smg, out.B + static_cast<int64_t>(f) * FD * FD, out.gf + static_cast<int64_t>(f) * FD, tid, kFusedThreads);
   if (tid == 0) {
     double s = 0.0;
     for (int w = 0; w < kFusedWarps; ++w) s += wcost[w];

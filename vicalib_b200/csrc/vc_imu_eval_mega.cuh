@@ -2,9 +2,8 @@
 // threads per SM), grid barriers where the multi-launch engine has launch boundaries:
 //
 //   T  warp tasks from one queue (longest first): IMU residual + 9x33 Jacobian of an interval (lane per tangent
-//      direction, vc_imu.cuh) | reprojection evaluate + Gram build of a frame (32 corners per slab through the
-//      warp's shared-memory slab and FP64 DMMA, vc_mega.cuh's phase B): frame block, E, gradient, per-(frame,
-//      camera) packed global block
+//      direction, vc_imu.cuh) | reprojection evaluate + Gram build of a frame (build_frame_warp, vc_fused.cuh, as
+//      lm_mega_kernel's phase B): frame block, E, gradient, per-(frame, camera) packed global block
 //   -- grid barrier
 //   A  per frame (one warp): J^T J of the two intervals touching the frame into B, U, E, gradient, and
 //      the interval's packed 15x15 IMU global block
@@ -76,143 +75,23 @@ __host__ __device__ inline size_t eval_mega_smem_doubles(int G) {
   return m + kMaxCams * (kCamStateStride + 9) + 16;
 }
 
-template <int MODEL>
-__device__ __forceinline__ double evm_eval(const double* T, const double* cam, const double* Rc, const double* mask, V3 pw, double pcu,
-                                           double pcv, double mult, double* slab, int lane) {
-  return eval_obs_to_tile<MODEL, kSlabLd>(T, cam, Rc, mask, pw, pcu, pcv, mult, slab, lane, 32 + lane);
-}
-
-// reprojection evaluate + Gram build of frame f by one warp (vc_mega.cuh phase B, with 9 x 9 frame blocks and the
-// packed camera blocks written per (frame, camera) group instead of accumulated per warp)
+// reprojection blocks of frame f by one warp (build_frame_warp): the packed camera blocks are stored per (frame,
+// camera) group, the frame's cost goes to cost_part[f]
 __device__ inline void evm_build_frame(const EvalMegaArgs& a, const Blocks& bt, const double* x, int f, double* slab, const double* smCam,
                                        const double* smRc, const unsigned char* tri_lut, int lane) {
   constexpr int FD = 9;
-  const int G = a.dp.G, nf = a.dp.n_frames, n_cams = a.dp.n_cams;
-  double* smB = slab + kSlabDoubles;  // [36] | [6]
-  double* smg = smB + 36;
-  const double* frag = slab + (lane >> 2) * kSlabLd + (lane & 3);
-  const double* T = x + 7 * static_cast<int64_t>(f);
+  const int G = a.dp.G, nf = a.dp.n_frames;
+  double cost = build_frame_warp<FD, false>(
+      a.dp, x + 7 * static_cast<int64_t>(f), smCam, smRc, a.mask, a.pw, a.pc, bt.E + static_cast<int64_t>(f) * FD * G, slab, tri_lut,
+      lane, 0.0,
+      [&](int c) {
+        const int g = a.group_of[c * nf + f];
+        return g < 0 ? make_int2(0, 0) : make_int2(a.grp_start[g], a.grp_count[g]);
+      },
+      [&](int c) { return a.Cg + static_cast<int64_t>(a.group_of[c * nf + f]) * kCgStride; });
   __syncwarp();
-  for (int q = lane; q < 42; q += 32) smB[q] = 0.0;
-  double* Ef = bt.E + static_cast<int64_t>(f) * FD * G;
-  for (int q = lane; q < FD * G; q += 32) Ef[q] = 0.0;
-  double cost = 0.0;
-  for (int c = 0; c < n_cams; ++c) {
-    const int g = a.group_of[c * nf + f];
-    if (g < 0) continue;
-    const CamInfo& ci = a.dp.cams[c];
-    const int K = ci.K, NG = 6 + K, model = ci.model;
-    const int start = a.grp_start[g], cnt = a.grp_count[g];
-    const double* cam = smCam + kCamStateStride * c;
-    const double* Rc = smRc + 9 * c;
-    const double* mask = a.mask + ci.goff;
-    double acc[3][2];
-#pragma unroll
-    for (int b = 0; b < 3; ++b) acc[b][0] = acc[b][1] = 0.0;
-    // software pipeline: the next slab's observation is loaded while this slab goes through the DMMAs
-    double nx[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-    if (lane < cnt) {
-      const int64_t i = start + lane;
-      nx[0] = a.pw[3 * i]; nx[1] = a.pw[3 * i + 1]; nx[2] = a.pw[3 * i + 2]; nx[3] = a.pc[2 * i]; nx[4] = a.pc[2 * i + 1];
-    }
-    for (int s0 = 0; s0 < cnt; s0 += 32) {
-      const int m = min(32, cnt - s0);
-      const int m4 = (m + 3) & ~3;
-      const V3 pw{nx[0], nx[1], nx[2]};
-      const double pcu = nx[3], pcv = nx[4];
-      if (s0 + 32 + lane < cnt) {
-        const int64_t i = start + s0 + 32 + lane;
-        nx[0] = a.pw[3 * i]; nx[1] = a.pw[3 * i + 1]; nx[2] = a.pw[3 * i + 2]; nx[3] = a.pc[2 * i]; nx[4] = a.pc[2 * i + 1];
-      }
-      __syncwarp();  // the previous slab's fragment loads are done
-      if (lane < m) {
-        switch (model) {
-          case kLinear: cost += evm_eval<kLinear>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-          case kFov: cost += evm_eval<kFov>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-          case kPoly2: cost += evm_eval<kPoly2>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-          case kPoly3: cost += evm_eval<kPoly3>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-          default: cost += evm_eval<kKb4>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-        }
-      } else if (lane < m4) {  // zero the padding rows of both halves
-#pragma unroll
-        for (int q = 0; q < kFusedCols; ++q) {
-          slab[q * kSlabLd + lane] = 0.0;
-          slab[q * kSlabLd + 32 + lane] = 0.0;
-        }
-      }
-      __syncwarp();
-      // SYRK over k: steps [0, m4/4) cover residual row 0, [m4/4, m4/2) residual row 1
-      const int ns = m4 >> 2;
-      for (int s = 0; s < 2 * ns; ++s) {
-        const int k0 = s < ns ? 4 * s : 32 + 4 * (s - ns);
-        const double a0 = frag[k0], a1 = frag[8 * kSlabLd + k0];
-        dmma_m8n8k4(acc[0][0], acc[0][1], a0, a0);  // (0,0)
-        dmma_m8n8k4(acc[1][0], acc[1][1], a1, a0);  // (1,0)
-        dmma_m8n8k4(acc[2][0], acc[2][1], a1, a1);  // (1,1)
-      }
-    }
-    // the three accumulator blocks -> symmetric 16 x 16 Gram matrix (in the slab)
-    __syncwarp();
-    double* Gm = slab;
-    {
-      const int rr = lane >> 2, cc = 2 * (lane & 3);
-      const double vm = a.dp.visual_mult;
-#pragma unroll
-      for (int b = 0; b < 3; ++b) {
-        const int i = (b == 0 ? 0 : 8) + rr, j = (b == 2 ? 8 : 0) + cc;
-        const double v0 = acc[b][0] * vm, v1 = acc[b][1] * vm;
-        if (b == 1 || j <= i) { Gm[i * 16 + j] = v0; Gm[j * 16 + i] = v0; }
-        if (b == 1 || j + 1 <= i) { Gm[i * 16 + j + 1] = v1; Gm[(j + 1) * 16 + i] = v1; }
-      }
-    }
-    __syncwarp();
-    // expand: frame block, frame gradient, E (extrinsic columns through A), the camera's packed global block
-    const double* Grf = Gm + (6 + K) * 16;
-    const int nsym = NG * (NG + 1) / 2;
-    const int n_out = 36 + 6 + 6 * NG + nsym + NG;
-    double* Cc = a.Cg + static_cast<int64_t>(g) * kCgStride;
-    for (int e = lane; e < n_out; e += 32) {
-      int o = e;
-      if (o < 36) { smB[o] += Gm[(o / 6) * 16 + (o % 6)]; continue; }
-      o -= 36;
-      if (o < 6) { smg[o] += Grf[o]; continue; }
-      o -= 6;
-      if (o < 6 * NG) {
-        const int j = o / NG, p = o - j * NG;
-        Ef[j * G + ci.goff + p] = p < 6 ? mask[p] * times_A(Gm + j * 16, p, Rc) : Gm[p * 16 + j];
-        continue;
-      }
-      o -= 6 * NG;
-      if (o < nsym) {
-        const int p = tri_lut[o] >> 4, q = tri_lut[o] & 15;
-        double v;
-        if (q >= 6) {
-          v = Gm[p * 16 + q];                                        // intrinsics x intrinsics
-        } else if (p >= 6) {
-          v = mask[q] * times_A(Gm + p * 16, q, Rc);                // intrinsics x extrinsics
-        } else {                                                     // extrinsics x extrinsics: (A^T Gff A)[p][q]
-          if (p < 3) {
-            v = -times_A(Gm + (3 + p) * 16, q, Rc);
-          } else {
-            const double* r = Rc + 3 * (p - 3);
-            v = -(r[0] * times_A(Gm, q, Rc) + r[1] * times_A(Gm + 16, q, Rc) + r[2] * times_A(Gm + 32, q, Rc));
-          }
-          v *= mask[p] * mask[q];
-        }
-        Cc[o] = v;
-        continue;
-      }
-      o -= nsym;
-      Cc[105 + o] = o < 6 ? mask[o] * times_A(Grf, o, Rc) : Grf[o];
-    }
-  }
-  __syncwarp();
-  double* Bf = bt.B + static_cast<int64_t>(f) * FD * FD;
-  for (int q = lane; q < FD * FD; q += 32) {
-    const int i = q / FD, j = q - i * FD;
-    Bf[q] = (i < 6 && j < 6) ? smB[i * 6 + j] : 0.0;
-  }
-  if (lane < FD) bt.gf[static_cast<int64_t>(f) * FD + lane] = lane < 6 ? smg[lane] : 0.0;
+  store_frame_block<FD>(slab + kSlabDoubles, slab + kSlabDoubles + 36, bt.B + static_cast<int64_t>(f) * FD * FD,
+                        bt.gf + static_cast<int64_t>(f) * FD, lane, 32);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) cost += __shfl_xor_sync(0xffffffffu, cost, o);
   if (lane == 0) a.cost_part[f] = cost;
@@ -260,11 +139,7 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
   const size_t head = eval_mega_smem_doubles(G) - (kMaxCams * (kCamStateStride + 9) + 16);
   double* smCam = smem + head;
   double* smRc = smCam + kMaxCams * kCamStateStride;
-  for (int e = tid; e < 105; e += kEvThreads) {
-    int p = 0;
-    while ((p + 1) * (p + 2) / 2 <= e) ++p;
-    tri_lut[e] = static_cast<unsigned char>((p << 4) | (e - p * (p + 1) / 2));
-  }
+  fill_tri_lut(tri_lut, tid, kEvThreads);
   if (tid < n_cams) {
     const double* xc = x + a.dp.off_cam + kCamStateStride * tid;
     double R[9];

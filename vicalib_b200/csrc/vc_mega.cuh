@@ -11,9 +11,9 @@
 //      one GPU: plain totals + grid barrier; shards: tagged words into every rank's buffer, readers poll
 //   G  every CTA, redundantly: reduced system C + D - sum E^T X, Cholesky, globals' step
 //   U  per frame (warp):  back-substitution, x (+) step, step statistics; trial camera states
-//   B  per frame (warp): fused evaluate + Gram build at the trial point, 32 corners at a time through the
-//      warp's own shared-memory slab and FP64 DMMA (accumulators stay in registers across slabs; no block
-//      barrier anywhere in the phase); the camera blocks are accumulated per warp, packed per camera
+//   B  per frame (warp): fused evaluate + Gram build at the trial point (build_frame_warp, vc_fused.cuh), 32
+//      corners at a time through the warp's own shared-memory slab and FP64 DMMA (no block barrier anywhere in
+//      the phase); the camera blocks are accumulated per warp, packed per camera
 //   -- grid barrier
 //   R2 packed camera blocks / scalars added up and published, as R1
 //   D  every CTA, redundantly: expands the packed blocks, takes the accept-reject decision of Ceres'
@@ -34,9 +34,6 @@ namespace cg = cooperative_groups;
 
 constexpr int kMegaMaxWarps = 16;
 constexpr int kMegaMaxThreads = 32 * kMegaMaxWarps;
-constexpr int kSlabLd = 64 + 4;                        // 32 corners x 2 residual rows (+4: conflict-free fragments)
-constexpr int kSlabDoubles = kFusedCols * kSlabLd;     // one warp's tile
-constexpr int kWarpDoubles = kSlabDoubles + 48;        // + frame block (36) + frame gradient (6), padded
 constexpr int kGtabMax = 256;
 constexpr int kMegaPartExtra = 8;  // scalars appended to each CTA's partial slot
 // Totals buffer: every rank owns one (32 MiB, the vision kernel uses the first 4); in a frame-sharded run (one process per GPU) all ranks of the
@@ -54,7 +51,6 @@ constexpr int kXchgCtlOff = 442368;
 constexpr int kXchgPlainS = kXchgCtlOff + 64;
 constexpr int kXchgPlainC = kXchgPlainS + 32768;
 constexpr int kMegaCommFailed = 1000;  // Ctl::done value when a peer never showed up
-static_assert(kSlabLd % 16 == 4, "fragment loads need ld == 4 (mod 16)");
 enum { kPCost = 0, kPGf2, kPDotG, kPDotD, kPStep2, kPXnorm2, kPGfMax, kPNotPD };
 enum { kProfS = 0, kProfG, kProfU, kProfB, kProfD, kProfSync, kProfCount };
 
@@ -229,12 +225,6 @@ __device__ inline void mega_chol_solve_smem(double* S, int G, int lane, double* 
   }
 }
 
-template <int MODEL>
-__device__ __forceinline__ double mega_eval(const double* T, const double* cam, const double* Rc, const double* mask, V3 pw, double pcu,
-                                            double pcv, double mult, double* slab, int lane) {
-  return eval_obs_to_tile<MODEL, kSlabLd>(T, cam, Rc, mask, pw, pcu, pcv, mult, slab, lane, 32 + lane);
-}
-
 __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a) {
   extern __shared__ double smem[];
   cg::grid_group grid = cg::this_grid();
@@ -274,11 +264,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       const int g = a.group_of[c * nf + bid + k * nb];
       gtab[e] = g < 0 ? make_int2(0, 0) : make_int2(a.grp_start[g], a.grp_count[g]);
     }
-  for (int e = tid; e < 105; e += nthreads) {
-    int p = 0;
-    while ((p + 1) * (p + 2) / 2 <= e) ++p;
-    tri_lut[e] = static_cast<unsigned char>((p << 4) | (e - p * (p + 1) / 2));
-  }
+  fill_tri_lut(tri_lut, tid, nthreads);
   __syncthreads();
   if (ctl->done) return;
   if (bid == 0 && tid == 0 && !(ctlw[2] & 2ull)) {  // the stop bit of the previous launch; the abort bit is sticky
@@ -573,141 +559,19 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
     double cost = 0.0, gf2 = 0.0, gfmax = 0.0;
     {
       double* slab = wmem + static_cast<size_t>(warp) * kWarpDoubles;  // [16][kSlabLd]; reused as the 16 x 16 Gram matrix
-      double* smB = slab + kSlabDoubles;                               // [36] | [6]
-      double* smg = smB + 36;
+      const double* smg = slab + kSlabDoubles + 36;
       double* Cmine = Cw + static_cast<size_t>(warp) * NP;
-      const double* frag = slab + (lane >> 2) * kSlabLd + (lane & 3);
       for (int k = warp; k < nk; k += nwarps) {
         const int f = bid + k * nb;
-        const double* T = x_new + 7 * static_cast<int64_t>(f);
+        // the camera blocks are added up per warp: the same lane owns an entry for every frame of this warp
+        cost = build_frame_warp<FD, true>(a.dp, x_new + 7 * static_cast<int64_t>(f), smCam, smRc, a.mask, a.pw, a.pc,
+                                          bt.E + static_cast<int64_t>(f) * FD * G, slab, tri_lut, lane, cost,
+                                          [&](int c) { return lookup(k, c); }, [&](int c) { return Cmine + c * kCgStride; });
         __syncwarp();
-        for (int q = lane; q < 42; q += 32) smB[q] = 0.0;
-        double* Ef = bt.E + static_cast<int64_t>(f) * FD * G;
-        bool zero_E = n_cams > 1;  // one camera: the expansion below writes every column
-        for (int c = 0; c < n_cams; ++c) {
-          const int2 grp = lookup(k, c);
-          if (grp.y == 0) continue;
-          if (zero_E) {
-            for (int q = lane; q < FD * G; q += 32) Ef[q] = 0.0;
-            zero_E = false;
-          }
-          const CamInfo& ci = a.dp.cams[c];
-          const int K = ci.K, NG = 6 + K, model = ci.model;
-          const int start = grp.x, cnt = grp.y;
-          const double* cam = smCam + kCamStateStride * c;
-          const double* Rc = smRc + 9 * c;
-          const double* mask = a.mask + ci.goff;
-          double acc[3][2];
-#pragma unroll
-          for (int b = 0; b < 3; ++b) acc[b][0] = acc[b][1] = 0.0;
-          // software pipeline: the next slab's observation is loaded while this slab goes through the DMMAs
-          double nx[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
-          if (lane < cnt) {
-            const int64_t i = start + lane;
-            nx[0] = a.pw[3 * i]; nx[1] = a.pw[3 * i + 1]; nx[2] = a.pw[3 * i + 2]; nx[3] = a.pc[2 * i]; nx[4] = a.pc[2 * i + 1];
-          }
-          for (int s0 = 0; s0 < cnt; s0 += 32) {
-            const int m = min(32, cnt - s0);
-            const int m4 = (m + 3) & ~3;
-            const V3 pw{nx[0], nx[1], nx[2]};
-            const double pcu = nx[3], pcv = nx[4];
-            if (s0 + 32 + lane < cnt) {
-              const int64_t i = start + s0 + 32 + lane;
-              nx[0] = a.pw[3 * i]; nx[1] = a.pw[3 * i + 1]; nx[2] = a.pw[3 * i + 2]; nx[3] = a.pc[2 * i]; nx[4] = a.pc[2 * i + 1];
-            }
-            __syncwarp();  // the previous slab's fragment loads are done
-            if (lane < m) {
-              switch (model) {
-                case kLinear: cost += mega_eval<kLinear>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-                case kFov: cost += mega_eval<kFov>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-                case kPoly2: cost += mega_eval<kPoly2>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-                case kPoly3: cost += mega_eval<kPoly3>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-                default: cost += mega_eval<kKb4>(T, cam, Rc, mask, pw, pcu, pcv, a.dp.visual_mult, slab, lane); break;
-              }
-            } else if (lane < m4) {  // zero the padding rows of both halves
-#pragma unroll
-              for (int q = 0; q < kFusedCols; ++q) {
-                slab[q * kSlabLd + lane] = 0.0;
-                slab[q * kSlabLd + 32 + lane] = 0.0;
-              }
-            }
-            __syncwarp();
-            // SYRK over k: steps [0, m4/4) cover residual row 0, [m4/4, m4/2) residual row 1
-            // SYRK over k: steps [0, m4/4) cover residual row 0, [m4/4, m4/2) residual row 1 (two accumulator sets
-            // for six independent DMMA chains measured no faster: the phase is not DMMA-latency bound)
-            const int ns = m4 >> 2;
-            for (int s = 0; s < 2 * ns; ++s) {
-              const int k0 = s < ns ? 4 * s : 32 + 4 * (s - ns);
-              const double a0 = frag[k0], a1 = frag[8 * kSlabLd + k0];
-              dmma_m8n8k4(acc[0][0], acc[0][1], a0, a0);  // (0,0)
-              dmma_m8n8k4(acc[1][0], acc[1][1], a1, a0);  // (1,0)
-              dmma_m8n8k4(acc[2][0], acc[2][1], a1, a1);  // (1,1)
-            }
-          }
-          // the three accumulator blocks -> symmetric 16 x 16 Gram matrix (in the slab)
-          __syncwarp();
-          double* Gm = slab;
-          {
-            const int rr = lane >> 2, cc = 2 * (lane & 3);
-            const double vm = a.dp.visual_mult;
-#pragma unroll
-            for (int b = 0; b < 3; ++b) {
-              const int i = (b == 0 ? 0 : 8) + rr, j = (b == 2 ? 8 : 0) + cc;
-              const double v0 = acc[b][0] * vm, v1 = acc[b][1] * vm;
-              // diagonal blocks: both triangles are computed (bitwise equal), keep j <= i and mirror
-              if (b == 1 || j <= i) { Gm[i * 16 + j] = v0; Gm[j * 16 + i] = v0; }
-              if (b == 1 || j + 1 <= i) { Gm[i * 16 + j + 1] = v1; Gm[(j + 1) * 16 + i] = v1; }
-            }
-          }
-          __syncwarp();
-          // expand: frame block, frame gradient, E (extrinsic columns through A), the camera's packed global block
-          const double* Grf = Gm + (6 + K) * 16;
-          const int nsym = NG * (NG + 1) / 2;
-          const int n_out = 36 + 6 + 6 * NG + nsym + NG;
-          double* Cc = Cmine + c * kCgStride;
-          for (int e = lane; e < n_out; e += 32) {
-            int o = e;
-            if (o < 36) { smB[o] += Gm[(o / 6) * 16 + (o % 6)]; continue; }
-            o -= 36;
-            if (o < 6) { smg[o] += Grf[o]; continue; }
-            o -= 6;
-            if (o < 6 * NG) {
-              const int j = o / NG, p = o - j * NG;
-              Ef[j * G + ci.goff + p] = p < 6 ? mask[p] * times_A(Gm + j * 16, p, Rc) : Gm[p * 16 + j];
-              continue;
-            }
-            o -= 6 * NG;
-            if (o < nsym) {
-              const int p = tri_lut[o] >> 4, q = tri_lut[o] & 15;
-              double v;
-              if (q >= 6) {
-                v = Gm[p * 16 + q];                                        // intrinsics x intrinsics
-              } else if (p >= 6) {
-                v = mask[q] * times_A(Gm + p * 16, q, Rc);                // intrinsics x extrinsics
-              } else {                                                     // extrinsics x extrinsics: (A^T Gff A)[p][q]
-                if (p < 3) {
-                  v = -times_A(Gm + (3 + p) * 16, q, Rc);
-                } else {
-                  const double* r = Rc + 3 * (p - 3);
-                  v = -(r[0] * times_A(Gm, q, Rc) + r[1] * times_A(Gm + 16, q, Rc) + r[2] * times_A(Gm + 32, q, Rc));
-                }
-                v *= mask[p] * mask[q];
-              }
-              Cc[o] += v;  // the same lane owns the entry for every frame of this warp
-              continue;
-            }
-            o -= nsym;
-            Cc[105 + o] += o < 6 ? mask[o] * times_A(Grf, o, Rc) : Grf[o];
-          }
-        }
-        if (zero_E)  // no camera saw the frame
-          for (int q = lane; q < FD * G; q += 32) Ef[q] = 0.0;
-        __syncwarp();
-        double* Bf = bt.B + static_cast<int64_t>(f) * FD * FD;
-        for (int q = lane; q < 36; q += 32) Bf[q] = smB[q];
+        store_frame_block<FD>(slab + kSlabDoubles, smg, bt.B + static_cast<int64_t>(f) * FD * FD, bt.gf + static_cast<int64_t>(f) * FD,
+                              lane, 32);
         if (lane < 6) {
           const double gv = smg[lane];
-          bt.gf[static_cast<int64_t>(f) * FD + lane] = gv;
           gf2 += gv * gv;
           gfmax = fmax(gfmax, fabs(gv));
         }
