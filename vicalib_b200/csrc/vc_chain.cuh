@@ -11,6 +11,7 @@
 // separator at every level), which is why it is preferred to a sequential sweep.
 #pragma once
 #include "vc_internal.h"
+#include "vc_kernels.cuh"
 
 namespace vc {
 
@@ -33,22 +34,14 @@ __global__ void chain_init_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl
   const Blocks& b = ctl->cur ? b1 : b0;
   const double rinv = 1.0 / ctl->radius;
   const int G = dp.G, f = blockIdx.x, tid = threadIdx.x;
-  // sharded chain: a rank's first frame (and its ghost copy on the previous rank) is damped once, by its
-  // owner, from the diagonal summed over both ranks; sepdiag[slot*FD + r]
-  const bool sep = sepdiag != nullptr && (f == 0 || (dp.ghost && f == dp.n_frames - 1));
   const bool is_ghost = dp.ghost && f == dp.n_frames - 1;
-  const double* sd = sep ? sepdiag + (dp.rank + (is_ghost ? 1 : 0)) * FD : nullptr;
   const double* sf = scale + static_cast<int64_t>(f) * FD;
   const double* sc = scale + static_cast<int64_t>(dp.n_frames) * FD;
   for (int e = tid; e < FD * FD; e += blockDim.x) {
     const int r = e / FD, c = e - r * FD;
     const double bij = b.B[static_cast<int64_t>(f) * FD * FD + e];
     double v = bij * sf[r] * sf[c];
-    if (r == c) {
-      if (D2x) v += D2x[static_cast<int64_t>(f) * FD + r];
-      else if (!sep) v += lm_damp(bij, sf[r], rinv);
-      else if (!is_ghost) v += lm_damp(sd[r], sf[r], rinv);
-    }
+    if (r == c) v = frame_damp<FD>(v, f, r, bij, sf[r], rinv, D2x, sepdiag, dp.rank, is_ghost);
     L.A[static_cast<int64_t>(f) * FD * FD + e] = v;
     double u = 0.0;
     if (f > 0) u = b.U[static_cast<int64_t>(f) * FD * FD + e] * scale[static_cast<int64_t>(f - 1) * FD + r] * sf[c];
@@ -291,7 +284,7 @@ __global__ void __launch_bounds__(kChainThreads, 4) chain_eliminate_kernel(ElimA
   }
   if (tid == 0) {
     a.next.orig[j] = L.orig[s];
-    if (bad) a.scalars[7] = 1.0;  // kScNotPD
+    if (bad) a.scalars[kScNotPD] = 1.0;
   }
   double* out = a.Spart + static_cast<int64_t>(j) * NS;
   for (int e = tid; e < NS; e += kChainThreads) out[e] = Sacc[e];
@@ -400,7 +393,7 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
         double v = -a.Ssum[e];
         if (a.add_globals) {
           v += b.C[e] * sc[r] * sc[c];
-          if (r == c) v += a.D2x ? a.D2x[nfp + r] : lm_damp(b.C[e], sc[r], rinv);
+          if (r == c) v += global_damp(r, b.C[e], sc[r], rinv, a.D2x, nfp);
         }
         S[r * N + c] = v;
       } else {
@@ -466,7 +459,7 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
       for (int k = lane; k < i; k += 32) rhs[k] -= S[i * N + k] * xi;
       __syncwarp();
     }
-    if (bad && lane == 0) a.scalars[7] = 1.0;
+    if (bad && lane == 0) a.scalars[kScNotPD] = 1.0;
   }
   __syncthreads();
   for (int i = tid; i < G; i += 256) a.delta[nfp + i] = bad ? 0.0 : rhs[i];

@@ -254,52 +254,7 @@ __global__ void dl_combine_kernel(Ctl* ctl, DlVecs v, double* delta, int64_t n) 
 
 // ---------------------------------------------------------------- accept / reject, radius and mu (Ceres TrustRegionMinimizer + DoglegStrategy)
 __global__ void dl_decide_kernel(Ctl* c, double* sc) {
-  if (threadIdx.x != 0 || blockIdx.x != 0 || c->done) return;
-  const int iter = ++c->iter;
-  const double cand = sc[kScCost];
-  const double model_change = c->dl_model_change;
-  const bool invalid = !c->dl_ok || !(model_change > 0.0) || !isfinite(cand);
-  sc[kScNotPD] = 0.0;
-  c->last_accepted = 0;
-  c->last_cand_cost = cand;
-  c->last_rho = 0.0;
-  c->last_cost_change = 0.0;
-  c->last_step_norm = 0.0;
-  if (invalid) {  // DoglegStrategy::StepIsInvalid: more regularisation for the next Gauss-Newton solve
-    c->dl_mu *= 10.0;
-  } else {
-    const double step_norm = sqrt(sc[kScStep2]);
-    const double cost_change = c->cost - cand;
-    c->last_step_norm = step_norm;
-    c->last_cost_change = cost_change;
-    if (!c->fixed && step_norm <= c->param_tol * (c->x_norm + c->param_tol)) { c->done = 1 + VCGPU_TERM_PARAM_TOL; return; }
-    if (!c->fixed && fabs(cost_change) <= c->function_tol * c->cost) { c->done = 1 + VCGPU_TERM_FUNCTION_TOL; return; }
-    const double rho = cost_change / model_change;
-    c->last_rho = rho;
-    if (rho > 1e-3) {
-      c->cur = 1 - c->cur;
-      c->cost = cand;
-      c->gmax = sc[kScGmax];
-      c->gnorm = sqrt(sc[kScGnorm2]);
-      c->x_norm = sqrt(sc[kScXnorm2]);
-      ++c->successful;
-      if (rho < 0.25) c->radius *= 0.5;                                   // DoglegStrategy::StepAccepted
-      if (rho > 0.75) c->radius = fmax(c->radius, 3.0 * c->dl_step_norm);
-      c->dl_mu = fmax(1e-8, 2.0 * c->dl_mu / 10.0);
-      c->last_accepted = 1;
-      if (!c->fixed) {
-        if (c->gmax <= c->gradient_tol) c->done = 1 + VCGPU_TERM_GRADIENT_TOL;
-        else if (c->gnorm > 0.0 && c->gnorm < 1e-9) c->done = 1 + VCGPU_TERM_CALLBACK;  // vicalibrator.h:713-717
-      }
-    } else {
-      c->radius *= 0.5;  // DoglegStrategy::StepRejected
-    }
-  }
-  if (c->radius < 1e-32) {
-    if (c->fixed) c->radius = 1e4;
-    else if (!c->done) c->done = 1 + VCGPU_TERM_RADIUS;
-  }
-  if (!c->done && iter >= c->max_iters) c->done = 1 + VCGPU_TERM_NO_CONVERGENCE;
+  if (threadIdx.x == 0 && blockIdx.x == 0) decide_step<Strategy::kDogleg>(c, sc, 1);
 }
 
 }  // namespace vc

@@ -196,53 +196,30 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
   mark(kEvProfReduce);
   grid.sync();
   // ------------------------------------------------------------ D: scalars + decision (CTA 0)
-  // entries of a rank's slot in the exchange: C | gc (NS), 7 scalars (+ 1 pad), own first frame diag 9 | gradient 9,
+  // entries of a rank's slot in the exchange: C | gc (NS), scalars kScCost .. kScGmax (+ 1 pad), own first frame diag 9 | gradient 9,
   // ghost diag 9 | gradient 9
   constexpr int kSepFd = 9;
   const int eSc = NS, eSep = NS + 8;
   if (bid == 0) {
-    double w[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    double w[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     for (int b = tid; b < nb; b += kEvThreads) {
-      for (int q = 0; q < 6; ++q) w[q] += __ldcg(a.red_part + 8 * b + q);
-      w[6] = fmax(w[6], __ldcg(a.red_part + 8 * b + 6));
+      for (int q = 0; q < kScGmax; ++q) w[q] += __ldcg(a.red_part + 8 * b + q);
+      w[kScGmax] = fmax(w[kScGmax], __ldcg(a.red_part + 8 * b + kScGmax));
     }
     if (!sharded) {
       for (int k = tid; k < G; k += kEvThreads) {
         const double v = __ldcg(bt.gc + k);
-        w[1] += v * v;
-        w[6] = fmax(w[6], fabs(v));
+        w[kScGnorm2] += v * v;
+        w[kScGmax] = fmax(w[kScGmax], fabs(v));
       }
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-      for (int q = 0; q < 6; ++q) w[q] += __shfl_down_sync(0xffffffffu, w[q], o);
-      w[6] = fmax(w[6], __shfl_down_sync(0xffffffffu, w[6], o));
-    }
-    __syncthreads();
-    if (lane == 0)
-      for (int q = 0; q < 7; ++q) shr[warp][q] = w[q];
-    __syncthreads();
+    double t[kScNotPD];
+    cta_sum_scalars(w, shr, t);
     if (tid == 0) {
-      double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-      for (int ww = 0; ww < kEvWarps; ++ww) {
-        for (int q = 0; q < 6; ++q) t[q] += shr[ww][q];
-        t[6] = fmax(t[6], shr[ww][6]);
-      }
       if (sharded) {  // this rank's share; the totals are formed below
-        for (int q = 0; q < 7; ++q) xchg_put(a.x, xbufs, eSc + q, t[q]);
+        for (int q = 0; q < kScNotPD; ++q) xchg_put(a.x, xbufs, eSc + q, t[q]);
       } else {
-        *bt.cost = t[0];
-        a.scalars[kScCost] = t[0];
-        a.scalars[kScGmax] = t[6];
-        a.scalars[kScGnorm2] = t[1];
-        if (a.step_part) {
-          a.scalars[kScDotG] = t[2];
-          a.scalars[kScDotD] = t[3];
-          a.scalars[kScStep2] = t[4];
-          a.scalars[kScXnorm2] = t[5];
-        }
-        if (a.decide_mode >= 0) decide_step(a.ctl, a.scalars, a.decide_mode);
+        finish_scalars(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
         *a.counter = 0u;  // the task queue of the next launch
         __threadfence();
       }
@@ -277,7 +254,7 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
     grid.sync();
     if (bid == 0) {
       double* tot = &shr[0][0];  // [ranks][8] the ranks' scalars
-      if (tid < a.x.nranks * 7) tot[(tid / 7) * 8 + tid % 7] = xchg_get(a.x, xbufs, tid / 7, eSc + tid % 7);
+      if (tid < a.x.nranks * kScNotPD) tot[(tid / kScNotPD) * 8 + tid % kScNotPD] = xchg_get(a.x, xbufs, tid / kScNotPD, eSc + tid % kScNotPD);
       double gm = 0.0, g2 = 0.0;
       for (int k = tid; k < G; k += kEvThreads) {
         const double v = __ldcg(bt.gc + k);
@@ -298,26 +275,16 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
       if (lane == 0) { gsh[warp][0] = g2; gsh[warp][1] = gm; }
       __syncthreads();
       if (tid == 0) {
-        double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        double t[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
         for (int r = 0; r < a.x.nranks; ++r) {
-          for (int q = 0; q < 6; ++q) t[q] += tot[r * 8 + q];
-          t[6] = fmax(t[6], tot[r * 8 + 6]);
+          for (int q = 0; q < kScGmax; ++q) t[q] += tot[r * 8 + q];
+          t[kScGmax] = fmax(t[kScGmax], tot[r * 8 + kScGmax]);
         }
         for (int ww = 0; ww < kEvWarps; ++ww) {
-          t[1] += gsh[ww][0];
-          t[6] = fmax(t[6], gsh[ww][1]);
+          t[kScGnorm2] += gsh[ww][0];
+          t[kScGmax] = fmax(t[kScGmax], gsh[ww][1]);
         }
-        *bt.cost = t[0];
-        a.scalars[kScCost] = t[0];
-        a.scalars[kScGmax] = t[6];
-        a.scalars[kScGnorm2] = t[1];
-        if (a.step_part) {
-          a.scalars[kScDotG] = t[2];
-          a.scalars[kScDotD] = t[3];
-          a.scalars[kScStep2] = t[4];
-          a.scalars[kScXnorm2] = t[5];
-        }
-        if (a.decide_mode >= 0) decide_step(a.ctl, a.scalars, a.decide_mode);
+        finish_scalars(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
         *a.counter = 0u;
         __threadfence();
       }

@@ -145,6 +145,7 @@ __device__ __forceinline__ double src_A(const NodeSrc& s, int64_t p, int e) {
   const double* sf = s.scale + p * FD;
   const double bij = s.b.B[p * FD * FD + e];
   double v = bij * sf[r] * sf[c];
+  // frame_damp's rule, written out: through frame_damp the compiler fuses this add differently and the solve's bits change
   if (r == c) {
     const bool is_ghost = s.ghost && p == s.nf - 1;
     if (is_ghost) ;  // damped once, by the rank that owns the frame
@@ -283,6 +284,7 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
       double* d = nd == 0 ? Al + el : Ap + (e - FD * FD);
       const double a = *d, sr = *scl((nd + 1) * FD + r), sq = *scl((nd + 1) * FD + q);
       double v = a * sr * sq;
+      // frame_damp's rule, written out as in src_A (a chunk's nodes s .. s + m stop short of the ghost)
       if (r == q) {
         if (src.D2x) v += src.D2x[static_cast<int64_t>(s + nd) * FD + r];
         else if (src.sepdiag && s + nd == 0) v += lm_damp(src.sepdiag[src.rank * FD + r], sr, src.rinv);
@@ -563,55 +565,6 @@ template <int FD>
 __device__ __forceinline__ void chain_backsub_level(const ChainLevel cur, int l, double* delta, int64_t nfp, int G, int gw, int nw, int lane) {
   const int n_slots = chain_backsub_slots(cur);
   for (int t = gw; t < n_slots; t += nw) chain_backsub_node<FD>(cur, l, delta, nfp, G, t, lane);
-}
-
-// x (+) step of one frame into the trial state, and the frame's share of the step statistics
-// (acc: step.g, step.D2.step, |x_new - x|^2, |x_new|^2)
-__device__ __forceinline__ void chain_update_frame(const ChainSolveArgs& a, const Blocks& b, double rinv, int f, const double* d,
-                                                   double acc[4]) {
-  constexpr int FD = 9;
-  const int cur = a.ctl->cur;
-  const double* x_cur = a.state[cur];
-  double* x_new = a.state[1 - cur];
-  double du[FD];
-  // sharded: a rank's first frame is damped from the diagonal summed over both owners; its ghost copy on the previous
-  // rank moves with the same step but is counted (damping term, norms) by the owner only
-  const bool is_ghost = a.dp.ghost && f == a.dp.n_frames - 1;
-#pragma unroll
-  for (int r = 0; r < FD; ++r) {
-    const int64_t k = static_cast<int64_t>(f) * FD + r;
-    const double sc = a.scale[k];
-    double d2;
-    if (is_ghost) d2 = 0.0;
-    else if (a.D2x) d2 = a.D2x[k];
-    else if (a.sepdiag && f == 0) d2 = lm_damp(a.sepdiag[a.dp.rank * FD + r], sc, rinv);
-    else d2 = lm_damp(b.B[k * FD + r], sc, rinv);
-    acc[0] += d[r] * b.gf[k] * sc;
-    acc[1] += d[r] * d[r] * d2;
-    du[r] = d[r] * sc;
-  }
-  const double* x = x_cur + 7 * static_cast<int64_t>(f);
-  double xo[7];
-  se3_plus(x, du, xo);
-#pragma unroll
-  for (int k = 0; k < 7; ++k) {
-    x_new[7 * static_cast<int64_t>(f) + k] = xo[k];
-    if (!is_ghost) {
-      acc[2] += (xo[k] - x[k]) * (xo[k] - x[k]);
-      acc[3] += xo[k] * xo[k];
-    }
-  }
-  const double* v = x_cur + a.dp.off_v + 3 * static_cast<int64_t>(f);
-  double* vo = x_new + a.dp.off_v + 3 * static_cast<int64_t>(f);
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    const double nv = v[k] + du[6 + k];
-    vo[k] = nv;
-    if (!is_ghost) {
-      acc[2] += (nv - v[k]) * (nv - v[k]);
-      acc[3] += nv * nv;
-    }
-  }
 }
 
 // The deferred UpdateImuWeights as a function of its own (its own register allocation: inlined into the solve kernel
@@ -918,7 +871,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
           if (a.x.rank == 0) {  // the globals' own block joins once
             const int r = e / G, c = e - r * G;
             v += b.C[e] * sc[r] * sc[c];
-            if (r == c) v += a.D2x ? a.D2x[nfp + r] : lm_damp(b.C[e], sc[r], rinv);
+            if (r == c) v += global_damp(r, b.C[e], sc[r], rinv, a.D2x, nfp);
           }
         } else {
           v = p - (a.x.rank == 0 ? b.gc[e - G * G] * sc[e - G * G] : 0.0);
@@ -1018,7 +971,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
         if (e < G * G) {
           const int r = e / G, c = e - r * G;
           double v = cv[u] * sc[r] * sc[c] - p[u];
-          if (r == c) v += a.D2x ? a.D2x[nfp + r] : lm_damp(cv[u], sc[r], rinv);
+          if (r == c) v += global_damp(r, cv[u], sc[r], rinv, a.D2x, nfp);
           S[r * LD + c] = v;
         } else {
           const int r = e - G * G;
@@ -1110,13 +1063,14 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
       if (a.do_update && tid < nt) {  // the top nodes' frames
         double d[FD];
         for (int r = 0; r < FD; ++r) d[r] = bd ? 0.0 : rhs[G + (slot0 + tid) * FD + r];
-        chain_update_frame(a, b, rinv, a.n_levels > 1 ? top.orig[tid] : tid, d, acc);
+        frame_plus<FD>(a.dp, b, a.scale, rinv, a.D2x, a.sepdiag, a.n_levels > 1 ? top.orig[tid] : tid, d, true, a.state[a.ctl->cur],
+                       a.state[1 - a.ctl->cur], acc);
       }
       // globals: cameras + IMU parameters (one thread; the step.g / step.D2.step sums over the globals by its warp)
       double gs0 = 0.0, gs1 = 0.0;
       if (a.do_update && warp == kCsThreads / 32 - 1) {
         for (int k = lane; k < G; k += 32) {
-          const double d2 = a.D2x ? a.D2x[nfp + k] : lm_damp(b.C[k * G + k], sc[k], rinv);
+          const double d2 = global_damp(k, b.C[k * G + k], sc[k], rinv, a.D2x, nfp);
           const double dk = bd ? 0.0 : rhs[k];
           gs0 += dk * b.gc[k] * sc[k];
           gs1 += dk * dk * d2;
@@ -1131,14 +1085,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
         const double* x_cur = a.state[a.ctl->cur];
         double* x_new = a.state[1 - a.ctl->cur];
         double g4[4] = {gs0, gs1, 0.0, 0.0};
-        const double* dg = bd ? nullptr : rhs;
-        for (int c = 0; c < a.dp.n_cams; ++c) {
-          const double* x = x_cur + a.dp.off_cam + kCamStateStride * c;
-          double* xo = x_new + a.dp.off_cam + kCamStateStride * c;
-          cam_plus(a.dp, c, x, dg, sc, xo);
-          cam_stats(a.dp, c, x, xo, g4 + 2);
-        }
-        imu_plus(a.dp, x_cur + a.dp.off_imu, dg, sc, x_new + a.dp.off_imu, g4 + 2);
+        globals_plus(a.dp, x_cur, x_new, bd ? nullptr : rhs, sc, g4 + 2);
         for (int q = 0; q < 4; ++q) a.step_part[4 * static_cast<int64_t>(nb) + q] = g4[q];
       }
     }
@@ -1227,7 +1174,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
         double d[FD];
 #pragma unroll
         for (int r = 0; r < FD; ++r) d[r] = __ldcg(a.delta + static_cast<int64_t>(f) * FD + r);
-        chain_update_frame(a, b, rinv, f, d, acc);
+        frame_plus<FD>(a.dp, b, a.scale, rinv, a.D2x, a.sepdiag, f, d, true, a.state[a.ctl->cur], a.state[1 - a.ctl->cur], acc);
       }
     }
     // ---------------------------------------------------------- step statistics of this CTA

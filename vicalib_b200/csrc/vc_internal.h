@@ -54,7 +54,7 @@ struct Blocks {  // block normal equations (device pointers)
 
 // Trust-region state kept ON THE DEVICE so iterations can be enqueued back to back with no host
 // round trip: the accept/reject decision (Ceres TrustRegionMinimizer + LevenbergMarquardtStrategy,
-// SURVEY App. A.3) is taken by decide_kernel and every kernel selects its buffers through `cur`.
+// SURVEY App. A.3) is taken by decide_step (vc_kernels.cuh) and every kernel selects its buffers through `cur`.
 struct Ctl {
   int cur;           // which double buffer holds the accepted point
   int done;          // 0 = running, else 1 + VCGPU_TERM_*

@@ -20,18 +20,38 @@ namespace vc {
 
 __device__ __forceinline__ int pick(const Ctl* c, int which) { return which ? 1 - c->cur : c->cur; }
 
-// scalars produced by the evaluation / step kernels for decide_step (indices into d_scalars)
+// scalars of a trust-region step, in one order for the per-CTA partials, the multi-GPU all-reduce buffer, the persistent
+// kernels' exchange slots and d_scalars (decide_step reads them there).  The entries before kScGmax are sums, kScGmax
+// and kScNotPD are maxima.
 enum {
   kScCost = 0,      // robust cost of the evaluated point
-  kScGmax = 1,      // gradient max norm
-  kScGnorm2 = 2,    // gradient squared 2-norm
-  kScDotG = 3,      // step . g        (scaled space)
-  kScDotD = 4,      // step . D2 step  (scaled space)
-  kScStep2 = 5,     // |x_trial - x|^2 (ambient)
-  kScXnorm2 = 6,    // |x_trial|^2 (ambient)
+  kScGnorm2 = 1,    // gradient squared 2-norm
+  kScDotG = 2,      // step . g        (scaled space)
+  kScDotD = 3,      // step . D2 step  (scaled space)
+  kScStep2 = 4,     // |x_trial - x|^2 (ambient)
+  kScXnorm2 = 5,    // |x_trial|^2 (ambient)
+  kScGmax = 6,      // gradient max norm
   kScNotPD = 7,     // >0 if a Cholesky pivot failed
   kScCount = 16
 };
+
+// v plus the damping D^2 of diagonal entry r of frame f of the Jacobi-scaled system (diag: the frame's B_rr): the
+// explicit D2x if one is given, else the LM rule on B_rr or, for a sharded run's first frame, on the diagonal summed over
+// the two ranks that hold a piece of it (sepdiag).  The ghost (the next rank's first frame) is damped once, by its owner,
+// never here (DESIGN §6).  v = 0 gives the damping itself.  (The add stays inside each case: the compiler fuses it with
+// lm_damp's multiply there, which the solves' bits depend on.)
+template <int FD>
+__device__ __forceinline__ double frame_damp(double v, int f, int r, double diag, double scale, double rinv, const double* D2x,
+                                             const double* sepdiag, int rank, bool is_ghost) {
+  if (is_ghost) return v;
+  if (D2x) return v + D2x[static_cast<int64_t>(f) * FD + r];
+  if (sepdiag && f == 0) return v + lm_damp(sepdiag[rank * FD + r], scale, rinv);
+  return v + lm_damp(diag, scale, rinv);
+}
+// ... and to diagonal entry k of the globals (Ckk: C_kk; nfp: frame entries before the globals in D2x)
+__device__ __forceinline__ double global_damp(int k, double Ckk, double scale, double rinv, const double* D2x, int64_t nfp) {
+  return D2x ? D2x[nfp + k] : lm_damp(Ckk, scale, rinv);
+}
 
 // ---------------------------------------------------------------- reprojection evaluate (two-pass path + hooks)
 struct EvalArgs {
@@ -219,9 +239,14 @@ __global__ void __launch_bounds__(kBuildThreads) build_frames_kernel(BuildArgs a
 }
 
 // ---------------------------------------------------------------- accept / reject on the device
+enum class Strategy { kLM, kDogleg };  // Ceres' LevenbergMarquardtStrategy, DoglegStrategy (vc_dogleg.cuh)
+
 // mode 0: initial point (iteration 0): adopt cost / gradient norms
-// mode 1: one iteration of Ceres' TrustRegionMinimizer loop with the LM strategy's radius rules
+// mode 1: one iteration of Ceres' TrustRegionMinimizer loop.  The strategy decides what an invalid step does, the
+// radius after an accepted or rejected step, where the model change comes from and the reset at the radius floor.
+template <Strategy S>
 __device__ inline void decide_step(Ctl* c, double* sc, int mode) {
+  constexpr bool kDl = S == Strategy::kDogleg;
   if (c->done) return;
   if (mode == 0) {
     c->cost = sc[kScCost];
@@ -235,18 +260,23 @@ __device__ inline void decide_step(Ctl* c, double* sc, int mode) {
   }
   const int iter = ++c->iter;
   const double cand = sc[kScCost];
-  // model_cost_change = -step.g - step.H.step/2, with (H + D2) step = -g
-  const double model_change = -0.5 * sc[kScDotG] + 0.5 * sc[kScDotD];
-  const bool invalid = sc[kScNotPD] > 0.0 || !(model_change > 0.0) || !isfinite(cand);
+  // model_cost_change = -step.g - step.H.step/2; LM: with (H + D2) step = -g; dogleg: from dl_dots_kernel
+  const double model_change = kDl ? c->dl_model_change : -0.5 * sc[kScDotG] + 0.5 * sc[kScDotD];
+  const bool solved = kDl ? c->dl_ok != 0 : !(sc[kScNotPD] > 0.0);
+  const bool invalid = !solved || !(model_change > 0.0) || !isfinite(cand);
   sc[kScNotPD] = 0.0;
   c->last_accepted = 0;
   c->last_cand_cost = cand;
   c->last_rho = 0.0;
   c->last_cost_change = 0.0;
   c->last_step_norm = 0.0;
-  if (invalid) {  // StepIsInvalid == StepRejected for the LM strategy
-    c->radius /= c->decrease_factor;
-    c->decrease_factor *= 2.0;
+  if (invalid) {
+    if (kDl) {  // DoglegStrategy::StepIsInvalid: more regularisation for the next Gauss-Newton solve
+      c->dl_mu *= 10.0;
+    } else {    // StepIsInvalid == StepRejected for the LM strategy
+      c->radius /= c->decrease_factor;
+      c->decrease_factor *= 2.0;
+    }
   } else {
     const double step_norm = sqrt(sc[kScStep2]);
     const double cost_change = c->cost - cand;
@@ -269,24 +299,71 @@ __device__ inline void decide_step(Ctl* c, double* sc, int mode) {
       c->gnorm = sqrt(sc[kScGnorm2]);
       c->x_norm = sqrt(sc[kScXnorm2]);
       ++c->successful;
-      const double t = 2.0 * rho - 1.0;
-      c->radius = fmin(1e16, c->radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
-      c->decrease_factor = 2.0;
+      if (kDl) {  // DoglegStrategy::StepAccepted
+        if (rho < 0.25) c->radius *= 0.5;
+        if (rho > 0.75) c->radius = fmax(c->radius, 3.0 * c->dl_step_norm);
+        c->dl_mu = fmax(1e-8, 2.0 * c->dl_mu / 10.0);
+      } else {
+        const double t = 2.0 * rho - 1.0;
+        c->radius = fmin(1e16, c->radius / fmax(1.0 / 3.0, 1.0 - t * t * t));
+        c->decrease_factor = 2.0;
+      }
       c->last_accepted = 1;
       if (!c->fixed) {
         if (c->gmax <= c->gradient_tol) c->done = 1 + VCGPU_TERM_GRADIENT_TOL;
         else if (c->gnorm > 0.0 && c->gnorm < 1e-9) c->done = 1 + VCGPU_TERM_CALLBACK;  // vicalibrator.h:713-717
       }
+    } else if (kDl) {  // DoglegStrategy::StepRejected
+      c->radius *= 0.5;
     } else {
       c->radius /= c->decrease_factor;
       c->decrease_factor *= 2.0;
     }
   }
   if (c->radius < 1e-32) {
-    if (c->fixed) { c->radius = 1e4; c->decrease_factor = 2.0; }
-    else if (!c->done) c->done = 1 + VCGPU_TERM_RADIUS;
+    if (c->fixed) {
+      c->radius = 1e4;
+      if (!kDl) c->decrease_factor = 2.0;
+    } else if (!c->done) {
+      c->done = 1 + VCGPU_TERM_RADIUS;
+    }
   }
   if (!c->done && iter >= c->max_iters) c->done = 1 + VCGPU_TERM_NO_CONVERGENCE;
+}
+
+// v[kScCost .. kScGmax] of every thread summed (kScGmax: maximised) over the CTA in a fixed order: a shuffle-down tree
+// per warp, one slot per warp (shr), then thread 0 adds the warps up in order into t.  Every thread of the CTA calls it.
+__device__ inline void cta_sum_scalars(double v[kScNotPD], double (*shr)[8], double t[kScNotPD]) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+    for (int q = 0; q < kScGmax; ++q) v[q] += __shfl_down_sync(0xffffffffu, v[q], o);
+    v[kScGmax] = fmax(v[kScGmax], __shfl_down_sync(0xffffffffu, v[kScGmax], o));
+  }
+  __syncthreads();  // shr is free
+  if (lane == 0)
+    for (int q = 0; q < kScNotPD; ++q) shr[warp][q] = v[q];
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int q = 0; q < kScNotPD; ++q) t[q] = 0.0;
+    for (int w = 0; w < static_cast<int>(blockDim.x >> 5); ++w) {
+      for (int q = 0; q < kScGmax; ++q) t[q] += shr[w][q];
+      t[kScGmax] = fmax(t[kScGmax], shr[w][kScGmax]);
+    }
+  }
+}
+
+// the evaluated point's totals t[kScCost .. kScXnorm2, kScGmax] -> its cost (unless null) and the scalars sc (the step
+// entries only when the point is a trial step), then the decision (decide_mode: -1 none, else decide_step's mode)
+__device__ inline void finish_scalars(Ctl* ctl, double* sc, double* cost, const double* t, bool with_step, int decide_mode) {
+  if (cost) *cost = t[kScCost];
+  sc[kScCost] = t[kScCost];
+  sc[kScGnorm2] = t[kScGnorm2];
+  sc[kScGmax] = t[kScGmax];
+  if (with_step)
+    for (int q = kScDotG; q <= kScXnorm2; ++q) sc[q] = t[q];
+  if (decide_mode >= 0) decide_step<Strategy::kLM>(ctl, sc, decide_mode);
 }
 
 // ---------------------------------------------------------------- reduce + finalize + decide in one launch
@@ -322,7 +399,7 @@ struct RedFinArgs {
 // -> Cpart[bid], of the cost / gradient-norm / step partials -> red_part[bid].  acc: NS doubles of shared memory.
 __device__ __forceinline__ void reduce_level1(const RedFinArgs& a, const DevProblem& dp, const Blocks& out, double* acc, double (*shr)[8],
                                               int bid, int nb) {
-  const int G = dp.G, tid = threadIdx.x, NS = G * G + G, lane = tid & 31, warp = tid >> 5;
+  const int G = dp.G, tid = threadIdx.x, NS = G * G + G;
   for (int k = tid; k < NS; k += 256) acc[k] = 0.0;
   __syncthreads();
   for (int c = 0; c < dp.n_cams; ++c) {
@@ -384,42 +461,29 @@ __device__ __forceinline__ void reduce_level1(const RedFinArgs& a, const DevProb
   double* cp = a.Cpart + static_cast<int64_t>(bid) * NS;
   for (int k = tid; k < NS; k += 256) cp[k] = acc[k];
   // slice reductions: cost, |gf|^2, step sums (4), |gf|_inf
-  double v[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  double v[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   {
     const int lo = static_cast<int>(static_cast<int64_t>(a.n_cost_part) * bid / nb), hi = static_cast<int>(static_cast<int64_t>(a.n_cost_part) * (bid + 1) / nb);
-    for (int k = lo + tid; k < hi; k += 256) v[0] += a.cost_part[k];
+    for (int k = lo + tid; k < hi; k += 256) v[kScCost] += a.cost_part[k];
     const int li = static_cast<int>(static_cast<int64_t>(a.n_imu_cost_part) * bid / nb), hi2 = static_cast<int>(static_cast<int64_t>(a.n_imu_cost_part) * (bid + 1) / nb);
-    for (int k = li + tid; k < hi2; k += 256) v[0] += a.imu_cost_part[k];
+    for (int k = li + tid; k < hi2; k += 256) v[kScCost] += a.imu_cost_part[k];
     const int64_t lg = static_cast<int64_t>(a.n_frames_fd) * bid / nb, hg = static_cast<int64_t>(a.n_frames_fd) * (bid + 1) / nb;
     for (int64_t k = lg + tid; k < hg; k += 256) {
       if (k < a.gf_skip_below || k >= a.gf_skip_from) continue;
       const double g = out.gf[k];
-      v[6] = fmax(v[6], fabs(g));
-      v[1] += g * g;
+      v[kScGmax] = fmax(v[kScGmax], fabs(g));
+      v[kScGnorm2] += g * g;
     }
-    if (a.step_part) {
+    if (a.step_part) {  // step_part rows: step.g, step.D2.step, |x_new - x|^2, |x_new|^2 (kScDotG ..)
       const int ls = static_cast<int>(static_cast<int64_t>(a.n_step_part) * bid / nb), hs = static_cast<int>(static_cast<int64_t>(a.n_step_part) * (bid + 1) / nb);
       for (int k = ls + tid; k < hs; k += 256)
-        for (int q = 0; q < 4; ++q) v[2 + q] += a.step_part[4 * k + q];
+        for (int q = 0; q < 4; ++q) v[kScDotG + q] += a.step_part[4 * k + q];
     }
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-    for (int q = 0; q < 6; ++q) v[q] += __shfl_down_sync(0xffffffffu, v[q], o);
-    v[6] = fmax(v[6], __shfl_down_sync(0xffffffffu, v[6], o));
-  }
-  if (lane == 0)
-    for (int q = 0; q < 7; ++q) shr[warp][q] = v[q];
-  __syncthreads();
-  if (tid == 0) {
-    double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    for (int w = 0; w < 8; ++w) {
-      for (int q = 0; q < 6; ++q) t[q] += shr[w][q];
-      t[6] = fmax(t[6], shr[w][6]);
-    }
-    for (int q = 0; q < 7; ++q) a.red_part[8 * bid + q] = t[q];
-  }
+  double t[kScNotPD];
+  cta_sum_scalars(v, shr, t);
+  if (tid == 0)
+    for (int q = 0; q < kScNotPD; ++q) a.red_part[8 * bid + q] = t[q];
 }
 
 __global__ void __launch_bounds__(256) reduce_finalize_kernel(RedFinArgs a) {
@@ -429,7 +493,7 @@ __global__ void __launch_bounds__(256) reduce_finalize_kernel(RedFinArgs a) {
   __shared__ int is_last;
   if (a.ctl->done) return;
   const Blocks& out = a.out[pick(a.ctl, a.which)];
-  const int G = a.dp.G, tid = threadIdx.x, NS = G * G + G, lane = tid & 31, warp = tid >> 5;
+  const int G = a.dp.G, tid = threadIdx.x, NS = G * G + G;
   const int nb = gridDim.x, bid = blockIdx.x;
   reduce_level1(a, a.dp, out, acc, shr, bid, nb);
   if (tid == 0) {
@@ -472,40 +536,16 @@ __global__ void __launch_bounds__(256) reduce_finalize_kernel(RedFinArgs a) {
     }
     __syncthreads();
   }
-  double w[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  double w[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   if (tid < nb)
-    for (int q = 0; q < 7; ++q) w[q] = __ldcg(a.red_part + 8 * tid + q);
+    for (int q = 0; q < kScNotPD; ++q) w[q] = __ldcg(a.red_part + 8 * tid + q);
   if (!a.multi) {
-    w[1] += g2;
-    w[6] = fmax(w[6], gm);
+    w[kScGnorm2] += g2;
+    w[kScGmax] = fmax(w[kScGmax], gm);
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-    for (int q = 0; q < 6; ++q) w[q] += __shfl_down_sync(0xffffffffu, w[q], o);
-    w[6] = fmax(w[6], __shfl_down_sync(0xffffffffu, w[6], o));
-  }
-  if (lane == 0)
-    for (int q = 0; q < 7; ++q) shr[warp][q] = w[q];
-  __syncthreads();
-  if (tid == 0) {
-    double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    for (int ww = 0; ww < 8; ++ww) {
-      for (int q = 0; q < 6; ++q) t[q] += shr[ww][q];
-      t[6] = fmax(t[6], shr[ww][6]);
-    }
-    *out.cost = t[0];
-    a.scalars[kScCost] = t[0];
-    a.scalars[kScGmax] = t[6];
-    a.scalars[kScGnorm2] = t[1];
-    if (a.step_part) {
-      a.scalars[kScDotG] = t[2];
-      a.scalars[kScDotD] = t[3];
-      a.scalars[kScStep2] = t[4];
-      a.scalars[kScXnorm2] = t[5];
-    }
-    if (a.decide_mode >= 0) decide_step(a.ctl, a.scalars, a.decide_mode);
-  }
+  double t[kScNotPD];
+  cta_sum_scalars(w, shr, t);
+  if (tid == 0) finish_scalars(a.ctl, a.scalars, out.cost, t, a.step_part != nullptr, a.decide_mode);
 }
 
 // level 2 for large global blocks: C | gc were summed by sum_partials_sel_kernel; this one-CTA launch
@@ -514,47 +554,23 @@ __global__ void __launch_bounds__(256) finalize_small_kernel(RedFinArgs a, int n
   __shared__ double shr[8][8];
   if (a.ctl->done) return;
   const Blocks& out = a.out[pick(a.ctl, a.which)];
-  const int G = a.dp.G, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  double w[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  const int G = a.dp.G, tid = threadIdx.x;
+  double w[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
   if (tid < nb)
-    for (int q = 0; q < 7; ++q) w[q] = a.red_part[8 * tid + q];
+    for (int q = 0; q < kScNotPD; ++q) w[q] = a.red_part[8 * tid + q];
   if (!a.multi)
     for (int k = tid; k < G; k += 256) {
       const double v = out.gc[k];
-      w[1] += v * v;
-      w[6] = fmax(w[6], fabs(v));
+      w[kScGnorm2] += v * v;
+      w[kScGmax] = fmax(w[kScGmax], fabs(v));
     }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-    for (int q = 0; q < 6; ++q) w[q] += __shfl_down_sync(0xffffffffu, w[q], o);
-    w[6] = fmax(w[6], __shfl_down_sync(0xffffffffu, w[6], o));
-  }
-  if (lane == 0)
-    for (int q = 0; q < 7; ++q) shr[warp][q] = w[q];
-  __syncthreads();
-  if (tid == 0) {
-    double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
-    for (int ww = 0; ww < 8; ++ww) {
-      for (int q = 0; q < 6; ++q) t[q] += shr[ww][q];
-      t[6] = fmax(t[6], shr[ww][6]);
-    }
-    *out.cost = t[0];
-    a.scalars[kScCost] = t[0];
-    a.scalars[kScGmax] = t[6];
-    a.scalars[kScGnorm2] = t[1];
-    if (a.step_part) {
-      a.scalars[kScDotG] = t[2];
-      a.scalars[kScDotD] = t[3];
-      a.scalars[kScStep2] = t[4];
-      a.scalars[kScXnorm2] = t[5];
-    }
-    if (a.decide_mode >= 0) decide_step(a.ctl, a.scalars, a.decide_mode);
-  }
+  double t[kScNotPD];
+  cta_sum_scalars(w, shr, t);
+  if (tid == 0) finish_scalars(a.ctl, a.scalars, out.cost, t, a.step_part != nullptr, a.decide_mode);
 }
 
 // ---------------------------------------------------------------- multi-GPU: pack / unpack around the all-reduce
-// buffer: [C G*G | gc G | cost, |gf|^2, dotG, dotD, step2, xnorm2 | per-rank |gf|_inf slots]
+// buffer: [C G*G | gc G | scalars kScCost .. kScXnorm2 | per-rank |gf|_inf slots]
 // sharded inertial runs append [diag(B) of separator frames P*9 | g of separator frames P*9]
 __global__ void mg_pack_kernel(int G, const Ctl* ctl, int which, Blocks b0, Blocks b1, const double* scalars, int rank,
                                int nranks, double* buf, int sep_fd, int n_frames, int ghost) {
@@ -563,7 +579,7 @@ __global__ void mg_pack_kernel(int G, const Ctl* ctl, int which, Blocks b0, Bloc
   const int NS = G * G + G, tid = blockIdx.x * blockDim.x + threadIdx.x;
   for (int k = tid; k < NS; k += gridDim.x * blockDim.x) buf[k] = k < G * G ? b.C[k] : b.gc[k - G * G];
   if (sep_fd > 0) {
-    double* sd = buf + NS + 6 + nranks;
+    double* sd = buf + NS + kScGmax + nranks;
     double* sg = sd + nranks * sep_fd;
     for (int k = tid; k < nranks * sep_fd; k += gridDim.x * blockDim.x) {
       const int slot = k / sep_fd, r = k - slot * sep_fd;
@@ -573,13 +589,8 @@ __global__ void mg_pack_kernel(int G, const Ctl* ctl, int which, Blocks b0, Bloc
     }
   }
   if (tid == 0) {
-    buf[NS + 0] = scalars[kScCost];
-    buf[NS + 1] = scalars[kScGnorm2];
-    buf[NS + 2] = scalars[kScDotG];
-    buf[NS + 3] = scalars[kScDotD];
-    buf[NS + 4] = scalars[kScStep2];
-    buf[NS + 5] = scalars[kScXnorm2];
-    for (int r = 0; r < nranks; ++r) buf[NS + 6 + r] = r == rank ? scalars[kScGmax] : 0.0;
+    for (int q = 0; q < kScGmax; ++q) buf[NS + q] = scalars[q];
+    for (int r = 0; r < nranks; ++r) buf[NS + kScGmax + r] = r == rank ? scalars[kScGmax] : 0.0;
   }
 }
 __global__ void mg_unpack_decide_kernel(int G, Ctl* ctl, int which, Blocks b0, Blocks b1, double* scalars, int nranks,
@@ -600,7 +611,7 @@ __global__ void mg_unpack_decide_kernel(int G, Ctl* ctl, int which, Blocks b0, B
     }
   }
   if (sep_fd > 0) {  // separator frames: keep the summed diagonal / gradient, norm the gradient once
-    const double* sd = buf + NS + 6 + nranks;
+    const double* sd = buf + NS + kScGmax + nranks;
     for (int k = tid; k < 2 * nranks * sep_fd; k += 256) {
       sep_out[k] = sd[k];
       if (k >= nranks * sep_fd) {
@@ -615,16 +626,12 @@ __global__ void mg_unpack_decide_kernel(int G, Ctl* ctl, int which, Blocks b0, B
   if (tid == 0) {
     gm = 0.0; g2 = 0.0;
     for (int k = 0; k < 256; ++k) { gm = fmax(gm, shm[k]); g2 += shs[k]; }
-    for (int r = 0; r < nranks; ++r) gm = fmax(gm, buf[NS + 6 + r]);
-    *b.cost = buf[NS];
-    scalars[kScCost] = buf[NS];
-    scalars[kScGmax] = gm;
-    scalars[kScGnorm2] = buf[NS + 1] + g2;
-    scalars[kScDotG] = buf[NS + 2];
-    scalars[kScDotD] = buf[NS + 3];
-    scalars[kScStep2] = buf[NS + 4];
-    scalars[kScXnorm2] = buf[NS + 5];
-    if (decide_mode >= 0) decide_step(ctl, scalars, decide_mode);
+    double t[kScNotPD];
+    for (int q = 0; q < kScGmax; ++q) t[q] = buf[NS + q];
+    for (int r = 0; r < nranks; ++r) gm = fmax(gm, buf[NS + kScGmax + r]);
+    t[kScGnorm2] += g2;
+    t[kScGmax] = gm;
+    finish_scalars(ctl, scalars, b.cost, t, true, decide_mode);
   }
 }
 
@@ -697,7 +704,7 @@ __global__ void __launch_bounds__(kSolveThreads) frame_solve_kernel(SolveArgs a)
         for (int j = 0; j <= i; ++j) {
           const double bij = Bf[i * FD + j];
           double v = bij * s[i] * s[j];
-          if (i == j) v += a.D2x ? a.D2x[static_cast<int64_t>(f) * FD + i] : lm_damp(bij, s[i], rinv);
+          if (i == j) v += frame_damp<FD>(0.0, f, i, bij, s[i], rinv, a.D2x, nullptr, 0, a.dp.ghost && f == a.dp.n_frames - 1);
           L[i][j] = v;
         }
       bool ok = true;
@@ -824,7 +831,7 @@ __global__ void __launch_bounds__(256) global_solve_kernel(GlobalSolveArgs a) {
       if (e < G * G) {
         const int r = e / G, c = e - r * G;
         double v = b.C[e] * sc[r] * sc[c] - p;
-        if (r == c) v += a.D2x ? a.D2x[nfp + r] : lm_damp(b.C[e], sc[r], rinv);
+        if (r == c) v += global_damp(r, b.C[e], sc[r], rinv, a.D2x, nfp);
         S[e] = v;
       } else {
         const int r = e - G * G;
@@ -866,7 +873,7 @@ __global__ void __launch_bounds__(256) global_solve_kernel(GlobalSolveArgs a) {
       for (int k = lane; k < i; k += 32) rhs[k] -= S[i * G + k] * xi;
       __syncwarp();
     }
-    if (bad && lane == 0) a.scalars[7] = 1.0;
+    if (bad && lane == 0) a.scalars[kScNotPD] = 1.0;
   }
   __syncthreads();
   for (int i = tid; i < G; i += 256) a.delta[nfp + i] = bad ? 0.0 : rhs[i];
@@ -912,6 +919,66 @@ __device__ inline void imu_plus(const DevProblem& dp, const double* x, const dou
     xo[k] = free ? x[k] + dd : x[k];
     st[0] += dd * dd;
     if (free) st[1] += xo[k] * xo[k];
+  }
+}
+// every camera and the IMU parameters into the trial state, with their |x_new - x|^2 and |x_new|^2 added to st[0..1]
+__device__ inline void globals_plus(const DevProblem& dp, const double* x_cur, double* x_new, const double* dg, const double* sc,
+                                    double* st) {
+  for (int c = 0; c < dp.n_cams; ++c) {
+    const double* x = x_cur + dp.off_cam + kCamStateStride * c;
+    double* xo = x_new + dp.off_cam + kCamStateStride * c;
+    cam_plus(dp, c, x, dg, sc, xo);
+    cam_stats(dp, c, x, xo, st);
+  }
+  imu_plus(dp, x_cur + dp.off_imu, dg, sc, x_new + dp.off_imu, st);
+}
+
+// Frame f into the trial state (d: its scaled step): se3_plus of the pose (copied when no residual uses the frame), the
+// velocity plus its step for FD == 9 (copied for FD == 6), and the frame's share of the step statistics acc: step.g,
+// step.D2.step, |x_new - x|^2, |x_new|^2.  The ghost moves with the step too; its damping and norms are counted by its
+// owner, and its gradient is this rank's piece of the shared frame's gradient, so step.g counts it.
+template <int FD>
+__device__ __forceinline__ void frame_plus(const DevProblem& dp, const Blocks& b, const double* scale, double rinv,
+                                           const double* D2x, const double* sepdiag, int f, const double* d, bool used,
+                                           const double* x_cur, double* x_new, double acc[4]) {
+  const bool is_ghost = FD == 9 && dp.ghost && f == dp.n_frames - 1;  // (only inertial runs have a ghost)
+  double du[FD];
+#pragma unroll
+  for (int r = 0; r < FD; ++r) {
+    const int64_t k = static_cast<int64_t>(f) * FD + r;
+    const double sc = scale[k];
+    const double d2 = frame_damp<FD>(0.0, f, r, b.B[k * FD + r], sc, rinv, D2x, sepdiag, dp.rank, is_ghost);
+    acc[0] += d[r] * b.gf[k] * sc;
+    acc[1] += d[r] * d[r] * d2;
+    du[r] = d[r] * sc;
+  }
+  const bool counted = used && !is_ghost;
+  const double* x = x_cur + 7 * static_cast<int64_t>(f);
+  double xo[7];
+  if (used) {
+    se3_plus(x, du, xo);
+  } else {
+#pragma unroll
+    for (int k = 0; k < 7; ++k) xo[k] = x[k];
+  }
+#pragma unroll
+  for (int k = 0; k < 7; ++k) {
+    x_new[7 * static_cast<int64_t>(f) + k] = xo[k];
+    if (counted) {
+      acc[2] += (xo[k] - x[k]) * (xo[k] - x[k]);
+      acc[3] += xo[k] * xo[k];
+    }
+  }
+  const double* v = x_cur + dp.off_v + 3 * static_cast<int64_t>(f);
+  double* vo = x_new + dp.off_v + 3 * static_cast<int64_t>(f);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const double nv = (FD == 9) ? v[k] + du[(FD == 9) ? 6 + k : 0] : v[k];
+    vo[k] = nv;
+    if (FD == 9 && counted) {
+      acc[2] += (nv - v[k]) * (nv - v[k]);
+      acc[3] += nv * nv;
+    }
   }
 }
 
@@ -963,50 +1030,9 @@ __global__ void __launch_bounds__(32 * kUpdateWarps) backsub_update_kernel(Updat
       for (int r = 0; r < FD; ++r) d[r] = a.delta[static_cast<int64_t>(f) * FD + r];
     }
     if (lane == 0) {
-      double du[FD];
-      const bool is_ghost = a.dp.ghost && f == nf - 1;
 #pragma unroll
-      for (int r = 0; r < FD; ++r) {
-        const int64_t k = static_cast<int64_t>(f) * FD + r;
-        const double sc = a.scale[k];
-        double d2;
-        if (a.D2x) d2 = a.D2x[k];
-        else if (a.sepdiag && f == 0) d2 = lm_damp(a.sepdiag[a.dp.rank * FD + r], sc, rinv);
-        else if (is_ghost) d2 = 0.0;  // damped (and counted) by its owner
-        else d2 = lm_damp(b.B[k * FD + r], sc, rinv);
-        a.delta[k] = d[r];
-        acc[0] += d[r] * b.gf[k] * sc;
-        acc[1] += d[r] * d[r] * d2;
-        du[r] = d[r] * sc;
-      }
-      const double* x = x_cur + 7 * static_cast<int64_t>(f);
-      const bool used = a.frame_used[f] != 0;
-      double xo[7];
-      if (used) {
-        se3_plus(x, du, xo);
-      } else {
-#pragma unroll
-        for (int k = 0; k < 7; ++k) xo[k] = x[k];
-      }
-#pragma unroll
-      for (int k = 0; k < 7; ++k) {
-        x_new[7 * static_cast<int64_t>(f) + k] = xo[k];
-        if (!is_ghost && used) {
-          acc[2] += (xo[k] - x[k]) * (xo[k] - x[k]);
-          acc[3] += xo[k] * xo[k];
-        }
-      }
-      const double* v = x_cur + a.dp.off_v + 3 * static_cast<int64_t>(f);
-      double* vo = x_new + a.dp.off_v + 3 * static_cast<int64_t>(f);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) {
-        const double nv = (FD == 9) ? v[k] + du[(FD == 9) ? 6 + k : 0] : v[k];
-        vo[k] = nv;
-        if (FD == 9 && !is_ghost) {
-          acc[2] += (nv - v[k]) * (nv - v[k]);
-          acc[3] += nv * nv;
-        }
-      }
+      for (int r = 0; r < FD; ++r) a.delta[static_cast<int64_t>(f) * FD + r] = d[r];
+      frame_plus<FD>(a.dp, b, a.scale, rinv, a.D2x, a.sepdiag, f, d, a.frame_used[f] != 0, x_cur, x_new, acc);
     }
   }
   if (lane == 0)
@@ -1023,15 +1049,9 @@ __global__ void __launch_bounds__(32 * kUpdateWarps) backsub_update_kernel(Updat
   if (blockIdx.x == 0 && threadIdx.x == 32 * kUpdateWarps - 1) {
     double g4[4] = {0.0, 0.0, 0.0, 0.0};
     const double* sc = a.scale + nfp;
-    for (int c = 0; c < a.dp.n_cams; ++c) {
-      const double* x = x_cur + a.dp.off_cam + kCamStateStride * c;
-      double* xo = x_new + a.dp.off_cam + kCamStateStride * c;
-      cam_plus(a.dp, c, x, dc, sc, xo);
-      cam_stats(a.dp, c, x, xo, g4 + 2);
-    }
-    imu_plus(a.dp, x_cur + a.dp.off_imu, dc, sc, x_new + a.dp.off_imu, g4 + 2);
+    globals_plus(a.dp, x_cur, x_new, dc, sc, g4 + 2);
     for (int k = 0; k < G; ++k) {
-      const double d2 = a.D2x ? a.D2x[nfp + k] : lm_damp(b.C[k * G + k], sc[k], rinv);
+      const double d2 = global_damp(k, b.C[k * G + k], sc[k], rinv, a.D2x, nfp);
       g4[0] += dc[k] * b.gc[k] * sc[k];
       g4[1] += dc[k] * dc[k] * d2;
     }

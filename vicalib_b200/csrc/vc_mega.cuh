@@ -35,7 +35,7 @@ namespace cg = cooperative_groups;
 constexpr int kMegaMaxWarps = 16;
 constexpr int kMegaMaxThreads = 32 * kMegaMaxWarps;
 constexpr int kGtabMax = 256;
-constexpr int kMegaPartExtra = 8;  // scalars appended to each CTA's partial slot
+constexpr int kMegaPartExtra = 8;  // scalars appended to each CTA's partial slot (kScCost .. kScNotPD)
 // Totals buffer: every rank owns one (32 MiB, the vision kernel uses the first 4); in a frame-sharded run (one process per GPU) all ranks of the
 // node map all of them (CUDA IPC).  A total is published as two 64-bit words {low half | tag}, {high half | tag}
 // (tag = exchange number): an 8-byte store is single-copy atomic, so a reader that sees both tags has the value —
@@ -51,7 +51,6 @@ constexpr int kXchgCtlOff = 442368;
 constexpr int kXchgPlainS = kXchgCtlOff + 64;
 constexpr int kXchgPlainC = kXchgPlainS + 32768;
 constexpr int kMegaCommFailed = 1000;  // Ctl::done value when a peer never showed up
-enum { kPCost = 0, kPGf2, kPDotG, kPDotD, kPStep2, kPXnorm2, kPGfMax, kPNotPD };
 enum { kProfS = 0, kProfG, kProfU, kProfB, kProfD, kProfSync, kProfCount };
 
 struct MegaArgs {
@@ -332,7 +331,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
             for (int j = 0; j <= i; ++j) {
               const double bij = Bf[i * FD + j];
               double v = bij * s[i] * s[j];
-              if (i == j) v += lm_damp(bij, s[i], rinv);
+              if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], rinv, nullptr, nullptr, 0, false);
               L[i][j] = v;
             }
           bool ok = true;
@@ -410,7 +409,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       if (tid == 0) {
         double v = 0.0;
         for (int w = 0; w < nwarps; ++w) v = fmax(v, wred[8 * w]);
-        out[NS + kPNotPD] = v;
+        out[NS + kScNotPD] = v;
       }
     }
     mark(kProfS);
@@ -430,10 +429,10 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       if (sharded) {
         // every rank's CTA sums go to every rank (tagged words over NVLink); ONE thread of this grid per entry waits for
         // them and adds them up in rank order (every rank computes the same bits)
-        mega_publish(a.partS, PS, nb, PS, a, 0, parS, epS, NS + kPNotPD, -1);
-        for (int e = bid * nthreads + tid; e < PS; e += nb * nthreads) totS[e] = mega_total(a, 0, PS, parS, epS, e, e == NS + kPNotPD);
+        mega_publish(a.partS, PS, nb, PS, a, 0, parS, epS, NS + kScNotPD, -1);
+        for (int e = bid * nthreads + tid; e < PS; e += nb * nthreads) totS[e] = mega_total(a, 0, PS, parS, epS, e, e == NS + kScNotPD);
       } else {
-        mega_reduce_stage1(a.partS, PS, nb, PS, totS, NS + kPNotPD, -1);
+        mega_reduce_stage1(a.partS, PS, nb, PS, totS, NS + kScNotPD, -1);
       }
       mark(kProfG);
       grid.sync();
@@ -445,7 +444,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           const int r = e / G, c = e - r * G;
           if (c > r) continue;
           double v = Ccur[e] * scg[r] * scg[c] - p;
-          if (r == c) v += lm_damp(Ccur[e], scg[r], rinv);
+          if (r == c) v += global_damp(r, Ccur[e], scg[r], rinv, nullptr, 0);
           S[e] = v;
         } else {
           const int r = e - G * G;
@@ -453,7 +452,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
         }
       }
       if (tid == 0) {
-        sc[kScNotPD] = __ldcg(totS + NS + kPNotPD);
+        sc[kScNotPD] = __ldcg(totS + NS + kScNotPD);
         bad = 0;
       }
       __syncthreads();
@@ -472,7 +471,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
     mark(kProfG);
 
     // ------------------------------------------------------------ U: back-substitution, trial states
-    double ustat[4] = {0.0, 0.0, 0.0, 0.0};  // lane 0 of each warp: dotG, dotD, step2, xnorm2
+    double ustat[4] = {0.0, 0.0, 0.0, 0.0};  // lane 0 of each warp: kScDotG .. kScXnorm2
     {
       if (warp == nwarps - 1) {  // trial camera states (every CTA needs them; the last warp is the one most likely
                                  // to own no frame); CTA 0 also stores the globals
@@ -498,7 +497,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           }
           for (int q = 0; q < kImuStateSize; ++q) x_new[a.dp.off_imu + q] = x_cur[a.dp.off_imu + q];
           for (int q = 0; q < G; ++q) {
-            const double d2 = lm_damp(Ccur[q * G + q], scg[q], rinv);
+            const double d2 = global_damp(q, Ccur[q * G + q], scg[q], rinv, nullptr, 0);
             ustat[0] += dg[q] * Ccur[G * G + q] * scg[q];
             ustat[1] += dg[q] * dg[q] * d2;
           }
@@ -517,36 +516,9 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           d[r] = -Xf[r * M + G] - s;
         }
         if (lane == 0) {
-          double du[FD];
 #pragma unroll
-          for (int r = 0; r < FD; ++r) {
-            const int64_t q = static_cast<int64_t>(f) * FD + r;
-            const double s = a.scale[q];
-            const double d2 = lm_damp(bc.B[q * FD + r], s, rinv);
-            a.delta[q] = d[r];
-            ustat[0] += d[r] * bc.gf[q] * s;
-            ustat[1] += d[r] * d[r] * d2;
-            du[r] = d[r] * s;
-          }
-          const double* x = x_cur + 7 * static_cast<int64_t>(f);
-          const bool used = a.frame_used[f] != 0;
-          double xo[7];
-          if (used) {
-            se3_plus(x, du, xo);
-          } else {
-#pragma unroll
-            for (int q = 0; q < 7; ++q) xo[q] = x[q];
-          }
-#pragma unroll
-          for (int q = 0; q < 7; ++q) {
-            x_new[7 * static_cast<int64_t>(f) + q] = xo[q];
-            if (used) {
-              ustat[2] += (xo[q] - x[q]) * (xo[q] - x[q]);
-              ustat[3] += xo[q] * xo[q];
-            }
-          }
-#pragma unroll
-          for (int q = 0; q < 3; ++q) x_new[a.dp.off_v + 3 * static_cast<int64_t>(f) + q] = x_cur[a.dp.off_v + 3 * static_cast<int64_t>(f) + q];
+          for (int r = 0; r < FD; ++r) a.delta[static_cast<int64_t>(f) * FD + r] = d[r];
+          frame_plus<FD>(a.dp, bc, a.scale, rinv, nullptr, nullptr, f, d, a.frame_used[f] != 0, x_cur, x_new, ustat);
         }
       }
       for (int e = tid; e < nwarps * NP; e += nthreads) Cw[e] = 0.0;
@@ -587,8 +559,9 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       }
       if (lane == 0) {
         double* w = wred + 8 * warp;
-        w[0] = cost; w[1] = gf2; w[2] = gfmax;
-        w[3] = ustat[0]; w[4] = ustat[1]; w[5] = ustat[2]; w[6] = ustat[3];
+        w[kScCost] = cost; w[kScGnorm2] = gf2; w[kScGmax] = gfmax;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) w[kScDotG + q] = ustat[q];
       }
       __syncthreads();
       double* out = a.partC + static_cast<int64_t>(bid) * PC;
@@ -598,15 +571,15 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
         out[e] = v;
       }
       if (tid == 0) {
-        double t[7] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        double t[kScNotPD] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
         for (int w = 0; w < nwarps; ++w) {
           const double* p = wred + 8 * w;
-          t[0] += p[0]; t[1] += p[1]; t[2] = fmax(t[2], p[2]);
-          t[3] += p[3]; t[4] += p[4]; t[5] += p[5]; t[6] += p[6];
+#pragma unroll
+          for (int q = 0; q < kScGmax; ++q) t[q] += p[q];
+          t[kScGmax] = fmax(t[kScGmax], p[kScGmax]);
         }
-        out[NP + kPCost] = t[0]; out[NP + kPGf2] = t[1]; out[NP + kPGfMax] = t[2];
-        out[NP + kPDotG] = t[3]; out[NP + kPDotD] = t[4]; out[NP + kPStep2] = t[5]; out[NP + kPXnorm2] = t[6];
-        out[NP + kPNotPD] = 0.0;
+        for (int q = 0; q < kScNotPD; ++q) out[NP + q] = t[q];
+        out[NP + kScNotPD] = 0.0;
       }
     }
     mark(kProfB);
@@ -620,11 +593,11 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       const int parC = static_cast<int>(epC & 1);
       double* totC = reinterpret_cast<double*>(a.xbuf[a.rank] + (sharded ? kXchgPlainC : kXchgCOff));
       if (sharded) {
-        mega_publish(a.partC, PC, nb, PC, a, kXchgCOff, parC, epC, NP + kPGfMax, NP + kPNotPD);
+        mega_publish(a.partC, PC, nb, PC, a, kXchgCOff, parC, epC, NP + kScGmax, NP + kScNotPD);
         for (int e = bid * nthreads + tid; e < PC; e += nb * nthreads)
-          totC[e] = mega_total(a, kXchgCOff, PC, parC, epC, e, e == NP + kPGfMax || e == NP + kPNotPD);
+          totC[e] = mega_total(a, kXchgCOff, PC, parC, epC, e, e == NP + kScGmax || e == NP + kScNotPD);
       } else {
-        mega_reduce_stage1(a.partC, PC, nb, PC, totC, NP + kPGfMax, NP + kPNotPD);
+        mega_reduce_stage1(a.partC, PC, nb, PC, totC, NP + kScGmax, NP + kScNotPD);
       }
       mark(kProfD);
       grid.sync();
@@ -653,10 +626,6 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       }
       __syncthreads();
       if (warp == 0) {
-        double v[7];
-        v[0] = totc[NP + kPCost]; v[1] = totc[NP + kPGf2]; v[2] = totc[NP + kPDotG];
-        v[3] = totc[NP + kPDotD]; v[4] = totc[NP + kPStep2]; v[5] = totc[NP + kPXnorm2];
-        v[6] = totc[NP + kPGfMax];
         double g2 = 0.0, gm = 0.0;
         for (int q = lane; q < G; q += 32) {
           const double gv = Ctrial[G * G + q];
@@ -669,19 +638,16 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           gm = fmax(gm, __shfl_xor_sync(0xffffffffu, gm, o));
         }
         if (lane == 0) {
-          sc[kScCost] = v[0];
-          sc[kScGnorm2] = v[1] + g2;
-          sc[kScGmax] = fmax(v[6], gm);
-          sc[kScDotG] = v[2];
-          sc[kScDotD] = v[3];
-          sc[kScStep2] = v[4];
-          sc[kScXnorm2] = v[5];
-          decide_step(ctl, sc, 1);
+          double t[kScNotPD];
+#pragma unroll
+          for (int q = 0; q < kScNotPD; ++q) t[q] = totc[NP + q];
+          t[kScGnorm2] += g2;
+          t[kScGmax] = fmax(t[kScGmax], gm);
+          finish_scalars(ctl, sc, bid == 0 ? bt.cost : nullptr, t, true, 1);
           if (bid == 0) {
             if (ctl->done) atomicOr(ctlw + 2, 1ull);
             *a.ctl = *ctl;
-            for (int q = 0; q < 8; ++q) a.scalars[q] = sc[q];
-            *bt.cost = v[0];
+            for (int q = 0; q <= kScNotPD; ++q) a.scalars[q] = sc[q];
           }
         }
       }

@@ -677,7 +677,7 @@ static int prepare(vcgpu_handle* h) {
     VC_TRY(dev_alloc(h, &h->d_delta, np));
     VC_TRY(dev_alloc(h, &h->d_red, 4 * (static_cast<size_t>(nf) + 2)));
     VC_TRY(dev_alloc(h, &h->d_red_part, 8 * kReduceBlocks));
-    VC_TRY(dev_alloc(h, &h->d_mg, NS + 6 + h->nranks + 18 * h->nranks));
+    VC_TRY(dev_alloc(h, &h->d_mg, NS + kScGmax + h->nranks + 18 * h->nranks));
     VC_TRY(dev_alloc(h, &h->d_sep, 18 * h->nranks));
     {
       const size_t N = static_cast<size_t>(G) + 9 * h->nranks;
