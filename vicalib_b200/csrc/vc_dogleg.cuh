@@ -25,6 +25,11 @@ struct DlVecs {           // all [nf*fd + G]
 };
 
 // ---------------------------------------------------------------- D, g~, u, mu D^2
+// D^2 of entry i: clamp(diag H) of the scaled system (diag: the unscaled H_ii, s: its Jacobi scale)
+__device__ __forceinline__ double dl_clamp(double diag, double s) {
+  const double c = diag * s * s;
+  return c < 1e-6 ? 1e-6 : (c > 1e32 ? 1e32 : c);
+}
 __global__ void dl_prep_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl* ctl, const double* scale, DlVecs v) {
   if (ctl->done) return;
   const Blocks& b = ctl->cur ? b1 : b0;
@@ -43,8 +48,7 @@ __global__ void dl_prep_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl* c
     g = b.gc[k];
   }
   const double s = scale[i];
-  double c = d * s * s;
-  c = c < 1e-6 ? 1e-6 : (c > 1e32 ? 1e32 : c);
+  const double c = dl_clamp(d, s);
   const double D = sqrt(c);
   const double gt = g * s / D;
   v.diag[i] = D;
@@ -223,26 +227,32 @@ __global__ void __launch_bounds__(256) dl_dots_kernel(DlDotArgs a) {
 }
 
 // ---------------------------------------------------------------- the dogleg point (Ceres DoglegStrategy::ComputeTraditionalDoglegStep)
+// step~ = cg g~ + cn gn from the step's scalars (radius, alpha, |g~|^2, |gn|^2, b = g~ . gn); returns |step~|.  The one
+// definition of the branch rule: dl_combine_kernel and the persistent kernel (vc_mega.cuh) both call it.
+__device__ inline double dogleg_point(double radius, double alpha, double g2, double gn2, double b, double* cg, double* cn) {
+  const double gn_norm = sqrt(gn2), g_norm = sqrt(g2);
+  if (gn_norm <= radius) {
+    *cg = 0.0; *cn = 1.0;
+    return gn_norm;
+  }
+  if (g_norm * alpha >= radius) {
+    *cg = -(radius / g_norm); *cn = 0.0;
+    return radius;
+  }
+  const double b_dot_a = -alpha * b;
+  const double a_sq = (alpha * g_norm) * (alpha * g_norm);
+  const double bma_sq = a_sq - 2.0 * b_dot_a + gn_norm * gn_norm;
+  const double cc = b_dot_a - a_sq;
+  const double d = sqrt(cc * cc + bma_sq * (radius * radius - a_sq));
+  const double beta = cc <= 0.0 ? (d - cc) / bma_sq : (radius * radius - a_sq) / (d + cc);
+  *cg = -alpha * (1.0 - beta); *cn = beta;
+  // |cg g~ + cn gn|^2 from the known inner products
+  return sqrt(fmax(0.0, *cg * *cg * g2 + 2.0 * *cg * *cn * b + *cn * *cn * gn2));
+}
 __global__ void dl_combine_kernel(Ctl* ctl, DlVecs v, double* delta, int64_t n) {
   if (ctl->done) return;
-  const double radius = ctl->radius, alpha = ctl->dl_alpha;
-  const double gn_norm = sqrt(ctl->dl_gn2), g_norm = sqrt(ctl->dl_g2);
-  double cg, cn, step_norm;  // step~ = cg * g~ + cn * gn
-  if (gn_norm <= radius) {
-    cg = 0.0; cn = 1.0; step_norm = gn_norm;
-  } else if (g_norm * alpha >= radius) {
-    cg = -(radius / g_norm); cn = 0.0; step_norm = radius;
-  } else {
-    const double b_dot_a = -alpha * ctl->dl_b;
-    const double a_sq = (alpha * g_norm) * (alpha * g_norm);
-    const double bma_sq = a_sq - 2.0 * b_dot_a + gn_norm * gn_norm;
-    const double cc = b_dot_a - a_sq;
-    const double d = sqrt(cc * cc + bma_sq * (radius * radius - a_sq));
-    const double beta = cc <= 0.0 ? (d - cc) / bma_sq : (radius * radius - a_sq) / (d + cc);
-    cg = -alpha * (1.0 - beta); cn = beta;
-    // |cg g~ + cn gn|^2 from the known inner products
-    step_norm = sqrt(fmax(0.0, cg * cg * ctl->dl_g2 + 2.0 * cg * cn * ctl->dl_b + cn * cn * ctl->dl_gn2));
-  }
+  double cg, cn;
+  const double step_norm = dogleg_point(ctl->radius, ctl->dl_alpha, ctl->dl_g2, ctl->dl_gn2, ctl->dl_b, &cg, &cn);
   const int64_t i = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (i < n) {
     const double st = ctl->dl_ok ? (cg * v.grad[i] + cn * v.gn[i]) / v.diag[i] : 0.0;

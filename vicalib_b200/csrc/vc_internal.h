@@ -184,8 +184,8 @@ struct vcgpu_handle {
   double *d_partS = nullptr, *d_partC = nullptr;  // [grid][G*G+G+8] / [grid][n_cams*kCgStride+8]
   unsigned long long* d_prof = nullptr;
   int dev_sms = 0, dev_smem_optin = 0;
-  size_t mega_smem_set = 0;
-  int mega_grid = 0, mega_warps = 0;  // 0 warps: does not fit / not supported, use the multi-launch engine
+  size_t mega_smem_set[2] = {0, 0};  // per instantiation of lm_mega_kernel ([strategy]: 0 LM, 1 DOGLEG)
+  int mega_grid = 0, mega_warps[2] = {0, 0};  // 0 warps: does not fit / not supported, use the multi-launch engine
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)
   bool imu_mega_ok = false;
   int imu_mega_grid = 0;

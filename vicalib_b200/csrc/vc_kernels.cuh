@@ -356,6 +356,7 @@ __device__ inline void cta_sum_scalars(double v[kScNotPD], double (*shr)[8], dou
 
 // the evaluated point's totals t[kScCost .. kScXnorm2, kScGmax] -> its cost (unless null) and the scalars sc (the step
 // entries only when the point is a trial step), then the decision (decide_mode: -1 none, else decide_step's mode)
+template <Strategy S = Strategy::kLM>
 __device__ inline void finish_scalars(Ctl* ctl, double* sc, double* cost, const double* t, bool with_step, int decide_mode) {
   if (cost) *cost = t[kScCost];
   sc[kScCost] = t[kScCost];
@@ -363,7 +364,7 @@ __device__ inline void finish_scalars(Ctl* ctl, double* sc, double* cost, const 
   sc[kScGmax] = t[kScGmax];
   if (with_step)
     for (int q = kScDotG; q <= kScXnorm2; ++q) sc[q] = t[q];
-  if (decide_mode >= 0) decide_step<Strategy::kLM>(ctl, sc, decide_mode);
+  if (decide_mode >= 0) decide_step<S>(ctl, sc, decide_mode);
 }
 
 // ---------------------------------------------------------------- reduce + finalize + decide in one launch

@@ -1,6 +1,7 @@
 // Persistent trust-region kernel for the vision-only problem (one GPU, or frame shards on several).
 //
-// One cooperative launch runs up to n_iters Levenberg-Marquardt iterations; one CTA per SM, every
+// One cooperative launch runs up to n_iters trust-region iterations, Levenberg-Marquardt or (one GPU) DOGLEG: the kernel
+// is instantiated per strategy (Strategy::kLM, kDogleg).  One CTA per SM, every
 // frame owned by the same WARP of the same CTA for the whole solve (frame f -> CTA f mod grid, warp
 // (f / grid) mod warps).  An iteration is a chain of per-frame warp phases and small every-CTA phases,
 // separated by grid barriers instead of launches:
@@ -11,6 +12,9 @@
 //      one GPU: plain totals + grid barrier; shards: tagged words into every rank's buffer, readers poll
 //   G  every CTA, redundantly: reduced system C + D - sum E^T X, Cholesky, globals' step
 //   U  per frame (warp):  back-substitution, x (+) step, step statistics; trial camera states
+//      DOGLEG: U1 per frame (warp): back-substitution x_f, CTA partials of the step scalars; one more grid barrier;
+//      every CTA sums them, takes the dogleg point (dogleg_point, vc_dogleg.cuh) and the model change; U2 as U with
+//      the dogleg step in place of x
 //   B  per frame (warp): fused evaluate + Gram build at the trial point (build_frame_warp, vc_fused.cuh), 32
 //      corners at a time through the warp's own shared-memory slab and FP64 DMMA (no block barrier anywhere in
 //      the phase); the camera blocks are accumulated per warp, packed per camera
@@ -21,11 +25,19 @@
 //
 // Every CTA (of every rank) reads bit-identical totals, so all take the same decision and the loop needs
 // no broadcast; all sums run in a fixed order (deterministic).  Replaces the body of ceres::Solve
-// (vicalibrator.h:956) for the staged vision solves; the inertial path keeps the multi-launch engine
-// (vc_engine.inl).
+// (vicalibrator.h:956) for the staged vision solves; the inertial path has its own persistent kernels
+// (vc_imu_mega.cuh, vc_imu_eval_mega.cuh), and frame-sharded DOGLEG runs the multi-launch engine (vc_engine.inl).
+//
+// DOGLEG (vc_dogleg.cuh's header) on the same Jacobi-scaled system H = S J^T J S, g = S J^T r: S and G solve
+// (H + mu D^2) x = -g (the damping mu clamp(diag H) in place of LM's clamp(diag H) / radius).  Every product with H the
+// step needs is local to a frame once the CTA holds the globals' parts (replicated), so U1 needs no mat-vec pass: per
+// frame the partials |g~_f|^2, u_f.(Hu)_f-share, |gn_f|^2, g~_f.gn_f, u.Hx and x.Hx frame shares (u = g~ / D, gn = D x),
+// the globals' shares added by every CTA alike.  Then step~ = cg g~ + cn gn, step = step~ / D and the model change
+// -step.g - step.H.step / 2 = -(cg |g~|^2 + cn g~.gn) - (cg^2 u.Hu + 2 cg cn u.Hx + cn^2 x.Hx) / 2.
 #pragma once
 #include <cooperative_groups.h>
 
+#include "vc_dogleg.cuh"
 #include "vc_fused.cuh"
 #include "vc_kernels.cuh"
 
@@ -75,10 +87,15 @@ struct MegaArgs {
   unsigned long long* prof;  // [kProfCount] ns per phase (CTA 0), or null
 };
 
-__host__ __device__ inline size_t mega_smem_doubles(int G, int n_cams, int n_warps) {
+// DOGLEG's step scalars: U1's per-CTA partials (in the Schur partial slot's unused entries partS[NS + 0 .. 5], summed by
+// every CTA after U1's barrier) and the globals' shares of them
+enum { kDlG2 = 0, kDlUHu, kDlGn2, kDlB, kDlUHx, kDlXHx, kDlParts };
+// dynamic shared memory of lm_mega_kernel (strategy: 0 LM, 1 DOGLEG); DOGLEG adds u_g, D_g, g~_g and its scalars
+__host__ __device__ inline size_t mega_smem_doubles(int G, int n_cams, int n_warps, int strategy) {
   const size_t NS = static_cast<size_t>(G) * G + G;
   return static_cast<size_t>(n_warps) * (kWarpDoubles + n_cams * kCgStride) + 3 * NS + G + kMaxCams * (kCamStateStride + 9) +
-         kScCount + 8 * kMegaMaxWarps + n_cams * kCgStride + kMegaPartExtra + sizeof(Ctl) / sizeof(double) + 8;
+         kScCount + 8 * kMegaMaxWarps + n_cams * kCgStride + kMegaPartExtra + sizeof(Ctl) / sizeof(double) + 8 +
+         (strategy == 1 ? 3 * static_cast<size_t>(G) + 8 : 0);
 }
 
 __device__ __forceinline__ unsigned long long global_ns() {
@@ -224,7 +241,9 @@ __device__ inline void mega_chol_solve_smem(double* S, int G, int lane, double* 
   }
 }
 
+template <Strategy Str>
 __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a) {
+  constexpr bool kDl = Str == Strategy::kDogleg;
   extern __shared__ double smem[];
   cg::grid_group grid = cg::this_grid();
   constexpr int FD = 6;
@@ -248,6 +267,10 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
   double* wred = sc + kScCount;                                      // [kMegaMaxWarps][8] per-warp scalars
   double* totc = wred + 8 * kMegaMaxWarps;                           // [NP + 8] packed camera blocks / scalars, grid (and rank) totals
   Ctl* ctl = reinterpret_cast<Ctl*>(totc + NP + kMegaPartExtra);
+  double* dl_u = reinterpret_cast<double*>(ctl + 1);                 // DOGLEG: [G] u_g = g~_g / D_g
+  double* dl_D = dl_u + G;                                           // [G] D_g
+  double* dl_gt = dl_D + G;                                          // [G] g~_g
+  double* dl_s = dl_gt + G;                                          // [8] globals' shares (kDl*), then cg, cn
   __shared__ int bad;
   __shared__ int2 gtab[kGtabMax];          // (start, count) of the observations of this CTA's (frame slot, camera) pairs
   __shared__ unsigned char tri_lut[128];   // packed lower-triangle index -> (row << 4 | col)
@@ -304,7 +327,8 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
     const Blocks& bt = a.blk[1 - cur];
     const double* x_cur = a.state[cur];
     double* x_new = a.state[1 - cur];
-    const double rinv = 1.0 / ctl->radius;
+    // the damping's multiplier: LM clamp(diag) / radius; DOGLEG mu clamp(diag), the Gauss-Newton solve's regularisation
+    const double dmul = kDl ? ctl->dl_mu : 1.0 / ctl->radius;
     const double* Ccur = Cacc + cur * NS;
     double notpd = 0.0;
 
@@ -331,7 +355,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
             for (int j = 0; j <= i; ++j) {
               const double bij = Bf[i * FD + j];
               double v = bij * s[i] * s[j];
-              if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], rinv, nullptr, nullptr, 0, false);
+              if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], dmul, nullptr, nullptr, 0, false);
               L[i][j] = v;
             }
           bool ok = true;
@@ -444,7 +468,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           const int r = e / G, c = e - r * G;
           if (c > r) continue;
           double v = Ccur[e] * scg[r] * scg[c] - p;
-          if (r == c) v += global_damp(r, Ccur[e], scg[r], rinv, nullptr, 0);
+          if (r == c) v += global_damp(r, Ccur[e], scg[r], dmul, nullptr, 0);
           S[e] = v;
         } else {
           const int r = e - G * G;
@@ -470,7 +494,149 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
     }
     mark(kProfG);
 
+    // ------------------------------------------------------------ U1 (DOGLEG): Gauss-Newton step, step scalars
+    if constexpr (kDl) {
+      for (int i = tid; i < G; i += nthreads) {
+        const double D = sqrt(dl_clamp(Ccur[i * G + i], scg[i]));
+        const double gt = Ccur[G * G + i] * scg[i] / D;
+        dl_D[i] = D;
+        dl_gt[i] = gt;
+        dl_u[i] = gt / D;
+      }
+      __syncthreads();
+      double part[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};  // lane 0 of each warp: its frames' shares
+      if (warp == nwarps - 1) {  // the globals' shares, the same bits in every CTA (x_g = dg)
+        double q[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int r = lane; r < G; r += 32) {
+          double cu = 0.0, cx = 0.0;  // rows of (S C S) u_g, (S C S) x_g
+          for (int c = 0; c < G; ++c) {
+            const double h = Ccur[r * G + c] * scg[r] * scg[c];
+            cu += h * dl_u[c];
+            cx += h * dg[c];
+          }
+          const double gn = dg[r] * dl_D[r];
+          q[kDlG2] += dl_gt[r] * dl_gt[r];
+          q[kDlUHu] += dl_u[r] * cu;
+          q[kDlGn2] += gn * gn;
+          q[kDlB] += dl_gt[r] * gn;
+          q[kDlUHx] += dl_u[r] * cx;
+          q[kDlXHx] += dg[r] * cx;
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+          for (int j = 0; j < kDlParts; ++j) q[j] += __shfl_xor_sync(0xffffffffu, q[j], o);
+        if (lane == 0)
+          for (int j = 0; j < kDlParts; ++j) dl_s[j] = q[j];
+      }
+      for (int k = warp; k < nk; k += nwarps) {
+        const int f = bid + k * nb;
+        const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
+        const double* Ef = bc.E + static_cast<int64_t>(f) * FD * G;
+        double x[FD], ex[FD], eu[FD];  // x_f, then rows of E S x_g and E S u_g (the frame's row scale not yet applied)
+#pragma unroll
+        for (int r = 0; r < FD; ++r) {
+          double s = 0.0, t = 0.0, v = 0.0;
+          for (int c = lane; c < G; c += 32) {
+            s += Xf[r * M + c] * dg[c];
+            const double e = Ef[r * G + c] * scg[c];
+            t += e * dg[c];
+            v += e * dl_u[c];
+          }
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            s += __shfl_xor_sync(0xffffffffu, s, o);
+            t += __shfl_xor_sync(0xffffffffu, t, o);
+            v += __shfl_xor_sync(0xffffffffu, v, o);
+          }
+          x[r] = -Xf[r * M + G] - s;
+          ex[r] = t;
+          eu[r] = v;
+        }
+        if (lane == 0) {
+          const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+          const double* Bf = bc.B + static_cast<int64_t>(f) * FD * FD;
+          const double* gf = bc.gf + static_cast<int64_t>(f) * FD;
+          double u[FD], wu[FD], wx[FD];
+#pragma unroll
+          for (int r = 0; r < FD; ++r) {
+            const double D = sqrt(dl_clamp(Bf[r * FD + r], sf[r]));
+            const double gt = gf[r] * sf[r] / D;
+            const double gn = x[r] * D;
+            u[r] = gt / D;
+            wu[r] = sf[r] * u[r];
+            wx[r] = sf[r] * x[r];
+            part[kDlG2] += gt * gt;
+            part[kDlGn2] += gn * gn;
+            part[kDlB] += gt * gn;
+            a.delta[static_cast<int64_t>(f) * FD + r] = x[r];
+          }
+#pragma unroll
+          for (int r = 0; r < FD; ++r) {
+            double bu = 0.0, bx = 0.0;
+#pragma unroll
+            for (int j = 0; j < FD; ++j) {
+              bu += Bf[r * FD + j] * wu[j];
+              bx += Bf[r * FD + j] * wx[j];
+            }
+            const double hu = sf[r] * (bu + eu[r]), hx = sf[r] * (bx + ex[r]);  // rows of H u, H x of the frame
+            const double gu = sf[r] * eu[r], gx = sf[r] * ex[r];                // rows of (S E S) u_g, (S E S) x_g
+            part[kDlUHu] += u[r] * hu + u[r] * gu;  // u_f.(S B S) u_f + 2 u_f.(S E S) u_g
+            part[kDlUHx] += u[r] * hx + x[r] * gu;  // u_f.(S B S) x_f + u_f.(S E S) x_g + x_f.(S E S) u_g
+            part[kDlXHx] += x[r] * hx + x[r] * gx;  // x_f.(S B S) x_f + 2 x_f.(S E S) x_g
+          }
+        }
+      }
+      if (lane == 0)
+        for (int j = 0; j < kDlParts; ++j) wred[8 * warp + j] = part[j];
+      __syncthreads();
+      if (tid == 0) {
+        double* out = a.partS + static_cast<int64_t>(bid) * PS + NS;
+        for (int j = 0; j < kDlParts; ++j) {
+          double v = 0.0;
+          for (int w = 0; w < nwarps; ++w) v += wred[8 * w + j];
+          out[j] = v;
+        }
+      }
+      mark(kProfU);
+      grid.sync();
+      mark(kProfSync);
+      if (warp == 0) {  // every CTA adds up the CTA partials alike, then the dogleg point and the model change
+        double t[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int b = lane; b < nb; b += 32)
+          for (int j = 0; j < kDlParts; ++j) t[j] += __ldcg(a.partS + static_cast<int64_t>(b) * PS + NS + j);
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1)
+#pragma unroll
+          for (int j = 0; j < kDlParts; ++j) t[j] += __shfl_xor_sync(0xffffffffu, t[j], o);
+        if (lane == 0) {
+          for (int j = 0; j < kDlParts; ++j) t[j] += dl_s[j];
+          ctl->dl_g2 = t[kDlG2];
+          ctl->dl_alpha = t[kDlG2] / t[kDlUHu];
+          ctl->dl_gn2 = t[kDlGn2];
+          ctl->dl_b = t[kDlB];
+          ctl->dl_ok = sc[kScNotPD] > 0.0 ? 0 : 1;
+          double cg, cn;
+          ctl->dl_step_norm = dogleg_point(ctl->radius, ctl->dl_alpha, ctl->dl_g2, ctl->dl_gn2, ctl->dl_b, &cg, &cn);
+          if (!ctl->dl_ok) cg = cn = 0.0;
+          // step.g = cg |g~|^2 + cn g~.gn;  step.H.step = cg^2 u.Hu + 2 cg cn u.Hx + cn^2 x.Hx
+          ctl->dl_model_change = -(cg * t[kDlG2] + cn * t[kDlB]) -
+                                 0.5 * (cg * cg * t[kDlUHu] + 2.0 * cg * cn * t[kDlUHx] + cn * cn * t[kDlXHx]);
+          dl_s[6] = cg;
+          dl_s[7] = cn;
+        }
+      }
+      __syncthreads();
+      for (int i = tid; i < G; i += nthreads) {  // the globals' step (cg g~ + cn gn) / D replaces x_g
+        const double v = ctl->dl_ok ? (dl_s[6] * dl_gt[i] + dl_s[7] * (dg[i] * dl_D[i])) / dl_D[i] : 0.0;
+        dg[i] = v;
+        if (bid == 0) a.delta[nfp + i] = v;
+      }
+      __syncthreads();
+    }
+
     // ------------------------------------------------------------ U: back-substitution, trial states
+    // (DOGLEG: the dogleg step in place of the back-substitution)
     double ustat[4] = {0.0, 0.0, 0.0, 0.0};  // lane 0 of each warp: kScDotG .. kScXnorm2
     {
       if (warp == nwarps - 1) {  // trial camera states (every CTA needs them; the last warp is the one most likely
@@ -497,7 +663,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           }
           for (int q = 0; q < kImuStateSize; ++q) x_new[a.dp.off_imu + q] = x_cur[a.dp.off_imu + q];
           for (int q = 0; q < G; ++q) {
-            const double d2 = global_damp(q, Ccur[q * G + q], scg[q], rinv, nullptr, 0);
+            const double d2 = global_damp(q, Ccur[q * G + q], scg[q], dmul, nullptr, 0);
             ustat[0] += dg[q] * Ccur[G * G + q] * scg[q];
             ustat[1] += dg[q] * dg[q] * d2;
           }
@@ -505,20 +671,33 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       }
       for (int k = warp; k < nk; k += nwarps) {
         const int f = bid + k * nb;
-        const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
         double d[FD];
+        if constexpr (kDl) {  // (cg g~ + cn gn) / D from U1's x_f (in delta)
+          const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+          const double* Bf = bc.B + static_cast<int64_t>(f) * FD * FD;
+          const double* gf = bc.gf + static_cast<int64_t>(f) * FD;
 #pragma unroll
-        for (int r = 0; r < FD; ++r) {
-          double s = 0.0;
-          for (int c = lane; c < G; c += 32) s += Xf[r * M + c] * dg[c];
+          for (int r = 0; r < FD; ++r) {
+            const double D = sqrt(dl_clamp(Bf[r * FD + r], sf[r]));
+            const double gt = gf[r] * sf[r] / D;
+            d[r] = ctl->dl_ok ? (dl_s[6] * gt + dl_s[7] * (a.delta[static_cast<int64_t>(f) * FD + r] * D)) / D : 0.0;
+          }
+        } else {
+          const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
 #pragma unroll
-          for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-          d[r] = -Xf[r * M + G] - s;
+          for (int r = 0; r < FD; ++r) {
+            double s = 0.0;
+            for (int c = lane; c < G; c += 32) s += Xf[r * M + c] * dg[c];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            d[r] = -Xf[r * M + G] - s;
+          }
         }
+        if constexpr (kDl) __syncwarp();  // every lane has read x_f before lane 0 overwrites it
         if (lane == 0) {
 #pragma unroll
           for (int r = 0; r < FD; ++r) a.delta[static_cast<int64_t>(f) * FD + r] = d[r];
-          frame_plus<FD>(a.dp, bc, a.scale, rinv, nullptr, nullptr, f, d, a.frame_used[f] != 0, x_cur, x_new, ustat);
+          frame_plus<FD>(a.dp, bc, a.scale, dmul, nullptr, nullptr, f, d, a.frame_used[f] != 0, x_cur, x_new, ustat);
         }
       }
       for (int e = tid; e < nwarps * NP; e += nthreads) Cw[e] = 0.0;
@@ -643,7 +822,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
           for (int q = 0; q < kScNotPD; ++q) t[q] = totc[NP + q];
           t[kScGnorm2] += g2;
           t[kScGmax] = fmax(t[kScGmax], gm);
-          finish_scalars(ctl, sc, bid == 0 ? bt.cost : nullptr, t, true, 1);
+          finish_scalars<Str>(ctl, sc, bid == 0 ? bt.cost : nullptr, t, true, 1);
           if (bid == 0) {
             if (ctl->done) atomicOr(ctlw + 2, 1ull);
             *a.ctl = *ctl;

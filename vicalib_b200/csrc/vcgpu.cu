@@ -442,24 +442,42 @@ static int device_attrs(vcgpu_handle* h) {
   return VCGPU_OK;
 }
 
-// persistent vision kernel: pick the team count that fits shared memory, allocate the partial slots
+// persistent vision kernel: pick the team count that fits shared memory, allocate the partial slots.  Each instantiation
+// (LM, and DOGLEG with its three extra G-vectors) gets its own team count, shared-memory attribute and occupancy check,
+// since the strategy may change between solves without a new prepare().
+template <vc::Strategy S>
+static int mega_fit(vcgpu_handle* h, int* warps_out) {
+  const DevProblem& dp = h->dp;
+  const int st = S == vc::Strategy::kDogleg ? 1 : 0;
+  *warps_out = 0;
+  // the dynamic request and the kernel's static shared memory (the group table) share the per-block opt-in
+  cudaFuncAttributes fa{};
+  CUDA_TRY(h, cudaFuncGetAttributes(&fa, vc::lm_mega_kernel<S>));
+  const size_t avail = static_cast<size_t>(h->dev_smem_optin) - fa.sharedSizeBytes;
+  int warps = vc::kMegaMaxWarps;
+  while (warps > 0 && vc::mega_smem_doubles(dp.G, dp.n_cams, warps, st) * sizeof(double) > avail) --warps;
+  if (warps == 0 || 12 * (dp.G + 1) > vc::kWarpDoubles) return VCGPU_OK;
+  const size_t smem = vc::mega_smem_doubles(dp.G, dp.n_cams, warps, st) * sizeof(double);
+  if (smem > h->mega_smem_set[st]) {
+    CUDA_TRY(h, cudaFuncSetAttribute(vc::lm_mega_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+    int per_sm = 0;
+    CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vc::lm_mega_kernel<S>, 32 * warps, smem));
+    if (per_sm < 1) return VCGPU_OK;
+    h->mega_smem_set[st] = smem;
+  }
+  *warps_out = warps;
+  return VCGPU_OK;
+}
 static int mega_prepare(vcgpu_handle* h) {
   const DevProblem& dp = h->dp;
-  h->mega_warps = 0;
+  h->mega_warps[0] = h->mega_warps[1] = 0;
   if (dp.inertial || (h->nranks > 1 && !h->xchg_ready)) return VCGPU_OK;
   VC_TRY(device_attrs(h));
   if (h->dev_smem_optin == 0) return VCGPU_OK;
-  int warps = vc::kMegaMaxWarps;
-  while (warps > 0 && vc::mega_smem_doubles(dp.G, dp.n_cams, warps) * sizeof(double) > static_cast<size_t>(h->dev_smem_optin)) --warps;
-  if (warps == 0 || 12 * (dp.G + 1) > vc::kWarpDoubles) return VCGPU_OK;
-  const size_t smem = vc::mega_smem_doubles(dp.G, dp.n_cams, warps) * sizeof(double);
-  if (smem > h->mega_smem_set) {
-    CUDA_TRY(h, cudaFuncSetAttribute(vc::lm_mega_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    int per_sm = 0;
-    CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vc::lm_mega_kernel, 32 * warps, smem));
-    if (per_sm < 1) return VCGPU_OK;
-    h->mega_smem_set = smem;
-  }
+  int warps[2];
+  VC_TRY(mega_fit<vc::Strategy::kLM>(h, &warps[0]));
+  VC_TRY(mega_fit<vc::Strategy::kDogleg>(h, &warps[1]));
+  if (warps[0] == 0 && warps[1] == 0) return VCGPU_OK;
   const size_t PS = static_cast<size_t>(dp.G) * dp.G + dp.G + vc::kMegaPartExtra;
   const size_t PC = static_cast<size_t>(dp.n_cams) * vc::kCgStride + vc::kMegaPartExtra;
   if (PS > 32768 || 4 * h->nranks * PS > static_cast<size_t>(vc::kXchgCOff) ||
@@ -473,7 +491,8 @@ static int mega_prepare(vcgpu_handle* h) {
     h->xchg_peer[0] = h->xchg_local;
   }
   h->mega_grid = h->dev_sms;
-  h->mega_warps = warps;
+  h->mega_warps[0] = warps[0];
+  h->mega_warps[1] = warps[1];
   VC_TRY(dev_alloc(h, &h->d_partS, h->mega_grid * PS));
   VC_TRY(dev_alloc(h, &h->d_partC, h->mega_grid * PC));
   CUDA_TRY(h, cudaMemsetAsync(h->d_partS, 0, h->mega_grid * PS * sizeof(double), h->stream));
