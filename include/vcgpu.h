@@ -136,6 +136,26 @@ int vcgpu_register_mirrors(vcgpu_handle* h, double* intr, double* q_ck, double* 
 /* ---- the hot path ---------------------------------------------------------------------- */
 /* ceres::Solve(solver_options_, problem_, &summary)  (vicalibrator.h:956) */
 int vcgpu_solve(vcgpu_handle* h, vcgpu_iter_cb cb, void* user, vcgpu_summary* out);
+/* vcgpu_solve of n handles in one call, free-running (no callback; the host mirrors are written once, at the end).
+ * Every rig runs inside its own thread-block cluster of 1, 2, 4 or 8 CTAs (the fewest whose warps hold the rig's
+ * frames), so many small rigs share the GPU instead of taking it in turns; rigs of the same strategy, cluster size
+ * and warp count go into ONE kernel launch.  Each handle's own options (strategy, tolerances, max_iters,
+ * jacobi_scaling, init_radius) and flags apply to it, each rig stops on its own, and its result equals its
+ * vcgpu_solve to rounding and does not depend, bit for bit, on what else is in the batch or in which order.
+ * out: n summaries or NULL.  device_seconds is the CUDA-event time of the launch the rig ran in (shared by the rigs
+ * of that launch); kernel_launches counts the rig's own start-point launches plus that one.
+ * Returns VCGPU_ERR_INVALID before anything is launched, with a message naming the index in vcgpu_last_error of every
+ * non-null handle of the batch, for: n <= 0, a null or repeated handle, handles on different devices, and a handle
+ * that has inertial terms on, frame shards, a vcgpu_set_profiling bit (1, 2, 4) or L2 flushing set,
+ * update_state_every_iteration set, no active observation, or a rig too large for the persistent vision kernel.
+ * There is no sequential fallback: call vcgpu_solve on such a handle.  A refused batch leaves its handles as they were.
+ * Device memory: nothing beyond what each handle holds for vcgpu_solve, which includes a 32 MiB totals buffer per
+ * handle (so n handles hold n x 32 MiB plus their problems), and n x ~1 KB of kernel arguments. */
+int vcgpu_solve_batch(vcgpu_handle* const* handles, int n, vcgpu_summary* out /* n, or NULL */);
+/* how vcgpu_solve_batch would run this handle: CTAs per cluster (1, 2, 4 or 8), warps per CTA, and how many clusters
+ * of that shape the device holds at once (cudaOccupancyMaxActiveClusters; further rigs of a batch queue behind them).
+ * Any pointer may be NULL.  VCGPU_ERR_INVALID where the batch would refuse the handle's rig. */
+int vcgpu_batch_plan(vcgpu_handle* h, int* cluster_size, int* warps, int* resident_clusters);
 /* run exactly n trust-region iterations with no convergence test and no host round trip per
  * iteration (benchmark entry: LM iterations / second) */
 int vcgpu_iterate(vcgpu_handle* h, int n_iterations, vcgpu_summary* out);

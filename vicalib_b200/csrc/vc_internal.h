@@ -12,6 +12,7 @@
 
 namespace vc {
 
+struct MegaArgs;  // vc_mega.cuh
 constexpr int kMaxCams = 8;
 constexpr int kCamStateStride = 17;  // q_ck(4) p_ck(3) intr(10)
 constexpr int kImuStateSize = 15;    // g2 b6 sf6 ts1
@@ -184,8 +185,8 @@ struct vcgpu_handle {
   double *d_partS = nullptr, *d_partC = nullptr;  // [grid][G*G+G+8] / [grid][n_cams*kCgStride+8]
   unsigned long long* d_prof = nullptr;
   int dev_sms = 0, dev_smem_optin = 0;
-  size_t mega_smem_set[2] = {0, 0};  // per instantiation of lm_mega_kernel ([strategy]: 0 LM, 1 DOGLEG)
-  int mega_grid = 0, mega_warps[2] = {0, 0};  // 0 warps: does not fit / not supported, use the multi-launch engine
+  int mega_grid = 0, mega_warps[2] = {0, 0};  // [strategy]; 0 warps: does not fit / not supported, use the multi-launch engine
+  vc::MegaArgs* d_batch_args = nullptr;  // vcgpu_solve_batch: the rigs of a launch group (held by the group's first handle)
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)
   bool imu_mega_ok = false;
   int imu_mega_grid = 0;

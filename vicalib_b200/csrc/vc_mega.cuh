@@ -1,7 +1,9 @@
 // Persistent trust-region kernel for the vision-only problem (one GPU, or frame shards on several).
 //
 // One cooperative launch runs up to n_iters trust-region iterations, Levenberg-Marquardt or (one GPU) DOGLEG: the kernel
-// is instantiated per strategy (Strategy::kLM, kDogleg).  One CTA per SM, every
+// is instantiated per strategy (Strategy::kLM, kDogleg).  The loop itself (mega_solve) is written against a scope — the
+// CTAs that share the rig and their barrier: the cooperative grid here (lm_mega_kernel), or one thread-block cluster per
+// rig in lm_mega_batch_kernel, which solves many rigs in one launch ("grid" below: the scope).  One CTA per SM, every
 // frame owned by the same WARP of the same CTA for the whole solve (frame f -> CTA f mod grid, warp
 // (f / grid) mod warps).  An iteration is a chain of per-frame warp phases and small every-CTA phases,
 // separated by grid barriers instead of launches:
@@ -241,15 +243,35 @@ __device__ inline void mega_chol_solve_smem(double* S, int G, int lane, double* 
   }
 }
 
-template <Strategy Str>
-__global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a) {
+// The CTAs that share one rig's solve.  A scope supplies what the solve loop needs from "the grid": this CTA's index
+// among them, their count, and a barrier over them that orders their global-memory writes.
+//   GridScope: the whole cooperative grid (lm_mega_kernel: one rig per launch; frame shards allowed).
+//   ClusterScope: one thread-block cluster (lm_mega_batch_kernel: one rig per cluster, many clusters per launch, none
+//   of which ever waits for another).  Never sharded, so mega_publish / mega_total are not instantiated for it.
+struct GridScope {
+  static constexpr bool kSharded = true;
+  cg::grid_group g = cg::this_grid();
+  __device__ __forceinline__ int bid() const { return blockIdx.x; }
+  __device__ __forceinline__ int nb() const { return gridDim.x; }
+  __device__ __forceinline__ void sync() { g.sync(); }
+};
+struct ClusterScope {
+  static constexpr bool kSharded = false;
+  cg::cluster_group c = cg::this_cluster();
+  __device__ __forceinline__ int bid() const { return static_cast<int>(c.block_rank()); }
+  __device__ __forceinline__ int nb() const { return static_cast<int>(c.num_blocks()); }
+  __device__ __forceinline__ void sync() { c.sync(); }  // barrier.cluster.arrive.release + wait.acquire
+};
+
+// The solve loop: up to a.n_iters trust-region iterations of strategy Str on the rig `a`, by the CTAs of `scope`.
+template <Strategy Str, class Scope>
+__device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
   constexpr bool kDl = Str == Strategy::kDogleg;
   extern __shared__ double smem[];
-  cg::grid_group grid = cg::this_grid();
   constexpr int FD = 6;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int nthreads = blockDim.x, nwarps = nthreads >> 5;
-  const int bid = blockIdx.x, nb = gridDim.x;
+  const int bid = scope.bid(), nb = scope.nb();
   const int n_cams = a.dp.n_cams;
   const int G = a.dp.G, M = G + 1, NS = G * G + G, PS = NS + kMegaPartExtra, nf = a.dp.n_frames;
   const int NP = n_cams * kCgStride, PC = NP + kMegaPartExtra;  // packed camera blocks
@@ -304,7 +326,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
     const int g = a.group_of[c * nf + bid + k * nb];
     return g < 0 ? make_int2(0, 0) : make_int2(a.grp_start[g], a.grp_count[g]);
   };
-  const bool sharded = a.nranks > 1;
+  const bool sharded = Scope::kSharded && a.nranks > 1;
   unsigned epS = static_cast<unsigned>(ctlw[0]), epC = static_cast<unsigned>(ctlw[1]);  // same on every CTA of every rank
   unsigned long long t_prev = 0;
   const bool prof = a.prof != nullptr && bid == 0 && tid == 0;
@@ -437,7 +459,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       }
     }
     mark(kProfS);
-    grid.sync();
+    scope.sync();
     if (tid == 0) exit_s = *reinterpret_cast<volatile unsigned long long*>(ctlw + 2);
     __syncthreads();
     if (exit_s) break;
@@ -453,13 +475,15 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       if (sharded) {
         // every rank's CTA sums go to every rank (tagged words over NVLink); ONE thread of this grid per entry waits for
         // them and adds them up in rank order (every rank computes the same bits)
-        mega_publish(a.partS, PS, nb, PS, a, 0, parS, epS, NS + kScNotPD, -1);
-        for (int e = bid * nthreads + tid; e < PS; e += nb * nthreads) totS[e] = mega_total(a, 0, PS, parS, epS, e, e == NS + kScNotPD);
+        if constexpr (Scope::kSharded) {
+          mega_publish(a.partS, PS, nb, PS, a, 0, parS, epS, NS + kScNotPD, -1);
+          for (int e = bid * nthreads + tid; e < PS; e += nb * nthreads) totS[e] = mega_total(a, 0, PS, parS, epS, e, e == NS + kScNotPD);
+        }
       } else {
-        mega_reduce_stage1(a.partS, PS, nb, PS, totS, NS + kScNotPD, -1);
+        mega_reduce_stage1(a.partS, PS, nb, PS, totS, NS + kScNotPD, -1, bid, nb);
       }
       mark(kProfG);
-      grid.sync();
+      scope.sync();
       mark(kProfSync);
       for (int e = tid; e < NS; e += nthreads) {
         if (e < G * G && e % G > e / G) continue;  // lower triangle only
@@ -599,7 +623,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
         }
       }
       mark(kProfU);
-      grid.sync();
+      scope.sync();
       mark(kProfSync);
       if (warp == 0) {  // every CTA adds up the CTA partials alike, then the dogleg point and the model change
         double t[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
@@ -762,7 +786,7 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       }
     }
     mark(kProfB);
-    grid.sync();
+    scope.sync();
     mark(kProfSync);
 
     // ------------------------------------------------------------ D: global block of the trial point, decision
@@ -772,14 +796,16 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       const int parC = static_cast<int>(epC & 1);
       double* totC = reinterpret_cast<double*>(a.xbuf[a.rank] + (sharded ? kXchgPlainC : kXchgCOff));
       if (sharded) {
-        mega_publish(a.partC, PC, nb, PC, a, kXchgCOff, parC, epC, NP + kScGmax, NP + kScNotPD);
-        for (int e = bid * nthreads + tid; e < PC; e += nb * nthreads)
-          totC[e] = mega_total(a, kXchgCOff, PC, parC, epC, e, e == NP + kScGmax || e == NP + kScNotPD);
+        if constexpr (Scope::kSharded) {
+          mega_publish(a.partC, PC, nb, PC, a, kXchgCOff, parC, epC, NP + kScGmax, NP + kScNotPD);
+          for (int e = bid * nthreads + tid; e < PC; e += nb * nthreads)
+            totC[e] = mega_total(a, kXchgCOff, PC, parC, epC, e, e == NP + kScGmax || e == NP + kScNotPD);
+        }
       } else {
-        mega_reduce_stage1(a.partC, PC, nb, PC, totC, NP + kScGmax, NP + kScNotPD);
+        mega_reduce_stage1(a.partC, PC, nb, PC, totC, NP + kScGmax, NP + kScNotPD, bid, nb);
       }
       mark(kProfD);
-      grid.sync();
+      scope.sync();
       mark(kProfSync);
       for (int e = tid; e < PC; e += nthreads) totc[e] = __ldcg(totC + e);
       __syncthreads();
@@ -849,6 +875,26 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a)
       else bf.gc[e - G * G] = Cf[e];
     }
   }
+}
+
+// One rig on the whole cooperative grid.
+template <Strategy Str>
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_kernel(MegaArgs a) {
+  mega_solve<Str>(a, GridScope());
+}
+
+// A batch of rigs, one thread-block cluster each (launched with a cluster dimension; no cooperative launch): cluster k
+// solves args[k].  The clusters share nothing and leave on their own rig's exit word.  The rig's arguments are staged in
+// shared memory once per CTA (the loop reads them all the time).
+template <Strategy Str>
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_batch_kernel(const MegaArgs* args) {
+  static_assert(sizeof(MegaArgs) % sizeof(unsigned long long) == 0, "MegaArgs is copied in 8-byte words");
+  __shared__ __align__(16) unsigned long long words[sizeof(MegaArgs) / sizeof(unsigned long long)];
+  ClusterScope scope;
+  const unsigned long long* src = reinterpret_cast<const unsigned long long*>(args + blockIdx.x / scope.nb());
+  for (int k = threadIdx.x; k < static_cast<int>(sizeof(MegaArgs) / sizeof(unsigned long long)); k += blockDim.x) words[k] = src[k];
+  __syncthreads();
+  mega_solve<Str>(*reinterpret_cast<const MegaArgs*>(words), scope);
 }
 
 }  // namespace vc

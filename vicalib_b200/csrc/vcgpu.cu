@@ -216,7 +216,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -442,6 +442,13 @@ static int device_attrs(vcgpu_handle* h) {
   return VCGPU_OK;
 }
 
+// The most warps per CTA (0: none) whose dynamic request fits `avail` bytes: what the per-block opt-in leaves beside the
+// static shared memory of the kernel that runs the loop (the group table; the batch kernel also stages its arguments)
+static int mega_warps_in(const DevProblem& dp, int st, size_t avail) {
+  int warps = vc::kMegaMaxWarps;
+  while (warps > 0 && vc::mega_smem_doubles(dp.G, dp.n_cams, warps, st) * sizeof(double) > avail) --warps;
+  return 12 * (dp.G + 1) > vc::kWarpDoubles ? 0 : warps;
+}
 // persistent vision kernel: pick the team count that fits shared memory, allocate the partial slots.  Each instantiation
 // (LM, and DOGLEG with its three extra G-vectors) gets its own team count, shared-memory attribute and occupancy check,
 // since the strategy may change between solves without a new prepare().
@@ -450,21 +457,18 @@ static int mega_fit(vcgpu_handle* h, int* warps_out) {
   const DevProblem& dp = h->dp;
   const int st = S == vc::Strategy::kDogleg ? 1 : 0;
   *warps_out = 0;
-  // the dynamic request and the kernel's static shared memory (the group table) share the per-block opt-in
   cudaFuncAttributes fa{};
   CUDA_TRY(h, cudaFuncGetAttributes(&fa, vc::lm_mega_kernel<S>));
-  const size_t avail = static_cast<size_t>(h->dev_smem_optin) - fa.sharedSizeBytes;
-  int warps = vc::kMegaMaxWarps;
-  while (warps > 0 && vc::mega_smem_doubles(dp.G, dp.n_cams, warps, st) * sizeof(double) > avail) --warps;
-  if (warps == 0 || 12 * (dp.G + 1) > vc::kWarpDoubles) return VCGPU_OK;
+  const int warps = mega_warps_in(dp, st, static_cast<size_t>(h->dev_smem_optin) - fa.sharedSizeBytes);
+  if (warps == 0) return VCGPU_OK;
   const size_t smem = vc::mega_smem_doubles(dp.G, dp.n_cams, warps, st) * sizeof(double);
-  if (smem > h->mega_smem_set[st]) {
+  // the opt-in belongs to the function, not to a handle: it is only ever raised, so that handles of different rigs
+  // (several may be live at once, and a batch prepares them all before any runs) keep each other's launches valid
+  if (smem > static_cast<size_t>(fa.maxDynamicSharedSizeBytes))
     CUDA_TRY(h, cudaFuncSetAttribute(vc::lm_mega_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-    int per_sm = 0;
-    CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vc::lm_mega_kernel<S>, 32 * warps, smem));
-    if (per_sm < 1) return VCGPU_OK;
-    h->mega_smem_set[st] = smem;
-  }
+  int per_sm = 0;
+  CUDA_TRY(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, vc::lm_mega_kernel<S>, 32 * warps, smem));
+  if (per_sm < 1) return VCGPU_OK;
   *warps_out = warps;
   return VCGPU_OK;
 }
@@ -745,6 +749,14 @@ static int prepare(vcgpu_handle* h) {
 extern "C" int vcgpu_solve(vcgpu_handle* h, vcgpu_iter_cb cb, void* user, vcgpu_summary* out) {
   if (!h) return VCGPU_ERR_INVALID;
   return run_solve(h, cb, user, out, 0);
+}
+extern "C" int vcgpu_solve_batch(vcgpu_handle* const* handles, int n, vcgpu_summary* out) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  return run_solve_batch(handles, n, out);
+}
+extern "C" int vcgpu_batch_plan(vcgpu_handle* h, int* cluster_size, int* warps, int* resident_clusters) {
+  if (!h) return VCGPU_ERR_INVALID;
+  return batch_plan_of(h, cluster_size, warps, resident_clusters);
 }
 extern "C" int vcgpu_iterate(vcgpu_handle* h, int n, vcgpu_summary* out) {
   if (!h || n <= 0) return VCGPU_ERR_INVALID;
