@@ -191,10 +191,13 @@ def gravity_vec(g):
 
 
 def get_range(t, w, a, ts, t0, t1):
-    """[interp(t0), samples with t0 < t_i + ts <= t1, interp(t1)] (interpolation-buffer.h:208-226)."""
+    """[interp(t0), samples with t0 < t_i + ts <= t1, interp(t1)] (interpolation-buffer.h:208-226).  A time at or past
+    the last sample gives that sample, at its own time (GetElement's end-of-buffer clamp)."""
     tt = [x + ts for x in t]
 
     def interp(time):
+        if time >= tt[-1]:
+            return (tt[-1], w[-1], a[-1])
         i = max(k for k in range(len(tt)) if tt[k] <= time)
         f = (time - tt[i]) / (tt[i + 1] - tt[i])
         return (time, w[i] * (1 - f) + w[i + 1] * f, a[i] * (1 - f) + a[i + 1] * f)
@@ -261,11 +264,19 @@ def imu_kat(rng):
     g = np.array([0.05, -0.03]); b = np.concatenate([rng.normal(0, 1e-2, 3), rng.normal(0, 1e-1, 3)])
     sf = 1 + 0.02 * rng.normal(size=6); ts = 0.0023
     W = 500 * np.eye(9) + 20 * rng.normal(size=(9, 9))
+    out_r, out_J = imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, (0, 1))
+    return dict(imu_t=t, imu_w=w, imu_a=a, ftime=ftime, T_wp=np.concatenate([q, p], 1), v_w=v, g=g, b=b, sf=sf, ts=np.array(ts),
+                W=W, r=np.array(out_r).reshape(2, nf - 1, 9), J=np.array(out_J).reshape(2, nf - 1, 9, 33))
+
+
+def imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, switches):
+    """residual and exact central-difference 9 x 33 Jacobian of every interval, for each switch value"""
+    nf = len(ftime)
     tm, wm, am = [mp.mpf(float(x)) for x in t], [V(x) for x in w], [V(x) for x in a]
     Wm = M(W)
     h = mp.mpf(10) ** -25
     out_r, out_J = [], []
-    for sw in (0, 1):
+    for sw in switches:
         for k in range(nf - 1):
             base = dict(R2=quat_R(q[k + 1]), p2=V(p[k + 1]), v2=V(v[k + 1]), R1=quat_R(q[k]), p1=V(p[k]), v1=V(v[k]),
                         g=[mp.mpf(float(x)) for x in g], b=[mp.mpf(float(x)) for x in b], sf=[mp.mpf(float(x)) for x in sf],
@@ -304,8 +315,48 @@ def imu_kat(rng):
             fd({"ts": base["ts"] + h}, {"ts": base["ts"] - h})
             out_r.append([float(x) for x in r0])
             out_J.append(np.array(cols).T)
-    return dict(imu_t=t, imu_w=w, imu_a=a, ftime=ftime, T_wp=np.concatenate([q, p], 1), v_w=v, g=g, b=b, sf=sf, ts=np.array(ts),
-                W=W, r=np.array(out_r).reshape(2, nf - 1, 9), J=np.array(out_J).reshape(2, nf - 1, 9, 33))
+    return out_r, out_J
+
+
+# time unit of the edge stream: sample times, frame times and ts are multiples of U / 4, so every t_i + ts is exact in
+# binary64 and in mpmath alike, and a tie is a tie in both
+U = 1.0 / 1024
+EDGE_SAMPLES = [0, 3, 5, 9, 10, 14, 20, 21, 27, 30, 38, 41, 44, 52, 55, 60, 61, 70]  # t_i = (100 + k) U
+EDGE_TS = 3 * U
+# interval 0 [108, 117]      a sample on each end (ties at start and end: zero-length RK4 steps)
+# interval 1 [117, 118.25]   starts on a tie, no interior sample
+# interval 2 [118.25, 122.5] no interior sample, two interpolated ends
+# interval 3 [122.5, 130.5]  the sample at 130 U is inside at ts = 0 and pushed past the end (133 U) by ts
+# interval 4 [130.5, 150.25] ordinary
+# interval 5 [150.25, 180]   ends past the last sample (173 U): the end-of-buffer clamp
+EDGE_FTIME = [108, 117, 118.25, 122.5, 130.5, 150.25, 180]
+
+
+def imu_edge_kat():
+    """The interpolation buffer's edges on an irregular stream (tests/golden/imu_edge_kat.npz, keys of imu_kat.npz with
+    one switch value, 0)."""
+    from vicalib_b200.synth import so3_exp as np_exp
+    rng = np.random.default_rng(20261016)
+    t = (100 + np.array(EDGE_SAMPLES, dtype=np.float64)) * U
+    n = len(t)
+    w = rng.normal(0, 0.4, (n, 3)); a = rng.normal(0, 1.0, (n, 3)) + np.array([0.3, 9.7, 0.5])
+    ftime = np.array(EDGE_FTIME) * U
+    nf = len(ftime)
+    tt = t + EDGE_TS
+    assert tt[EDGE_SAMPLES.index(5)] == ftime[0] and tt[EDGE_SAMPLES.index(14)] == ftime[1]  # the ties, in binary64
+    for k in (1, 2):
+        assert not np.any((tt > ftime[k]) & (tt < ftime[k + 1]))  # no interior sample
+    j = EDGE_SAMPLES.index(30)
+    assert ftime[3] < t[j] < ftime[4] < tt[j]  # moved across the end by ts
+    assert ftime[-1] > tt[-1] and ftime[-2] < tt[-1]  # the last interval ends past the last sample
+    q = np.stack([np_exp(rng.normal(0, 0.5, 3)) for _ in range(nf)])
+    p = rng.normal(0, 0.3, (nf, 3)); v = rng.normal(0, 0.5, (nf, 3))
+    g = np.array([0.05, -0.03]); b = np.concatenate([rng.normal(0, 1e-2, 3), rng.normal(0, 1e-1, 3)])
+    sf = 1 + 0.02 * rng.normal(size=6)
+    W = 500 * np.eye(9) + 20 * rng.normal(size=(9, 9))
+    out_r, out_J = imu_rows(t, w, a, ftime, q, p, v, g, b, sf, EDGE_TS, W, (0,))
+    return dict(imu_t=t, imu_w=w, imu_a=a, ftime=ftime, T_wp=np.concatenate([q, p], 1), v_w=v, g=g, b=b, sf=sf,
+                ts=np.array(EDGE_TS), W=W, r=np.array(out_r).reshape(1, nf - 1, 9), J=np.array(out_J).reshape(1, nf - 1, 9, 33))
 
 
 def edge_kat():
@@ -336,6 +387,9 @@ def edge_kat():
 if __name__ == "__main__":
     if "--edge" in sys.argv:  # only the branch / boundary fixture (the others are unchanged)
         edge_kat()
+        sys.exit(0)
+    if "--imu-edge" in sys.argv:  # only the interpolation-buffer edge fixture (the others are unchanged)
+        np.savez_compressed(os.path.join(HERE, "imu_edge_kat.npz"), **imu_edge_kat())
         sys.exit(0)
     rng = np.random.default_rng(20260924)
     out = {}
