@@ -1,0 +1,52 @@
+"""What the vision solve engines compute, in a form two builds of the library can be compared by.
+
+    python tools/solve_digest.py [workload] [out.npz]
+
+Solves the workload (default config2) with LM and DOGLEG on the persistent kernel and on the multi-launch engine
+(vcgpu_set_profiling's multi-launch bit), and 8 rigs of config 1's shape with one vcgpu_solve_batch per strategy.  Prints,
+per case, the iterations, the final cost and last trust-region radius as hex floats and a SHA-256 of the final state;
+with out.npz also stores the states, costs and radii.  Equal lines mean bit-for-bit equal results.
+"""
+import hashlib
+import os
+import sys
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from vicalib_b200 import synth
+from vicalib_b200.capi import Calibrator, solve_batch
+
+wl = sys.argv[1] if len(sys.argv) > 1 else "config2"
+KEYS = ("intr", "q_ck", "p_ck", "T_wp")
+out = {}
+
+
+def report(name, g, s, radius):
+    x = np.concatenate([g.state()[k].ravel() for k in KEYS])
+    out[name] = np.concatenate([x, [s["final_cost"], radius]])
+    print(f"{name:24s} {s['iterations']:3d} it  cost {float(s['final_cost']).hex():24s} radius {float(radius).hex():24s} "
+          f"state {hashlib.sha256(x.tobytes()).hexdigest()[:16]}")
+
+
+p = synth.make_config(wl)
+for strategy, sname in ((0, "LM"), (1, "DOGLEG")):
+    for mode, mname in ((0, "persistent"), (4, "multi-launch")):
+        g = Calibrator()
+        g.load(p)
+        g.set_options(strategy=strategy, max_iters=20, function_tol=0.0, gradient_tol=0.0, param_tol=0.0)
+        g.set_profiling(mode, False)
+        s = g.solve()
+        report(f"{sname} {mname}", g, s, s["rows"][-1][7])
+        g.close()
+    rigs = []
+    for i in range(8):
+        g = Calibrator()
+        g.load(synth.make_problem(models=("poly3",), n_frames=50, grid=(14, 10), seed=1000 + i))
+        g.set_options(strategy=strategy, max_iters=20, function_tol=0.0, gradient_tol=0.0, param_tol=0.0)
+        rigs.append(g)
+    for i, (g, s) in enumerate(zip(rigs, solve_batch(rigs))):
+        report(f"{sname} batch rig {i}", g, s, float("nan"))  # a batch solve reports no radius
+        g.close()
+if len(sys.argv) > 2:
+    np.savez(sys.argv[2], **out)

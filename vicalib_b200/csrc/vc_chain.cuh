@@ -290,43 +290,14 @@ __global__ void __launch_bounds__(kChainThreads, 4) chain_eliminate_kernel(ElimA
   for (int e = tid; e < NS; e += kChainThreads) out[e] = Sacc[e];
 }
 
-// sum of the per-CTA Schur partials (coalesced across entries)
+// sum of per-CTA partials (coalesced across entries), into out0 or, with `which` >= 0, into whichever of out0 / out1
+// belongs to the buffer `which` picks on the device ([C | gc] of the point being evaluated, contiguous in Blocks)
 // launch with 256 threads: 32 entries per CTA, 8 partial-slices per entry, fixed summation order
-__global__ void __launch_bounds__(256) sum_partials_kernel(const double* part, int n_part, int NS, double* out,
-                                                           const Ctl* ctl) {
+__global__ void __launch_bounds__(256) sum_partials_kernel(const double* part, int n_part, int NS, double* out0, double* out1,
+                                                           const Ctl* ctl, int which) {
   __shared__ double sh[8][33];
   if (ctl->done) return;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  const int e = blockIdx.x * 32 + tx;
-  double s = 0.0;
-  if (e < NS) {
-    double s1 = 0.0, s2 = 0.0, s3 = 0.0;
-    int b = ty;
-    for (; b + 24 < n_part; b += 32) {
-      s += part[static_cast<int64_t>(b) * NS + e];
-      s1 += part[static_cast<int64_t>(b + 8) * NS + e];
-      s2 += part[static_cast<int64_t>(b + 16) * NS + e];
-      s3 += part[static_cast<int64_t>(b + 24) * NS + e];
-    }
-    for (; b < n_part; b += 8) s += part[static_cast<int64_t>(b) * NS + e];
-    s = (s + s1) + (s2 + s3);
-  }
-  sh[ty][tx] = s;
-  __syncthreads();
-  if (ty == 0 && e < NS) {
-    double t = 0.0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) t += sh[k][tx];
-    out[e] = t;
-  }
-}
-
-// same sum, output selected on the device: [C | gc] of the buffer being evaluated (contiguous in Blocks)
-__global__ void __launch_bounds__(256) sum_partials_sel_kernel(const double* part, int n_part, int NS, double* out0,
-                                                               double* out1, const Ctl* ctl, int which) {
-  __shared__ double sh[8][33];
-  if (ctl->done) return;
-  double* out = (which ? 1 - ctl->cur : ctl->cur) ? out1 : out0;
+  double* out = which >= 0 && pick(ctl, which) ? out1 : out0;
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int e = blockIdx.x * 32 + tx;
   double s = 0.0;

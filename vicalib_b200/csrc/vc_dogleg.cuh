@@ -30,6 +30,11 @@ __device__ __forceinline__ double dl_clamp(double diag, double s) {
   const double c = diag * s * s;
   return c < 1e-6 ? 1e-6 : (c > 1e32 ? 1e32 : c);
 }
+// D and g~ = g / D of entry i of the scaled system (g: the unscaled gradient entry)
+__device__ __forceinline__ void dl_scaled(double diag, double g, double s, double* D, double* gt) {
+  *D = sqrt(dl_clamp(diag, s));
+  *gt = g * s / *D;
+}
 __global__ void dl_prep_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl* ctl, const double* scale, DlVecs v) {
   if (ctl->done) return;
   const Blocks& b = ctl->cur ? b1 : b0;
@@ -48,13 +53,12 @@ __global__ void dl_prep_kernel(DevProblem dp, Blocks b0, Blocks b1, const Ctl* c
     g = b.gc[k];
   }
   const double s = scale[i];
-  const double c = dl_clamp(d, s);
-  const double D = sqrt(c);
-  const double gt = g * s / D;
+  double D, gt;
+  dl_scaled(d, g, s, &D, &gt);
   v.diag[i] = D;
   v.grad[i] = gt;
   v.vec[i] = gt / D;
-  v.D2[i] = c * ctl->dl_mu;
+  v.D2[i] = dl_clamp(d, s) * ctl->dl_mu;
 }
 
 // ---------------------------------------------------------------- y = S H S v on the block-arrow system

@@ -549,7 +549,7 @@ __global__ void __launch_bounds__(256) reduce_finalize_kernel(RedFinArgs a) {
   if (tid == 0) finish_scalars(a.ctl, a.scalars, out.cost, t, a.step_part != nullptr, a.decide_mode);
 }
 
-// level 2 for large global blocks: C | gc were summed by sum_partials_sel_kernel; this one-CTA launch
+// level 2 for large global blocks: C | gc were summed by sum_partials_kernel; this one-CTA launch
 // finishes the scalars (fixed order) and decides
 __global__ void __launch_bounds__(256) finalize_small_kernel(RedFinArgs a, int nb) {
   __shared__ double shr[8][8];
@@ -674,9 +674,31 @@ struct SolveArgs {
 constexpr int kSolveThreads = 128;
 constexpr int kSolveWarps = kSolveThreads / 32;
 
+// The CTA's E^T X of the frames its first nact warps just staged (scaled [E | g] [FD][G + 1], then X_f [FD][G + 1];
+// stages `stride` doubles apart), added to Sacc: the lower triangle of [G][G], then the right-hand side [G].  Thread tid
+// of nthreads owns the same entries every time (deterministic).
+template <int FD>
+__device__ __forceinline__ void schur_accumulate(double* Sacc, const double* stages, int stride, int nact, int G, int tid,
+                                                 int nthreads) {
+  const int M = G + 1, NS = G * G + G;
+  for (int e = tid; e < NS; e += nthreads) {
+    const int ra = e < G * G ? e / G : e - G * G;
+    const int cb = e < G * G ? e - ra * G : G;
+    if (e < G * G && cb > ra) continue;  // lower triangle only
+    double sum = 0.0;
+    for (int w = 0; w < nact; ++w) {
+      const double* Ew = stages + static_cast<size_t>(w) * stride;
+      const double* Xv = Ew + FD * M;
+#pragma unroll
+      for (int q = 0; q < FD; ++q) sum += Ew[q * M + ra] * Xv[q * M + cb];
+    }
+    Sacc[e] += sum;
+  }
+}
+
 // One warp per frame: every lane factors the (damped, scaled) FD x FD block in registers and the
 // lanes split the right-hand-side columns [E | g]; the CTA then accumulates E^T X for its four
-// frames with a fixed thread->entry ownership (deterministic).
+// frames (schur_accumulate).
 template <int FD>
 __global__ void __launch_bounds__(kSolveThreads) frame_solve_kernel(SolveArgs a) {
   extern __shared__ double sm[];
@@ -760,23 +782,22 @@ __global__ void __launch_bounds__(kSolveThreads) frame_solve_kernel(SolveArgs a)
       }
     }
     __syncthreads();
-    const int nact = min(kSolveWarps, a.dp.n_frames - base);
-    for (int e = tid; e < NS; e += kSolveThreads) {
-      const int ra = e < G * G ? e / G : e - G * G;
-      const int cb = e < G * G ? e - ra * G : G;
-      double sum = 0.0;
-      for (int w = 0; w < nact; ++w) {
-        const double* Ew = sm + NS + w * (2 * FD * M);
-        const double* Xv = Ew + FD * M;
-#pragma unroll
-        for (int k = 0; k < FD; ++k) sum += Ew[k * M + ra] * Xv[k * M + cb];
-      }
-      Sacc[e] += sum;
-    }
+    schur_accumulate<FD>(Sacc, sm + NS, 2 * FD * M, min(kSolveWarps, a.dp.n_frames - base), G, tid, kSolveThreads);
   }
   __syncthreads();
   double* out = a.Spart + static_cast<int64_t>(blockIdx.x) * NS;
   for (int k = tid; k < NS; k += kSolveThreads) out[k] = Sacc[k];
+}
+
+// Entry e of the reduced (globals) system [S | rhs] = [S C S + D - sum E^T X | -S g_c + sum E^T x]: c is entry e of
+// [C | g_c], p of the summed Schur partials, sc the globals' scale (global_damp's arguments after it).
+__device__ __forceinline__ double reduced_system_entry(int e, int G, double c, double p, const double* sc, double rinv,
+                                                       const double* D2x, int64_t nfp) {
+  if (e >= G * G) return -c * sc[e - G * G] + p;
+  const int r = e / G, q = e - r * G;
+  double v = c * sc[r] * sc[q] - p;
+  if (r == q) v += global_damp(r, c, sc[r], rinv, D2x, nfp);
+  return v;
 }
 
 // ---------------------------------------------------------------- reduced dense solve
@@ -786,15 +807,12 @@ struct GlobalSolveArgs {
   const Ctl* ctl;
   const double* scale;
   const double* D2x;
-  const double* Ssum;  // [G*G+G] summed Schur partials (n_part == 0), or
-  const double* Spart; // [n_part][G*G+G] per-CTA partials summed here in fixed order
-  int n_part;
+  const double* Ssum;  // [G*G+G] summed Schur partials (lower triangle | right-hand side)
   double* delta;       // scaled step; globals written at delta[nf*fd ...]
   double* scalars;
 };
 __global__ void __launch_bounds__(256) global_solve_kernel(GlobalSolveArgs a) {
   extern __shared__ double sm[];
-  __shared__ double sh4[4][64];
   if (a.ctl->done) return;
   const Blocks& b = a.b[a.ctl->cur];
   const double rinv = 1.0 / a.ctl->radius;
@@ -805,41 +823,8 @@ __global__ void __launch_bounds__(256) global_solve_kernel(GlobalSolveArgs a) {
   if (tid == 0) bad = 0;
   const int64_t nfp = static_cast<int64_t>(a.dp.n_frames) * a.dp.fd;
   const double* sc = a.scale + nfp;
-  const int el = tid & 63, slice = tid >> 6;
-  for (int e0 = 0; e0 < NS; e0 += 64) {
-    const int e = e0 + el;
-    double p = 0.0;
-    if (a.n_part > 0) {
-      double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-      if (e < NS) {
-        int bb = slice;
-        for (; bb + 12 < a.n_part; bb += 16) {
-          s0 += a.Spart[static_cast<int64_t>(bb) * NS + e];
-          s1 += a.Spart[static_cast<int64_t>(bb + 4) * NS + e];
-          s2 += a.Spart[static_cast<int64_t>(bb + 8) * NS + e];
-          s3 += a.Spart[static_cast<int64_t>(bb + 12) * NS + e];
-        }
-        for (; bb < a.n_part; bb += 4) s0 += a.Spart[static_cast<int64_t>(bb) * NS + e];
-      }
-      sh4[slice][el] = (s0 + s1) + (s2 + s3);
-      __syncthreads();
-      p = (sh4[0][el] + sh4[1][el]) + (sh4[2][el] + sh4[3][el]);
-      __syncthreads();
-    } else if (e < NS) {
-      p = a.Ssum[e];
-    }
-    if (slice == 0 && e < NS) {
-      if (e < G * G) {
-        const int r = e / G, c = e - r * G;
-        double v = b.C[e] * sc[r] * sc[c] - p;
-        if (r == c) v += global_damp(r, b.C[e], sc[r], rinv, a.D2x, nfp);
-        S[e] = v;
-      } else {
-        const int r = e - G * G;
-        rhs[r] = -b.gc[r] * sc[r] + p;
-      }
-    }
-  }
+  for (int e = tid; e < NS; e += 256)  // (the strict upper triangle of S is never read)
+    S[e] = reduced_system_entry(e, G, e < G * G ? b.C[e] : b.gc[e - G * G], a.Ssum[e], sc, rinv, a.D2x, nfp);
   __syncthreads();
   for (int j = 0; j < G; ++j) {
     if (tid == 0) {
@@ -999,6 +984,21 @@ struct UpdateArgs {
 };
 constexpr int kUpdateWarps = 4;
 
+// One warp: a frame's back-substitution d = -x_f - X_f[:, :G] dg from Xf [FD][G + 1] (column G: x_f = (B_f + D_f)^-1 g_f)
+// and the globals' step dg; every lane gets d.
+template <int FD>
+__device__ __forceinline__ void frame_backsub(const double* Xf, const double* dg, int G, int lane, double* d) {
+  const int M = G + 1;
+#pragma unroll
+  for (int r = 0; r < FD; ++r) {
+    double s = 0.0;
+    for (int c = lane; c < G; c += 32) s += Xf[r * M + c] * dg[c];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    d[r] = -Xf[r * M + G] - s;
+  }
+}
+
 template <int FD>
 __global__ void __launch_bounds__(32 * kUpdateWarps) backsub_update_kernel(UpdateArgs a) {
   if (a.ctl->done) return;
@@ -1007,7 +1007,7 @@ __global__ void __launch_bounds__(32 * kUpdateWarps) backsub_update_kernel(Updat
   const double* x_cur = a.state[cur];
   double* x_new = a.state[1 - cur];
   const double rinv = 1.0 / a.ctl->radius;
-  const int G = a.dp.G, M = G + 1, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int G = a.dp.G, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int nf = a.dp.n_frames;
   const int64_t nfp = static_cast<int64_t>(nf) * FD;
   const double* dc = a.delta + nfp;
@@ -1017,15 +1017,7 @@ __global__ void __launch_bounds__(32 * kUpdateWarps) backsub_update_kernel(Updat
   if (f < nf) {
     double d[FD];
     if (a.X) {
-      const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
-#pragma unroll
-      for (int r = 0; r < FD; ++r) {
-        double s = 0.0;
-        for (int c = lane; c < G; c += 32) s += Xf[r * M + c] * dc[c];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-        d[r] = -Xf[r * M + G] - s;
-      }
+      frame_backsub<FD>(a.X + static_cast<int64_t>(f) * FD * (G + 1), dc, G, lane, d);
     } else {
 #pragma unroll
       for (int r = 0; r < FD; ++r) d[r] = a.delta[static_cast<int64_t>(f) * FD + r];

@@ -9,11 +9,12 @@
 // separated by grid barriers instead of launches:
 //
 //   S  per frame (warp):  L = chol(B_f + D_f),  X_f = (B_f + D_f)^-1 [E_f | g_f],  CTA partial of E^T X
+//      (schur_accumulate)
 //   -- grid barrier; every CTA leaves here, together, if CTA 0 published "stop" (or a peer timed out)
 //   R1 entry e of the Schur sum is added up over the CTAs by one warp of CTA (e mod grid) and published:
 //      one GPU: plain totals + grid barrier; shards: tagged words into every rank's buffer, readers poll
-//   G  every CTA, redundantly: reduced system C + D - sum E^T X, Cholesky, globals' step
-//   U  per frame (warp):  back-substitution, x (+) step, step statistics; trial camera states
+//   G  every CTA, redundantly: reduced system C + D - sum E^T X (reduced_system_entry), Cholesky, globals' step
+//   U  per frame (warp):  back-substitution (frame_backsub), x (+) step, step statistics; trial camera states
 //      DOGLEG: U1 per frame (warp): back-substitution x_f, CTA partials of the step scalars; one more grid barrier;
 //      every CTA sums them, takes the dogleg point (dogleg_point, vc_dogleg.cuh) and the model change; U2 as U with
 //      the dogleg step in place of x
@@ -26,7 +27,8 @@
 //      TrustRegionMinimizer (decide_step) on its own copy of Ctl
 //
 // Every CTA (of every rank) reads bit-identical totals, so all take the same decision and the loop needs
-// no broadcast; all sums run in a fixed order (deterministic).  Replaces the body of ceres::Solve
+// no broadcast; all sums run in a fixed order (deterministic).  The Schur accumulation, the reduced system's entries and the
+// back-substitution are vc_kernels.cuh's routines, shared with the multi-launch kernels.  Replaces the body of ceres::Solve
 // (vicalibrator.h:956) for the staged vision solves; the inertial path has its own persistent kernels
 // (vc_imu_mega.cuh, vc_imu_eval_mega.cuh), and frame-sharded DOGLEG runs the multi-launch engine (vc_engine.inl).
 //
@@ -106,6 +108,30 @@ __device__ __forceinline__ unsigned long long global_ns() {
   return t;
 }
 
+// Entry e's sum (is_max: maximum) over the nparts CTA partials part[b * stride + e], by the calling warp in a fixed
+// order; every lane gets it.
+__device__ __forceinline__ double partials_total(const double* part, int stride, int nparts, int e, bool is_max, int lane) {
+  const double* p = part + e;
+  double s0 = 0.0, s1 = 0.0;
+  int b = lane;
+  if (is_max) {
+    for (; b < nparts; b += 32) s0 = fmax(s0, __ldcg(p + static_cast<int64_t>(b) * stride));
+  } else {
+    for (; b + 32 < nparts; b += 64) {
+      s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
+      s1 += __ldcg(p + static_cast<int64_t>(b + 32) * stride);
+    }
+    if (b < nparts) s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
+    s0 += s1;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const double t = __shfl_xor_sync(0xffffffffu, s0, o);
+    s0 = is_max ? fmax(s0, t) : s0 + t;
+  }
+  return s0;
+}
+
 // Single GPU: entry e is added up over the CTAs by one warp of CTA (e mod grid) into tot[e]; a grid barrier
 // later every CTA reads tot[] (cheaper than polling tagged words when nobody is remote: no tag checks, no polling).
 // (bid of nb: the CTAs sharing the work — the whole grid unless the caller says otherwise)
@@ -113,26 +139,8 @@ __device__ inline void mega_reduce_stage1(const double* part, int stride, int np
                                           int bid = blockIdx.x, int nb = gridDim.x) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   for (int e = bid + warp * nb; e < n; e += nwarps * nb) {
-    const bool is_max = e == max_a || e == max_b;
-    const double* p = part + e;
-    double s0 = 0.0, s1 = 0.0;
-    int b = lane;
-    if (is_max) {
-      for (; b < nparts; b += 32) s0 = fmax(s0, __ldcg(p + static_cast<int64_t>(b) * stride));
-    } else {
-      for (; b + 32 < nparts; b += 64) {
-        s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
-        s1 += __ldcg(p + static_cast<int64_t>(b + 32) * stride);
-      }
-      if (b < nparts) s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
-      s0 += s1;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double t = __shfl_xor_sync(0xffffffffu, s0, o);
-      s0 = is_max ? fmax(s0, t) : s0 + t;
-    }
-    if (lane == 0) tot[e] = s0;
+    const double s = partials_total(part, stride, nparts, e, e == max_a || e == max_b, lane);
+    if (lane == 0) tot[e] = s;
   }
 }
 
@@ -143,25 +151,7 @@ __device__ inline void mega_publish(const double* part, int stride, int nparts, 
                                     unsigned tag, int max_a, int max_b) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
   for (int e = blockIdx.x + warp * gridDim.x; e < n; e += nwarps * gridDim.x) {
-    const bool is_max = e == max_a || e == max_b;
-    const double* p = part + e;
-    double s0 = 0.0, s1 = 0.0;
-    int b = lane;
-    if (is_max) {
-      for (; b < nparts; b += 32) s0 = fmax(s0, __ldcg(p + static_cast<int64_t>(b) * stride));
-    } else {
-      for (; b + 32 < nparts; b += 64) {
-        s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
-        s1 += __ldcg(p + static_cast<int64_t>(b + 32) * stride);
-      }
-      if (b < nparts) s0 += __ldcg(p + static_cast<int64_t>(b) * stride);
-      s0 += s1;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-      const double t = __shfl_xor_sync(0xffffffffu, s0, o);
-      s0 = is_max ? fmax(s0, t) : s0 + t;
-    }
+    const double s0 = partials_total(part, stride, nparts, e, e == max_a || e == max_b, lane);
     if (lane < a.nranks) {
       const unsigned long long bits = static_cast<unsigned long long>(__double_as_longlong(s0));
       const unsigned long long hi_tag = static_cast<unsigned long long>(tag) << 32;
@@ -431,20 +421,7 @@ __device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
           }
         }
         __syncthreads();
-        const int nact = min(nwarps, nk - base);
-        for (int e = tid; e < NS; e += nthreads) {
-          const int ra = e < G * G ? e / G : e - G * G;
-          const int cb = e < G * G ? e - ra * G : G;
-          if (e < G * G && cb > ra) continue;  // lower triangle only
-          double sum = 0.0;
-          for (int w = 0; w < nact; ++w) {
-            const double* Ew = wmem + static_cast<size_t>(w) * kWarpDoubles;
-            const double* Xv = Ew + FD * M;
-#pragma unroll
-            for (int q = 0; q < FD; ++q) sum += Ew[q * M + ra] * Xv[q * M + cb];
-          }
-          Sacc[e] += sum;
-        }
+        schur_accumulate<FD>(Sacc, wmem, kWarpDoubles, min(nwarps, nk - base), G, tid, nthreads);
       }
       __syncthreads();
       double* out = a.partS + static_cast<int64_t>(bid) * PS;
@@ -487,17 +464,7 @@ __device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
       mark(kProfSync);
       for (int e = tid; e < NS; e += nthreads) {
         if (e < G * G && e % G > e / G) continue;  // lower triangle only
-        const double p = __ldcg(totS + e);
-        if (e < G * G) {
-          const int r = e / G, c = e - r * G;
-          if (c > r) continue;
-          double v = Ccur[e] * scg[r] * scg[c] - p;
-          if (r == c) v += global_damp(r, Ccur[e], scg[r], dmul, nullptr, 0);
-          S[e] = v;
-        } else {
-          const int r = e - G * G;
-          S[e] = -Ccur[e] * scg[r] + p;
-        }
+        S[e] = reduced_system_entry(e, G, Ccur[e], __ldcg(totS + e), scg, dmul, nullptr, 0);
       }
       if (tid == 0) {
         sc[kScNotPD] = __ldcg(totS + NS + kScNotPD);
@@ -521,8 +488,8 @@ __device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
     // ------------------------------------------------------------ U1 (DOGLEG): Gauss-Newton step, step scalars
     if constexpr (kDl) {
       for (int i = tid; i < G; i += nthreads) {
-        const double D = sqrt(dl_clamp(Ccur[i * G + i], scg[i]));
-        const double gt = Ccur[G * G + i] * scg[i] / D;
+        double D, gt;
+        dl_scaled(Ccur[i * G + i], Ccur[G * G + i], scg[i], &D, &gt);
         dl_D[i] = D;
         dl_gt[i] = gt;
         dl_u[i] = gt / D;
@@ -584,8 +551,8 @@ __device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
           double u[FD], wu[FD], wx[FD];
 #pragma unroll
           for (int r = 0; r < FD; ++r) {
-            const double D = sqrt(dl_clamp(Bf[r * FD + r], sf[r]));
-            const double gt = gf[r] * sf[r] / D;
+            double D, gt;
+            dl_scaled(Bf[r * FD + r], gf[r], sf[r], &D, &gt);
             const double gn = x[r] * D;
             u[r] = gt / D;
             wu[r] = sf[r] * u[r];
@@ -702,20 +669,12 @@ __device__ __forceinline__ void mega_solve(const MegaArgs& a, Scope scope) {
           const double* gf = bc.gf + static_cast<int64_t>(f) * FD;
 #pragma unroll
           for (int r = 0; r < FD; ++r) {
-            const double D = sqrt(dl_clamp(Bf[r * FD + r], sf[r]));
-            const double gt = gf[r] * sf[r] / D;
+            double D, gt;
+            dl_scaled(Bf[r * FD + r], gf[r], sf[r], &D, &gt);
             d[r] = ctl->dl_ok ? (dl_s[6] * gt + dl_s[7] * (a.delta[static_cast<int64_t>(f) * FD + r] * D)) / D : 0.0;
           }
         } else {
-          const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
-#pragma unroll
-          for (int r = 0; r < FD; ++r) {
-            double s = 0.0;
-            for (int c = lane; c < G; c += 32) s += Xf[r * M + c] * dg[c];
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-            d[r] = -Xf[r * M + G] - s;
-          }
+          frame_backsub<FD>(a.X + static_cast<int64_t>(f) * FD * M, dg, G, lane, d);
         }
         if constexpr (kDl) __syncwarp();  // every lane has read x_f before lane 0 overwrites it
         if (lane == 0) {
