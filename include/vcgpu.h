@@ -156,6 +156,32 @@ int vcgpu_solve_batch(vcgpu_handle* const* handles, int n, vcgpu_summary* out /*
  * of that shape the device holds at once (cudaOccupancyMaxActiveClusters; further rigs of a batch queue behind them).
  * Any pointer may be NULL.  VCGPU_ERR_INVALID where the batch would refuse the handle's rig. */
 int vcgpu_batch_plan(vcgpu_handle* h, int* cluster_size, int* warps, int* resident_clusters);
+/* vcgpu_solve of n handles with inertial terms on, in one call, free-running (no callback; the host mirrors are written
+ * once, at the end).  Every rig runs inside its own thread-block cluster of 1, 2, 4 or 8 CTAs of the persistent
+ * inertial kernels (the fewest whose two elimination groups per CTA take the rig's level-0 chunks in one round), so
+ * many rigs share the GPU instead of taking it in turns.  An iteration is one solve launch and one evaluation launch
+ * per cluster size for the whole batch; the host reads every rig's control block between bursts of up to 4
+ * iterations.  Each handle's own options (max_iters, tolerances, jacobi_scaling, init_radius, update_imu_weights)
+ * and flags apply to it, each rig stops on its own, and its result equals its vcgpu_solve to rounding (the weights
+ * update runs in the evaluation launch, as with VCGPU_NO_DEFERRED_WEIGHTS) and does not depend, bit for bit, on what
+ * else is in the batch or in which order.  A vcgpu_solve after the batch gives the bits it gives on a fresh handle.
+ * out: n summaries or NULL.  device_seconds is the CUDA-event time of the batch's iteration loop (shared by all its
+ * rigs); kernel_launches counts the rig's own launches (Jacobi scale, weights updates) plus every batch launch it
+ * took part in: the start point's evaluation and two per iteration queued for it, the same count as vcgpu_solve's
+ * when every iteration runs.
+ * Returns VCGPU_ERR_INVALID before any kernel is launched, with a message naming the index in vcgpu_last_error of
+ * every non-null handle of the batch, for: n <= 0, a null or repeated handle, handles on different devices, and a
+ * handle without inertial terms (vision rigs: vcgpu_solve_batch), with strategy 1 (inertial DOGLEG runs on the
+ * multi-launch engine), frame shards, a vcgpu_set_profiling bit or L2 flushing set, update_state_every_iteration set,
+ * or a rig the persistent inertial kernels do not fit (G >= 68 on an H100).  There is no sequential fallback: call
+ * vcgpu_solve on such a handle.  A refused batch leaves its handles as they were.
+ * Device memory: nothing beyond what each handle holds for vcgpu_solve, and n x ~5 KB of kernel arguments held by
+ * handle 0. */
+int vcgpu_solve_batch_inertial(vcgpu_handle* const* handles, int n, vcgpu_summary* out /* n, or NULL */);
+/* how vcgpu_solve_batch_inertial would run this handle: CTAs per cluster (1, 2, 4 or 8) and how many clusters of that
+ * size the device holds at once (the smaller count of the solve and the evaluation kernel; further rigs of a batch
+ * queue behind them).  Any pointer may be NULL.  VCGPU_ERR_INVALID where the batch would refuse the handle. */
+int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int* resident_clusters);
 /* run exactly n trust-region iterations with no convergence test and no host round trip per
  * iteration (benchmark entry: LM iterations / second) */
 int vcgpu_iterate(vcgpu_handle* h, int n_iterations, vcgpu_summary* out);

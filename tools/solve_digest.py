@@ -3,9 +3,11 @@
     python tools/solve_digest.py [workload] [out.npz]
 
 Solves the workload (default config2) with LM and DOGLEG on the persistent kernel and on the multi-launch engine
-(vcgpu_set_profiling's multi-launch bit), and 8 rigs of config 1's shape with one vcgpu_solve_batch per strategy.  Prints,
-per case, the iterations, the final cost and last trust-region radius as hex floats and a SHA-256 of the final state;
-with out.npz also stores the states, costs and radii.  Equal lines mean bit-for-bit equal results.
+(vcgpu_set_profiling's multi-launch bit), and 8 rigs of config 1's shape with one vcgpu_solve_batch per strategy; then
+the inertial LM solve on the persistent inertial kernels: the target workload (weights held) and config3 with live
+weights.  Prints, per case, the iterations, the final cost and last trust-region radius as hex floats and a SHA-256 of
+the final state (inertial: with velocities, IMU parameters and the weights); with out.npz also stores the states, costs
+and radii.  Equal lines mean bit-for-bit equal results.
 """
 import hashlib
 import os
@@ -22,8 +24,9 @@ KEYS = ("intr", "q_ck", "p_ck", "T_wp")
 out = {}
 
 
-def report(name, g, s, radius):
-    x = np.concatenate([g.state()[k].ravel() for k in KEYS])
+def report(name, g, s, radius, keys=KEYS, extra=()):
+    st = g.state()
+    x = np.concatenate([np.ravel(st[k]) for k in keys] + [np.ravel(e) for e in extra])
     out[name] = np.concatenate([x, [s["final_cost"], radius]])
     print(f"{name:24s} {s['iterations']:3d} it  cost {float(s['final_cost']).hex():24s} radius {float(radius).hex():24s} "
           f"state {hashlib.sha256(x.tobytes()).hexdigest()[:16]}")
@@ -48,5 +51,15 @@ for strategy, sname in ((0, "LM"), (1, "DOGLEG")):
     for i, (g, s) in enumerate(zip(rigs, solve_batch(rigs))):
         report(f"{sname} batch rig {i}", g, s, float("nan"))  # a batch solve reports no radius
         g.close()
+IMU_KEYS = KEYS + ("v_w", "g", "b", "sf", "ts")
+for wl_imu, weights in (("target", 0), ("config3", 1)):
+    g = Calibrator()
+    g.load(synth.make_config(wl_imu))
+    g.set_flags(inertial=1, rotation_only=0, bias_active=1, scale_active=1, optimize_ts=1)
+    g.set_options(max_iters=10, function_tol=0.0, gradient_tol=0.0, param_tol=0.0, update_imu_weights=weights)
+    s = g.solve()
+    report(f"inertial LM {wl_imu}" + (" live weights" if weights else ""), g, s, s["rows"][-1][7], IMU_KEYS,
+           (g.imu_weights(),) if weights else ())
+    g.close()
 if len(sys.argv) > 2:
     np.savez(sys.argv[2], **out)

@@ -20,7 +20,7 @@ EXPORTS = [
     "vcgpu_create", "vcgpu_destroy", "vcgpu_last_error", "vcgpu_set_cameras", "vcgpu_set_frames",
     "vcgpu_set_observations", "vcgpu_set_imu", "vcgpu_set_imu_params", "vcgpu_set_flags",
     "vcgpu_set_options", "vcgpu_default_flags", "vcgpu_default_options", "vcgpu_register_mirrors",
-    "vcgpu_solve", "vcgpu_solve_batch", "vcgpu_batch_plan", "vcgpu_iterate", "vcgpu_evaluate", "vcgpu_cost", "vcgpu_remove_outliers",
+    "vcgpu_solve", "vcgpu_solve_batch", "vcgpu_batch_plan", "vcgpu_solve_batch_inertial", "vcgpu_batch_plan_inertial", "vcgpu_iterate", "vcgpu_evaluate", "vcgpu_cost", "vcgpu_remove_outliers",
     "vcgpu_get_obs_active", "vcgpu_update_imu_weights", "vcgpu_get_imu_weights", "vcgpu_set_imu_weights",
     "vcgpu_get_state", "vcgpu_num_residuals", "vcgpu_frame_dim", "vcgpu_num_globals", "vcgpu_eval_reproj",
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
@@ -198,6 +198,12 @@ class Calibrator:
         self._chk(self.L.vcgpu_batch_plan(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
 
+    def batch_plan_inertial(self):
+        """(CTAs per cluster, clusters of that size resident at once) of this rig in solve_batch_inertial"""
+        a, c = C.c_int(), C.c_int()
+        self._chk(self.L.vcgpu_batch_plan_inertial(self.h, C.byref(a), C.byref(c)))
+        return a.value, c.value
+
     def iterate(self, n):
         s = Summary()
         self._chk(self.L.vcgpu_iterate(self.h, C.c_int(n), C.byref(s)))
@@ -338,11 +344,21 @@ class Calibrator:
 def solve_batch(calibrators):
     """vcgpu_solve_batch: solve every Calibrator of the list in one call, each rig in its own thread-block cluster
     (free-running: no callback, no rows).  Returns one summary dict per calibrator, in order."""
+    return _solve_many(lib().vcgpu_solve_batch, calibrators)
+
+
+def solve_batch_inertial(calibrators):
+    """vcgpu_solve_batch_inertial: solve_batch for rigs with inertial terms on (each rig in its own thread-block cluster
+    of the persistent inertial kernels).  Returns one summary dict per calibrator, in order."""
+    return _solve_many(lib().vcgpu_solve_batch_inertial, calibrators)
+
+
+def _solve_many(entry, calibrators):
     n = len(calibrators)
     L = lib()
     hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
     out = (Summary * max(n, 1))()
-    rc = L.vcgpu_solve_batch(hs, C.c_int(n), out)
+    rc = entry(hs, C.c_int(n), out)
     if rc != 0:
         msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
         raise VcgpuError(f"vcgpu error {rc}: {msg}")

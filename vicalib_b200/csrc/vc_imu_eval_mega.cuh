@@ -97,30 +97,32 @@ __device__ inline void evm_build_frame(const EvalMegaArgs& a, const Blocks& bt, 
   if (lane == 0) a.cost_part[f] = cost;
 }
 
-// Phase W: the weights of intervals bid * 16 + k (+ grid * 16 ...), a team of 16 lanes each.  A function of its own, as
-// the solve kernel's weights queue (chain_weights_queue): inlined, its registers join the kernel's and both spill more.
-__device__ __noinline__ void eval_weights(const WeightQueueArgs w, const double* xs, double* smem) {
+// Phase W: the weights of intervals bid * 16 + k (+ nb * 16 ...), a team of 16 lanes each (CTA bid of the nb that
+// evaluate the rig).  A function of its own, as the solve kernel's weights queue (chain_weights_queue): inlined, its
+// registers join the kernel's and both spill more.
+__device__ __noinline__ void eval_weights(const WeightQueueArgs w, const double* xs, double* smem, int bid, int nb) {
   constexpr int kTeams = kEvThreads / wts::kTeam;
   const int tid = threadIdx.x, warp = tid >> 5, team = tid / wts::kTeam, tl = tid & (wts::kTeam - 1);
   wts::Work* work = reinterpret_cast<wts::Work*>(smem);
-  for (int base = blockIdx.x * kTeams; base < w.ni; base += gridDim.x * kTeams) {
+  for (int base = bid * kTeams; base < w.ni; base += nb * kTeams) {
     if (base + (warp * (32 / wts::kTeam)) >= w.ni) break;  // whole warp past the end
     wts::imu_weights_team(w, xs, base + team, &work[team], tl);
   }
 }
 
-__global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a) {
+// The evaluation of the rig `a` by the CTAs of `scope` (vc_mega.cuh): the cooperative grid (eval_mega_kernel) or one
+// thread-block cluster (eval_mega_batch_kernel; never sharded: the exchange is compiled out for it).
+template <class Scope>
+__device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
   extern __shared__ double smem[];
-  namespace cg = cooperative_groups;
-  cg::grid_group grid = cg::this_grid();
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int nb = gridDim.x, bid = blockIdx.x;
+  const int nb = scope.nb(), bid = scope.bid();
   const int G = a.dp.G, NS = G * G + G, nf = a.dp.n_frames, ni = nf - 1, n_cams = a.dp.n_cams;
   __shared__ unsigned char tri_lut[128];
   __shared__ double shr[8][8];
   __shared__ unsigned task_s[kEvWarps];
   __shared__ unsigned long long* xbufs[kMaxRanks];
-  xchg_stage(a.x, xbufs);  // (visible after the first barrier below)
+  if constexpr (Scope::kSharded) xchg_stage(a.x, xbufs);  // (visible after the first barrier below)
   if (a.ctl->done) return;  // uniform over the grid: written before this launch
   const int buf = a.which ? 1 - a.ctl->cur : a.ctl->cur;
   const Blocks& bt = a.blk[buf];
@@ -164,7 +166,7 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
     }
   }
   mark(kEvProfTasks);
-  grid.sync();
+  scope.sync();
   // ------------------------------------------------------------ A: IMU blocks of every frame
   {
     const ImuAccView aa{a.dp, a.imu_r, a.imu_J, a.imuCg, ni};
@@ -175,11 +177,11 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
     }
   }
   mark(kEvProfAccum);
-  grid.sync();
+  scope.sync();
   // ------------------------------------------------------------ R1: slice partials
   RedFinArgs ra;
   ra.ctl = a.ctl; ra.which = a.which; ra.decide_mode = a.decide_mode; ra.multi = 0; ra.level1_only = 1;
-  const bool sharded = a.x.nranks > 1;
+  const bool sharded = Scope::kSharded && a.x.nranks > 1;
   // sharded: the separator frames' (first frame, ghost) gradients are normed after they have been summed
   ra.gf_skip_below = sharded ? a.dp.fd : 0;
   ra.gf_skip_from = static_cast<int64_t>(sharded ? a.dp.n_own : nf) * a.dp.fd;
@@ -190,11 +192,11 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
   ra.step_part = a.step_part; ra.n_step_part = a.n_step_part; ra.n_frames_fd = nf * a.dp.fd;
   ra.out[0] = a.blk[0]; ra.out[1] = a.blk[1]; ra.scalars = a.scalars; ra.counter = nullptr;
   reduce_level1(ra, a.dp, bt, smem, shr, bid, nb);
-  grid.sync();
+  scope.sync();
   // ------------------------------------------------------------ R2: C | gc totals (contiguous in Blocks)
-  mega_reduce_stage1(a.Cpart, NS, nb, NS, bt.C, -1, -1);
+  mega_reduce_stage1(a.Cpart, NS, nb, NS, bt.C, -1, -1, bid, nb);
   mark(kEvProfReduce);
-  grid.sync();
+  scope.sync();
   // ------------------------------------------------------------ D: scalars + decision (CTA 0)
   // entries of a rank's slot in the exchange: C | gc (NS), scalars kScCost .. kScGmax (+ 1 pad), own first frame diag 9 | gradient 9,
   // ghost diag 9 | gradient 9
@@ -251,7 +253,7 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
         a.sep_out[(q < kSepFd ? 0 : a.x.nranks * kSepFd) + k * kSepFd + (q < kSepFd ? q : q - kSepFd)] = v;
       }
     }
-    grid.sync();
+    scope.sync();
     if (bid == 0) {
       double* tot = &shr[0][0];  // [ranks][8] the ranks' scalars
       if (tid < a.x.nranks * kScNotPD) tot[(tid / kScNotPD) * 8 + tid % kScNotPD] = xchg_get(a.x, xbufs, tid / kScNotPD, eSc + tid % kScNotPD);
@@ -292,7 +294,7 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
   }
   mark(kEvProfDecide);
   if (!a.do_weights || a.dp.rotation_only) return;  // uniform
-  grid.sync();
+  scope.sync();
   // ------------------------------------------------------------ W: UpdateImuWeights at the accepted point
   {
     const volatile Ctl* c = a.ctl;
@@ -300,9 +302,19 @@ __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a
     WeightQueueArgs wa;
     wa.dp.off_v = a.dp.off_v; wa.dp.off_imu = a.dp.off_imu; wa.buf = a.buf; wa.ftime = a.ftime; wa.wsqrt = a.wsqrt;
     wa.ni = ni; wa.sigma_g = a.sigma_g; wa.sigma_a = a.sigma_a;
-    eval_weights(wa, a.state[c->cur], smem);
+    eval_weights(wa, a.state[c->cur], smem, bid, nb);
   }
   mark(kEvProfWeights);
+}
+
+// One rig on the whole cooperative grid.
+__global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a) { eval_mega(a, GridScope()); }
+
+// A batch of rigs, one thread-block cluster each: cluster k evaluates args[k], read where they are (as
+// chain_solve_batch_kernel's)
+__global__ void __launch_bounds__(kEvThreads, 1) eval_mega_batch_kernel(const EvalMegaArgs* __restrict__ args) {
+  ClusterScope scope;
+  eval_mega(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

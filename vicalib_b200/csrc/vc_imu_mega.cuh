@@ -21,6 +21,8 @@
 #pragma once
 #include <cooperative_groups.h>
 
+#include <type_traits>
+
 #include "vc_chain.cuh"
 #include "vc_kernels.cuh"
 #include "vc_mega.cuh"
@@ -696,14 +698,18 @@ __device__ __noinline__ void dense_ldlt_tiles(double* S, int N, int LD, double* 
   DenseTiles<T, 0>::run(R, S, N, LD, wd, bad, ti, tk);
   __syncthreads();
 }
-// One damped solve of the frame-chain + globals system and (optionally) the state update, all in one launch.
-__global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveArgs a) {
+// One damped solve of the frame-chain + globals system and (optionally) the state update of the rig `a`, by the CTAs
+// of `scope` (vc_mega.cuh): the cooperative grid (chain_solve_kernel) or one thread-block cluster (chain_solve_batch_kernel).
+// The barriers count arrivals on the rig's own counters (a.sync) either way; the CTAs of a cluster are co-scheduled, as
+// those of a cooperative grid are, so a CTA that spins on them never waits for one that has not started.  A cluster is
+// never sharded: the exchange is compiled out for it.
+template <class Scope>
+__device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope) {
   extern __shared__ double smem[];
-  namespace cg = cooperative_groups;
   constexpr int FD = 9;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int grp = tid / kCsGroup, gtid = tid - grp * kCsGroup;
-  const int nb = gridDim.x, bid = blockIdx.x;
+  const int nb = scope.nb(), bid = scope.bid();
   const int n_groups = nb * kCsGroups, gid = bid * kCsGroups + grp;
   const int G = a.dp.G, NS = G * G + G, nf = a.dp.n_frames;
   const int64_t nfp = static_cast<int64_t>(nf) * FD;
@@ -712,7 +718,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
   __shared__ double part[kCsThreads / 32][4];
   __shared__ unsigned long long wtask;
   __shared__ unsigned long long* xbufs[kMaxRanks];
-  xchg_stage(a.x, xbufs);  // (visible after the first barrier below)
+  if constexpr (Scope::kSharded) xchg_stage(a.x, xbufs);  // (visible after the first barrier below)
   if (bid == 0 && tid == 0)
     for (int k = 0; k < kCsSyncWords; ++k) a.sync_next[k] = 0ull;
   if (a.ctl->done) return;  // uniform over the grid: written before this launch
@@ -732,7 +738,10 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
   // CTAs [ns, grid) leave after their last elimination level and work the weights queue; the solve goes on among the
   // first ns CTAs, which join the queue when they are done.  Barriers therefore count arrivals: everybody who took
   // part in a phase arrives, only those who go on wait.
-  const bool wts_go = a.wts_on && !a.dp.rotation_only && a.ctl->iter > 0 && a.ctl->last_accepted;
+  // The queue is the grid's: a cluster of at most 8 CTAs has none to spare (a batch computes the weights in its
+  // evaluation launch), and compiled into the cluster kernel too it would change how ptxas allocates the grid kernel's call.
+  constexpr bool kQueue = std::is_same<Scope, GridScope>::value;
+  const bool wts_go = kQueue && a.wts_on && !a.dp.rotation_only && a.ctl->iter > 0 && a.ctl->last_accepted;
   const int ns = wts_go ? min(max(a.n_solver, 1), nb) : nb;
   unsigned long long* bar = a.sync;      // this launch's counters (the host alternates the pair)
   unsigned long long* wq = a.sync + 1;
@@ -855,7 +864,7 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
   mark(kCsProfReduce);
   barrier(ns);
   // ------------------------------------------------------------ sharded: the ranks' partial systems meet here
-  const bool sharded = a.x.nranks > 1;
+  const bool sharded = Scope::kSharded && a.x.nranks > 1;
   const int TB = chain_top_block(G);
   if (sharded) {
     const ChainLevel& top = a.lev[a.n_levels - 1];
@@ -1195,6 +1204,17 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
     }
     mark(kCsProfUpdate);
   }
+}
+
+// One rig on the whole cooperative grid.
+__global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveArgs a) { chain_solve(a, GridScope()); }
+
+// A batch of rigs, one thread-block cluster each (launched with a cluster dimension; no cooperative launch): cluster k
+// solves args[k].  The arguments are read where they are, through the read-only data path: staged in shared memory they
+// would leave too little of it for the two groups' workspaces of the largest rig that fits (G = 67).
+__global__ void __launch_bounds__(kCsThreads, 1) chain_solve_batch_kernel(const ChainSolveArgs* __restrict__ args) {
+  ClusterScope scope;
+  chain_solve(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

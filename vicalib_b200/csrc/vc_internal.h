@@ -13,6 +13,8 @@
 namespace vc {
 
 struct MegaArgs;  // vc_mega.cuh
+struct ChainSolveArgs;  // vc_imu_mega.cuh
+struct EvalMegaArgs;  // vc_imu_eval_mega.cuh
 constexpr int kMaxCams = 8;
 constexpr int kCamStateStride = 17;  // q_ck(4) p_ck(3) intr(10)
 constexpr int kImuStateSize = 15;    // g2 b6 sf6 ts1
@@ -187,6 +189,10 @@ struct vcgpu_handle {
   int dev_sms = 0, dev_smem_optin = 0;
   int mega_grid = 0, mega_warps[2] = {0, 0};  // [strategy]; 0 warps: does not fit / not supported, use the multi-launch engine
   vc::MegaArgs* d_batch_args = nullptr;  // vcgpu_solve_batch: the rigs of a launch group (held by the group's first handle)
+  // vcgpu_solve_batch_inertial: the rigs of the batch as the solve [2 parities][n] and evaluation [start, iteration][n]
+  // batch kernels take them (held by the batch's first handle)
+  vc::ChainSolveArgs* d_batch_cs = nullptr;
+  vc::EvalMegaArgs* d_batch_ev = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)
   bool imu_mega_ok = false;
   int imu_mega_grid = 0;

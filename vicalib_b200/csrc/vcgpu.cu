@@ -216,7 +216,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_batch_cs); dev_free(&h->d_batch_ev); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -757,6 +757,14 @@ extern "C" int vcgpu_solve_batch(vcgpu_handle* const* handles, int n, vcgpu_summ
 extern "C" int vcgpu_batch_plan(vcgpu_handle* h, int* cluster_size, int* warps, int* resident_clusters) {
   if (!h) return VCGPU_ERR_INVALID;
   return batch_plan_of(h, cluster_size, warps, resident_clusters);
+}
+extern "C" int vcgpu_solve_batch_inertial(vcgpu_handle* const* handles, int n, vcgpu_summary* out) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  return run_solve_batch_inertial(handles, n, out);
+}
+extern "C" int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int* resident_clusters) {
+  if (!h) return VCGPU_ERR_INVALID;
+  return imu_batch_plan_of(h, cluster_size, resident_clusters);
 }
 extern "C" int vcgpu_iterate(vcgpu_handle* h, int n, vcgpu_summary* out) {
   if (!h || n <= 0) return VCGPU_ERR_INVALID;
