@@ -223,6 +223,27 @@ int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t* cam_id, c
  * per camera (w_ck 3 | p_ck 3 | intrinsics K), then with inertial terms (g 2 | b 6 | sf 6 | ts 1).  Rows / columns of
  * constant parameter blocks are zero (ceres::Covariance convention). */
 int vcgpu_get_covariance(vcgpu_handle* h, double* cov);
+/* vcgpu_get_covariance of n handles in one call; vision and inertial rigs may be mixed.  cov[i] (G_i x G_i row-major,
+ * G_i = vcgpu_num_globals) gets what vcgpu_get_covariance(handles[i]) returns at the handle's current state, equal to
+ * rounding: the same tangent layout, the same Jacobi-scaled undamped system, rows and columns of constant blocks exactly
+ * 0.0; each matrix is exactly symmetric (one triangle is computed and mirrored).  Every rig runs inside its own
+ * thread-block cluster, of the size its batch solve takes (a function of the rig alone), so its matrix does not depend,
+ * bit for bit, on what else is in the batch or in which order: per handle the start point's evaluation and Jacobi scale
+ * on its own stream, then one launch per (kind, cluster size) group in which each cluster eliminates the frames once,
+ * factors the reduced system once and solves its G unit right-hand sides, then one copy back per handle.  Options
+ * (strategy, tolerances, max_iters) play no part.  Nothing on the handle changes: state, IMU weights and what a later
+ * vcgpu_solve or batch solve computes stay as they were.
+ * status: n codes or NULL.  VCGPU_ERR_NUMERIC: the system of one or more rigs is not positive definite; their status is
+ * VCGPU_ERR_NUMERIC and their cov[i] is not written, every other rig's matrix is written with status VCGPU_OK, and the
+ * message names the failing indices.
+ * Returns VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in
+ * vcgpu_last_error of every non-null handle, for: n <= 0, a null or repeated handle, a null cov[i], handles on
+ * different devices, frame shards, any vcgpu_set_profiling bit or L2 flushing, and a rig the cluster kernels do not
+ * fit (vision: the persistent vision kernel's fit, or no active observation; inertial: G >= 68 on an H100).
+ * Device memory: per handle G^2 + 16 doubles (vision rigs also 9 (G^2 + G) of workspace), and a few KB of kernel
+ * arguments per rig, held by handle 0. */
+int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov /* n pointers */,
+                               int* status /* n, or NULL */);
 
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */

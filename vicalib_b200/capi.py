@@ -24,7 +24,8 @@ EXPORTS = [
     "vcgpu_get_obs_active", "vcgpu_update_imu_weights", "vcgpu_get_imu_weights", "vcgpu_set_imu_weights",
     "vcgpu_get_state", "vcgpu_num_residuals", "vcgpu_frame_dim", "vcgpu_num_globals", "vcgpu_eval_reproj",
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
-    "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_pose_pnp_ransac",
+    "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
+    "vcgpu_pose_pnp_ransac",
 ]
 
 
@@ -61,7 +62,11 @@ ITER_CB = C.CFUNCTYPE(C.c_int, C.POINTER(Iteration), C.c_void_p)
 
 
 class VcgpuError(RuntimeError):
-    pass
+    """A negative return code of the library.  covariance_batch also sets `status` (one code per rig) and
+    `covariances` (the matrices written, None for the rigs whose system is not positive definite)."""
+
+    status = None
+    covariances = None
 
 
 def lib():
@@ -363,3 +368,29 @@ def _solve_many(entry, calibrators):
         msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
         raise VcgpuError(f"vcgpu error {rc}: {msg}")
     return [{f[0]: getattr(out[i], f[0]) for f in Summary._fields_} for i in range(n)]
+
+
+def covariance_batch(calibrators, out=None):
+    """vcgpu_get_covariance_batch: the covariance of the globals of every Calibrator of the list (vision and inertial
+    rigs may be mixed), each rig in its own thread-block cluster.  Returns one G x G array per calibrator, in order;
+    out: optional list of C-contiguous float64 (G, G) arrays to write into.  Raises VcgpuError; where some rigs' systems
+    are not positive definite, the error's `status` gives every rig's code and `covariances` the other rigs' matrices."""
+    n = len(calibrators)
+    L = lib()
+    if out is None:
+        out = [None if g is None else np.zeros((g.G, g.G)) for g in calibrators]
+    for a in out:
+        if a is not None and (a.dtype != np.float64 or not a.flags.c_contiguous):
+            raise ValueError("covariance_batch: out arrays must be C-contiguous float64")
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    ptrs = (C.c_void_p * max(n, 1))(*[None if a is None else a.ctypes.data for a in out])
+    status = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_covariance_batch(hs, C.c_int(n), ptrs, status)
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:  # VCGPU_ERR_NUMERIC: the other rigs' matrices are written
+            e.status = [status[i] for i in range(n)]
+            e.covariances = [out[i] if status[i] == 0 else None for i in range(n)]
+        raise e
+    return list(out)

@@ -703,8 +703,11 @@ __device__ __noinline__ void dense_ldlt_tiles(double* S, int N, int LD, double* 
 // The barriers count arrivals on the rig's own counters (a.sync) either way; the CTAs of a cluster are co-scheduled, as
 // those of a cooperative grid are, so a CTA that spins on them never waits for one that has not started.  A cluster is
 // never sharded: the exchange is compiled out for it.
-template <class Scope>
-__device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope) {
+// kCov (chain_cov_batch_kernel, with a.D2x set): the elimination, the Schur reduction and the dense factorisation only;
+// in place of the dense phase's right-hand side, the G unit right-hand sides of the globals give the globals' block of
+// the [globals | top nodes] inverse, unscaled into cov (G x G; mask: 0 on constant globals).  No step, no state update.
+template <class Scope, bool kCov = false>
+__device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope, const double* mask = nullptr, double* cov = nullptr) {
   extern __shared__ double smem[];
   constexpr int FD = 9;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1024,6 +1027,18 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
     else if (tiles == 9) dense_ldlt_tiles<9>(S, N, LD, wd, &bad_dense);
     else dense_ldlt_smem(S, N, LD, wd, &bad_dense);
     __syncthreads();
+    if constexpr (kCov) {  // one warp per right-hand side at a time, in registers: no shared memory beyond the factors
+      if (bad_dense) {
+        if (tid == 0) a.scalars[kScNotPD] = 1.0;
+        return;
+      }
+      for (int j = warp; j < G; j += kCsThreads / 32) {
+        double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
+        if (mask[j] != 0.0) warp_inverse_column<kCovQ, true>(S, LD, wd, N, j, lane, x);
+        cov_store_column<kCovQ>(x, sc, mask, G, j, lane, cov);
+      }
+      return;
+    }
     if (prof) { const long long t = clock64(); a.prof[53] += static_cast<unsigned long long>(t - dt0); dt0 = t; }
     if (warp == 0) {  // x_i = (u_Ni - sum_{k>i} u_ki x_k) / d_i
       constexpr int kQ = 5;
@@ -1099,6 +1114,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
       }
     }
   }
+  if constexpr (kCov) return;  // the other CTAs: nothing after the elimination
   if (prof) { const long long t = clock64(); a.prof[55] += static_cast<unsigned long long>(t - dt0); }
   mark(kCsProfDense);
   if (a.n_levels <= 2) break;  // the next barrier is the one the whole grid meets at
@@ -1215,6 +1231,20 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveAr
 __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_batch_kernel(const ChainSolveArgs* __restrict__ args) {
   ClusterScope scope;
   chain_solve(args[blockIdx.x / scope.nb()], scope);
+}
+
+// a rig as chain_cov_batch_kernel takes it: the solve's arguments (D2x set, scalars[kScNotPD] zeroed: set where a pivot
+// fails), the constant-global mask [G] and the covariance it writes [G*G]
+struct ChainCovArgs {
+  ChainSolveArgs s;
+  const double* mask;
+  double* cov;
+};
+// A batch of inertial rigs, one thread-block cluster each: cluster k writes the covariance of args[k] (vcgpu_get_covariance_batch).
+__global__ void __launch_bounds__(kCsThreads, 1) chain_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
+  ClusterScope scope;
+  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
+  chain_solve<ClusterScope, true>(a.s, scope, a.mask, a.cov);
 }
 
 }  // namespace vc

@@ -15,6 +15,8 @@ namespace vc {
 struct MegaArgs;  // vc_mega.cuh
 struct ChainSolveArgs;  // vc_imu_mega.cuh
 struct EvalMegaArgs;  // vc_imu_eval_mega.cuh
+struct CovArgs;  // vc_mega.cuh
+struct ChainCovArgs;  // vc_imu_mega.cuh
 constexpr int kMaxCams = 8;
 constexpr int kCamStateStride = 17;  // q_ck(4) p_ck(3) intr(10)
 constexpr int kImuStateSize = 15;    // g2 b6 sf6 ts1
@@ -193,6 +195,11 @@ struct vcgpu_handle {
   // batch kernels take them (held by the batch's first handle)
   vc::ChainSolveArgs* d_batch_cs = nullptr;
   vc::EvalMegaArgs* d_batch_ev = nullptr;
+  // vcgpu_get_covariance_batch: the batch's vision and inertial rigs as the covariance kernels take them (held by the
+  // batch's first handle), and this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
+  vc::CovArgs* d_batch_cov = nullptr;
+  vc::ChainCovArgs* d_batch_ccov = nullptr;
+  double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)
   bool imu_mega_ok = false;
   int imu_mega_grid = 0;

@@ -856,4 +856,199 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) lm_mega_batch_kernel(const
   mega_solve<Str>(*reinterpret_cast<const MegaArgs*>(words), scope);
 }
 
+// ------------------------------------------------------------------ covariance of the globals (vcgpu_get_covariance_batch)
+// The [globals, globals] block of the inverse of the Jacobi-scaled, undamped arrow system S J^T J S (+ 1 on the diagonal
+// of constant globals) is the inverse of the reduced system the frame elimination produces.  One factorisation, then G
+// unit right-hand sides, one warp each.
+constexpr int kCovQ = 4;  // register slots per lane of a right-hand side: systems of up to 128 unknowns
+
+// Column j of the inverse of a factored n x n system, by one warp (n <= 32 kQ).  A: the factor's lower triangle,
+// row-major with leading dimension ld; p: the reciprocals of its pivots.  kLdlt = false: Cholesky M = L L^T (A = L,
+// p_i = 1 / L_ii).  kLdlt = true: M = L D L^T as chain_solve's dense phase keeps it (A_ik = L_ik d_k, p_i = 1 / d_i).
+// Entry k of the column lands in lane k mod 32, slot k / 32 of x.
+template <int kQ, bool kLdlt>
+__device__ __forceinline__ void warp_inverse_column(const double* A, int ld, const double* p, int n, int j, int lane, double (&x)[kQ]) {
+#pragma unroll
+  for (int q = 0; q < kQ; ++q) x[q] = 32 * q + lane == j ? 1.0 : 0.0;
+  // forward, from row j on (the rows above are zero): t_k = r_k p_k, r_i -= A_ik t_k below it.  Cholesky keeps t = L^-1 e_j,
+  // L D L^T keeps r = L^-1 e_j (unit L)
+#pragma unroll
+  for (int q = 0; q < kQ; ++q) {
+    for (int l = 0; l < 32; ++l) {
+      const int k = 32 * q + l;
+      if (k < j || k >= n) continue;
+      const double t = __shfl_sync(0xffffffffu, x[q], l) * p[k];
+      if (!kLdlt && lane == l) x[q] = t;
+#pragma unroll
+      for (int qq = q; qq < kQ; ++qq) {
+        const int i = 32 * qq + lane;
+        if (i > k && i < n) x[qq] -= A[i * ld + k] * t;
+      }
+    }
+  }
+  // backward, both forms: x_i = r_i p_i, r_k -= A_ik x_i above it
+#pragma unroll
+  for (int q = kQ - 1; q >= 0; --q) {
+    for (int l = 31; l >= 0; --l) {
+      const int i = 32 * q + l;
+      if (i >= n) continue;
+      const double xi = __shfl_sync(0xffffffffu, x[q], l) * p[i];
+      if (lane == l) x[q] = xi;
+      const double* row = A + i * ld + lane;
+#pragma unroll
+      for (int qq = 0; qq <= q; ++qq)
+        if (32 * qq + lane < i) x[qq] -= row[32 * qq] * xi;
+    }
+  }
+}
+
+// Column j of the covariance from column j of the scaled inverse (x: warp_inverse_column's layout, the globals first):
+// entries i >= j into cov[i][j] and cov[j][i] (one triangle, mirrored: the matrix is exactly symmetric), unscaled by
+// s_i s_j.  Rows and columns of constant globals (mask 0) are exactly 0.
+template <int kQ>
+__device__ __forceinline__ void cov_store_column(const double (&x)[kQ], const double* sc, const double* mask, int G, int j, int lane,
+                                                 double* cov) {
+  const bool free_j = mask[j] != 0.0;
+#pragma unroll
+  for (int q = 0; q < kQ; ++q) {
+    const int i = 32 * q + lane;
+    if (i < j || i >= G) continue;
+    const double v = free_j && mask[i] != 0.0 ? sc[i] * sc[j] * x[q] : 0.0;
+    cov[static_cast<int64_t>(i) * G + j] = v;
+    cov[static_cast<int64_t>(j) * G + i] = v;
+  }
+}
+
+// a vision rig as cov_mega_batch_kernel takes it
+struct CovArgs {
+  int n_frames, G;
+  Blocks b;             // the blocks of the evaluated point
+  const double* scale;  // Jacobi scale [nf*6 + G]
+  const double* D2x;    // explicit damping [nf*6 + G]: 0 on frames and free globals, 1 on constant globals
+  const double* mask;   // [G] 0: constant global
+  double* part;         // [cluster CTAs][G*G + G] CTA partials of the Schur sum
+  double* tot;          // [G*G + G] their total
+  double* cov;          // [G*G] the covariance, row-major
+  double* notpd;        // set to 1 where a pivot fails (zeroed before the launch)
+};
+// dynamic shared memory of cov_mega_batch_kernel: per warp its frame's scaled [E | g] and X, the reduced system, pivots
+__host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
+  return static_cast<size_t>(n_warps) * 12 * (G + 1) + static_cast<size_t>(G) * G + 2 * static_cast<size_t>(G);
+}
+
+// A batch of vision rigs, one thread-block cluster each: cluster k writes the covariance of args[k].  Frames are owned as
+// in mega_solve (frame f -> CTA f mod cluster size, warp (f / size) mod warps); every CTA forms and factors the reduced
+// system (the same bits everywhere), then the cluster's warps share the right-hand sides.
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(const CovArgs* __restrict__ args) {
+  extern __shared__ double smem[];
+  constexpr int FD = 6;
+  ClusterScope scope;
+  const CovArgs& a = args[blockIdx.x / scope.nb()];
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nthreads = blockDim.x, nwarps = nthreads >> 5;
+  const int bid = scope.bid(), nb = scope.nb();
+  const int G = a.G, M = G + 1, NS = G * G + G, nf = a.n_frames;
+  const int64_t nfp = static_cast<int64_t>(nf) * FD;
+  const int nk = bid < nf ? (nf - bid + nb - 1) / nb : 0;
+  double* wmem = smem;                                           // [nwarps][2][FD][M]
+  double* S = wmem + static_cast<size_t>(nwarps) * 2 * FD * M;   // [NS] Schur accumulator, then the reduced system
+  double* invd = S + NS;                                         // [G]
+  __shared__ int bad;
+  const double* scg = a.scale + nfp;
+  for (int e = tid; e < NS; e += nthreads) S[e] = 0.0;
+  if (tid == 0) bad = 0;
+  bool frame_bad = false;
+  for (int base = 0; base < nk; base += nwarps) {
+    const int k = base + warp;
+    __syncthreads();
+    if (k < nk) {
+      const int f = bid + k * nb;
+      double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
+      double* Xw = Esw + FD * M;
+      const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+      const double* Bf = a.b.B + static_cast<int64_t>(f) * FD * FD;
+      const double* Ef = a.b.E + static_cast<int64_t>(f) * FD * G;
+      double s[FD], L[FD][FD], iL[FD];
+#pragma unroll
+      for (int i = 0; i < FD; ++i) s[i] = sf[i];
+#pragma unroll
+      for (int i = 0; i < FD; ++i)
+#pragma unroll
+        for (int j = 0; j <= i; ++j) {
+          const double bij = Bf[i * FD + j];
+          double v = bij * s[i] * s[j];
+          if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], 0.0, a.D2x, nullptr, 0, false);
+          L[i][j] = v;
+        }
+#pragma unroll
+      for (int j = 0; j < FD; ++j) {
+        double d = L[j][j];
+#pragma unroll
+        for (int q = 0; q < j; ++q) d -= L[j][q] * L[j][q];
+        if (!(d > 0.0)) { frame_bad = true; d = 1.0; }
+        const double inv = rsqrt(d);
+        L[j][j] = d * inv;
+        iL[j] = inv;
+#pragma unroll
+        for (int i = j + 1; i < FD; ++i) {
+          double t = L[i][j];
+#pragma unroll
+          for (int q = 0; q < j; ++q) t -= L[i][q] * L[j][q];
+          L[i][j] = t * inv;
+        }
+      }
+      for (int c = lane; c < M; c += 32) {
+        double x[FD];
+        const double scc = c < G ? scg[c] : 1.0;
+#pragma unroll
+        for (int i = 0; i < FD; ++i) {
+          const double r = (c < G ? Ef[i * G + c] : 0.0) * s[i] * scc;  // the right-hand side plays no part
+          Esw[i * M + c] = r;
+          x[i] = r;
+        }
+#pragma unroll
+        for (int i = 0; i < FD; ++i) {
+          double t = x[i];
+#pragma unroll
+          for (int q = 0; q < i; ++q) t -= L[i][q] * x[q];
+          x[i] = t * iL[i];
+        }
+#pragma unroll
+        for (int i = FD - 1; i >= 0; --i) {
+          double t = x[i];
+#pragma unroll
+          for (int q = i + 1; q < FD; ++q) t -= L[q][i] * x[q];
+          x[i] = t * iL[i];
+        }
+#pragma unroll
+        for (int i = 0; i < FD; ++i) Xw[i * M + c] = x[i];
+      }
+    }
+    __syncthreads();
+    schur_accumulate<FD>(S, wmem, 2 * FD * M, min(nwarps, nk - base), G, tid, nthreads);
+  }
+  if (frame_bad) *a.notpd = 1.0;
+  __syncthreads();
+  double* out = a.part + static_cast<int64_t>(bid) * NS;
+  for (int e = tid; e < NS; e += nthreads) out[e] = S[e];
+  scope.sync();
+  mega_reduce_stage1(a.part, NS, nb, NS, a.tot, -1, -1, bid, nb);  // entry e by CTA e mod size, CTAs in order
+  scope.sync();
+  for (int e = tid; e < NS; e += nthreads) {
+    if (e < G * G && e % G > e / G) continue;  // lower triangle only
+    S[e] = e < G * G ? reduced_system_entry(e, G, a.b.C[e], __ldcg(a.tot + e), scg, 0.0, a.D2x, nfp) : 0.0;
+  }
+  __syncthreads();
+  if (warp == 0) mega_chol_solve_smem(S, G, lane, invd, &bad);
+  __syncthreads();
+  if (bad) {
+    if (bid == 0 && tid == 0) *a.notpd = 1.0;
+    return;
+  }
+  for (int j = bid * nwarps + warp; j < G; j += nb * nwarps) {
+    double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
+    if (a.mask[j] != 0.0) warp_inverse_column<kCovQ, false>(S, G, invd, G, j, lane, x);
+    cov_store_column<kCovQ>(x, scg, a.mask, G, j, lane, a.cov);
+  }
+}
+
 }  // namespace vc

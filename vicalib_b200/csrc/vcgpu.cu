@@ -12,6 +12,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <numeric>
+#include <tuple>
 
 #include <nccl.h>
 
@@ -216,7 +217,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_batch_cs); dev_free(&h->d_batch_ev); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_batch_cs); dev_free(&h->d_batch_ev); dev_free(&h->d_batch_cov); dev_free(&h->d_batch_ccov); dev_free(&h->d_cov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -765,6 +766,11 @@ extern "C" int vcgpu_solve_batch_inertial(vcgpu_handle* const* handles, int n, v
 extern "C" int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int* resident_clusters) {
   if (!h) return VCGPU_ERR_INVALID;
   return imu_batch_plan_of(h, cluster_size, resident_clusters);
+}
+extern "C" int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_covariance_batch");
+  return run_covariance_batch(handles, n, cov, status);
 }
 extern "C" int vcgpu_iterate(vcgpu_handle* h, int n, vcgpu_summary* out) {
   if (!h || n <= 0) return VCGPU_ERR_INVALID;
