@@ -221,11 +221,12 @@ int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t* cam_id, c
 /* GetSolutionCovariance (vicalibrator.h:802-857; compiled out upstream behind COMPUTE_VICALIB_COVARIANCE): the
  * [globals, globals] block of (J^T J)^-1 at the current state, tangent space, G x G row-major with G = vcgpu_num_globals:
  * per camera (w_ck 3 | p_ck 3 | intrinsics K), then with inertial terms (g 2 | b 6 | sf 6 | ts 1).  Rows / columns of
- * constant parameter blocks are zero (ceres::Covariance convention). */
+ * constant or unused parameter blocks (the blocks of a camera no active observation sees) are zero (ceres::Covariance
+ * convention). */
 int vcgpu_get_covariance(vcgpu_handle* h, double* cov);
 /* vcgpu_get_covariance of n handles in one call; vision and inertial rigs may be mixed.  cov[i] (G_i x G_i row-major,
  * G_i = vcgpu_num_globals) gets what vcgpu_get_covariance(handles[i]) returns at the handle's current state, equal to
- * rounding: the same tangent layout, the same Jacobi-scaled undamped system, rows and columns of constant blocks exactly
+ * rounding: the same tangent layout, the same Jacobi-scaled undamped system, rows and columns of constant or unused blocks exactly
  * 0.0; each matrix is exactly symmetric (one triangle is computed and mirrored).  Every rig runs inside its own
  * thread-block cluster, of the size its batch solve takes (a function of the rig alone), so its matrix does not depend,
  * bit for bit, on what else is in the batch or in which order: per handle the start point's evaluation and Jacobi scale

@@ -39,9 +39,13 @@ int Problem::CamOffset(int c) const {
 int Problem::ImuOffset() const { return CamOffset(n_cams); }
 int Problem::NumGlobals() const { return ImuOffset() + (flags.inertial ? 15 : 0); }
 
-// vicalibrator.h:572-592, 657-676
+// vicalibrator.h:572-592, 657-676.  A camera no active observation sees is in no residual (the IMU residual takes no
+// camera block, vicalibrator.h:628-632): Ceres removes its blocks like those of an unused frame.
 void Problem::GlobalMask(std::vector<double>* mask) const {
   mask->assign(NumGlobals(), 1.0);
+  std::vector<uint8_t> seen(n_cams, 0);
+  for (int64_t i = 0; i < n_obs; ++i)
+    if (obs_active[i]) seen[obs_cam[i]] = 1;
   for (int c = 0; c < n_cams; ++c) {
     const int off = CamOffset(c), K = NumIntrinsics(model[c]);
     if (c == 0) {
@@ -52,6 +56,8 @@ void Problem::GlobalMask(std::vector<double>* mask) const {
     }
     if (flags.fix_intrinsics)
       for (int i = 0; i < K; ++i) (*mask)[off + 6 + i] = 0.0;
+    if (!seen[c])
+      for (int i = 0; i < 6 + K; ++i) (*mask)[off + i] = 0.0;
   }
   if (flags.inertial) {
     const int o = ImuOffset();

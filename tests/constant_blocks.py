@@ -3,7 +3,8 @@
 Ceres minimises over the parameter blocks that are neither constant nor unused (Program::RemoveFixedBlocks): it never
 moves the others, and its parameter tolerance, step_norm <= param_tol * (x_norm + param_tol), takes x_norm over the
 blocks it keeps.  Which blocks ViCalibrator::SetupProblem holds constant (vicalibrator.h:572-600, 657-676) is restated
-here from the flags alone, independently of the oracle's GlobalMask and the device's fill_mask.
+here from the flags, and which frames and cameras no residual uses from the observations, independently of the
+oracle's GlobalMask and the device's fill_mask.
 """
 import numpy as np
 
@@ -47,6 +48,15 @@ def frames_used(p, flags):
     return used
 
 
+def cams_used(p, active=None):
+    """1 per camera an active observation sees: the IMU residual takes no camera block, so a camera without one is in
+    no residual at all (vision or inertial)"""
+    used = np.zeros(p.n_cams, bool)
+    cam = np.asarray(p.obs_cam)
+    used[cam if active is None else cam[np.asarray(active) > 0]] = True
+    return used
+
+
 def free_blocks(flags):
     """{block name: free?} for the global blocks (cam0's extrinsics are listed separately from the other cameras')"""
     inertial = bool(flags.get("inertial", 0))
@@ -61,6 +71,7 @@ def state_norms(st, p, flags):
     inertial = bool(flags.get("inertial", 0))
     free = free_blocks(flags)
     used = frames_used(p, flags)
+    cams = cams_used(p)
     K = num_intr(p.models)
     s_free = s_all = 0.0
 
@@ -76,9 +87,9 @@ def state_norms(st, p, flags):
         if inertial:
             add(st["v_w"][f], used[f])
     for c in range(p.n_cams):
-        add(st["q_ck"][c], c > 0 or free["q0"])
-        add(st["p_ck"][c], c > 0 or free["p0"])
-        add(st["intr"][c, :K[c]], free["intr"])
+        add(st["q_ck"][c], cams[c] and (c > 0 or free["q0"]))
+        add(st["p_ck"][c], cams[c] and (c > 0 or free["p0"]))
+        add(st["intr"][c, :K[c]], cams[c] and free["intr"])
     if inertial:
         for k in ("g", "b", "sf"):
             add(st[k], free[k])
@@ -99,6 +110,8 @@ def constant_parts(st, p, flags):
     unused = ~frames_used(p, flags)
     if unused.any():
         out["T_wp_unused"] = st["T_wp"][unused]
+    for c in np.flatnonzero(~cams_used(p)):
+        out[f"q_ck{c}"], out[f"p_ck{c}"], out[f"intr{c}"] = st["q_ck"][c], st["p_ck"][c], st["intr"][c]
     if flags.get("inertial", 0):
         for k in ("g", "b", "sf"):
             if not free[k]:

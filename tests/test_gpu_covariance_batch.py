@@ -273,12 +273,13 @@ def test_refusals():
 
 
 # ------------------------------------------------------------------ 6. a singular rig among healthy ones
-def test_singular_rig():
+def test_singular_rig_among_healthy():
     from vicalib_b200.capi import VcgpuError
 
-    # camera 1 loses every observation: its columns are free but empty, so J^T J is singular
+    # every reprojection residual weighted 0: the frames' and the free globals' columns are empty, so J^T J is singular
+    # (a camera that loses every observation is not: it leaves the problem, test_emptied_camera_rig_among_healthy)
     sing = _vision(18, 90, models=("poly3", "poly3"))
-    sing.remove_outliers(np.array([np.inf, 0.0]), 1.0)
+    sing.set_flags(visual_mult=0.0)
     with pytest.raises(VcgpuError) as e:
         sing.covariance()
     assert "vcgpu error -3" in str(e.value)
@@ -295,3 +296,33 @@ def test_singular_rig():
     for i in (0, 2):
         _check_matrix(bufs[i], np.diag(bufs[i]) != 0)
         assert _corr_err(bufs[i], gs[i].covariance()) <= BAR[i == 2]
+
+
+# ------------------------------------------------------------------ 7. a camera emptied by remove_outliers
+def test_emptied_camera_rig_among_healthy():
+    """Camera 1 loses every observation to vcgpu_remove_outliers: it is in no residual any more, so its blocks leave the
+    problem (as Ceres removes them) and both entry points return VCGPU_OK, exact-zero rows and columns for it, and the
+    dense inverse of the oracle's J^T J (which drops it the same way) elsewhere."""
+    from oracle.binding import Oracle
+    from vicalib_b200.capi import covariance_batch
+
+    p = synth.make_problem(models=("poly3", "poly3"), n_frames=18, grid=(10, 7), seed=90)
+    rmse = np.array([np.inf, 0.0])
+    emptied = _vision(18, 90, models=("poly3", "poly3"))
+    assert emptied.remove_outliers(rmse, 1.0) == int((p.obs_cam == 1).sum())
+    o = Oracle(p)
+    o.remove_outliers(rmse, 1.0)
+    mask = o.global_mask()
+    cam1 = np.arange(13, 26)
+    assert mask[:13].any() and not mask[cam1].any()
+    solo = emptied.covariance()
+    healthy = [_vision(18, 91), _inertial(90, 92)]
+    gs = [healthy[0], emptied, healthy[1]]
+    covs = covariance_batch(gs)
+    _check_matrix(covs[1], mask)
+    assert not solo[cam1].any() and not solo[:, cam1].any()
+    ref = _dense_cov(o)
+    assert _corr_err(covs[1], ref) <= BAR[False] and _corr_err(solo, ref) <= BAR[False]
+    for i in (0, 2):
+        _check_matrix(covs[i], np.diag(covs[i]) != 0)
+        assert _corr_err(covs[i], gs[i].covariance()) <= BAR[i == 2]

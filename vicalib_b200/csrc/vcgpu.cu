@@ -351,6 +351,11 @@ static void fill_mask(const vcgpu_handle* h, std::vector<double>* mask) {
     }
     if (f.fix_intrinsics)
       for (int i = 0; i < ci.K; ++i) (*mask)[ci.goff + 6 + i] = 0.0;
+    // A camera no active observation sees is in no residual (the IMU residual takes no camera block): Ceres removes
+    // its blocks (Program::RemoveFixedBlocks), so they are never moved and stay out of x_norm, like an unused frame's.
+    // A frame shard sees its own frames' observations only, so a sharded handle keeps every camera.
+    if (ci.n_obs == 0 && h->nranks == 1)
+      for (int i = 0; i < 6 + ci.K; ++i) (*mask)[ci.goff + i] = 0.0;
   }
   if (f.inertial) {  // vicalibrator.h:657-676
     const int o = dp.imu_goff;
@@ -959,7 +964,8 @@ extern "C" int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const dou
 // [globals, globals] block of (J^T J)^-1 at the current state, i.e. the inverse of the Schur complement of the frames —
 // one solve of the (undamped, unscaled) arrow system per global column on the device, through the same frame
 // elimination the trust-region step uses.  Tangent space: per camera (w_ck 3 | p_ck 3 | intrinsics K), then with
-// inertial terms (g 2 | b 6 | sf 6 | ts 1); rows / columns of constant parameters are zero like ceres::Covariance's.
+// inertial terms (g 2 | b 6 | sf 6 | ts 1); rows / columns of constant or unused parameters (fill_mask) are zero like
+// ceres::Covariance's.
 extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   VC_TRY(prepare(h));
