@@ -1,7 +1,8 @@
 // IMU residual family on the device and the block-tridiagonal frame chain it induces.
 //
-//   imu_eval_kernel      one warp per frame interval, one tangent direction per lane (forward-mode
-//                        dual numbers through the RK4 integrator): r (9) and J (9x33)
+//   imu_eval_kernel      three frame intervals per warp, a team of 10 lanes each: a lane carries one attitude-coupled
+//                        tangent direction through the RK4 integrator (forward-mode dual numbers) and two (p, v)-only
+//                        or end-map-only columns beside it: r (9) and J (9x33)
 //                        [SwitchedFullImuCostFunction, ceres-cost-functions.h:379-490]
 //   imu_accumulate_kernel adds J^T J of the two intervals touching a frame into the frame blocks
 //                        (B, off-diagonal U, E columns of the 15 IMU globals, gradients)
@@ -48,9 +49,10 @@ __device__ __forceinline__ void se3_local_column(const double* x, int col, doubl
   }
 }
 
-// the same fields as ImuEvalArgs / ImuAccArgs with the problem description by reference
+// the fields of ImuEvalArgs the evaluation reads, by value (the persistent kernel passes them to a __noinline__ task
+// function: a reference to its parameter block would force the whole block into local memory)
 struct ImuEvalView {
-  const DevProblem& dp;
+  struct { int64_t off_v, off_imu; int rotation_only; } dp;
   imu::ImuBuf buf;
   const double* ftime;
   const double* wsqrt;
@@ -59,6 +61,7 @@ struct ImuEvalView {
   int ni, apply_loss;
   double mult;
 };
+// the same fields as ImuAccArgs with the problem description by reference
 struct ImuAccView {
   const DevProblem& dp;
   const double *r, *J;
@@ -67,104 +70,146 @@ struct ImuAccView {
 };
 
 constexpr int kImuWarps = 4;
+// An interval's 33 Jacobian columns by a team of 10 lanes, 3 teams per warp (lanes 30, 31 idle).  p and v never feed
+// back into the integrator, so only 10 columns reach the attitude: pose1 rotation 9-11, gyro bias 20-22, gyro scale
+// 26-28 and ts 32.  Team lane t carries column imu_col_chain(t) through the RK4 chain as a dual number, and two more
+// columns that need only the end map T_end T2^-1 -> log: imu_col_acc(t) (accelerometer bias 23-25 and scale 29-31 on
+// lanes 0-5, an AccelTangent of the chain; gravity 18-19 and v1 15-16 on lanes 6-9) and imu_col_end(t) (pose2 0-5,
+// pose1 translation 6-8, v1 17).  The v2 columns 12-14 are analytic.
+constexpr int kImuTeam = 10, kImuTeams = 3;
+__device__ __forceinline__ int imu_col_chain(int t) { return t < 3 ? 9 + t : t < 6 ? 17 + t : t < 9 ? 20 + t : 32; }
+__device__ __forceinline__ int imu_col_acc(int t) { return t < 3 ? 23 + t : t < 6 ? 26 + t : t < 8 ? 12 + t : 7 + t; }
+__device__ __forceinline__ int imu_col_end(int t) { return t < 9 ? t : 17; }
 
-// residual (9) and tangent Jacobian (9 x 33) of interval k by one warp: lane -> Jacobian column
+// residual (9) and tangent Jacobian (9 x 33) of interval k by team lane t (0..9) of its team
 // A: ImuEvalArgs or a view with the same fields (the persistent kernel binds `dp` by reference to its own parameter)
 template <class A>
-__device__ __forceinline__ void imu_eval_interval(const A& a, int k, int lane, const double* state) {
+__device__ __forceinline__ void imu_eval_team(const A& a, int k, int t, const double* state) {
   using imu::D1;
-  // lane -> Jacobian column: pose2 0-5 | pose1 6-11 | (v2 12-14 analytic) | v1 15-17 | g 18-19 | b 20-25 | sf 26-31 | ts 32
-  const int col = lane < 12 ? lane : lane + 3;
+  const int cc = imu_col_chain(t);
   const double* X2 = state + 7 * static_cast<int64_t>(k + 1);
   const double* X1 = state + 7 * static_cast<int64_t>(k);
   const double* V2 = state + a.dp.off_v + 3 * static_cast<int64_t>(k + 1);
   const double* V1 = state + a.dp.off_v + 3 * static_cast<int64_t>(k);
   const double* P = state + a.dp.off_imu;  // g2 b6 sf6 ts
-  double s2[7], s1[7];
-  se3_local_column(X2, col < 6 ? col : 0, s2);
-  se3_local_column(X1, (col >= 6 && col < 12) ? col - 6 : 0, s1);
-  D1 x2[7], x1[7], v2[3], v1[3], g2[2], b[6], sf[6], ts;
+  double s1[7];
+  se3_local_column(X1, t < 3 ? 3 + t : 0, s1);
+  D1 x1[7], v1[3], g2[2], b[6], sf[6], ts;
 #pragma unroll
-  for (int i = 0; i < 7; ++i) {
-    x2[i] = D1(X2[i], col < 6 ? s2[i] : 0.0);
-    x1[i] = D1(X1[i], (col >= 6 && col < 12) ? s1[i] : 0.0);
-  }
+  for (int i = 0; i < 7; ++i) x1[i] = D1(X1[i], t < 3 ? s1[i] : 0.0);
 #pragma unroll
-  for (int i = 0; i < 3; ++i) {
-    v2[i] = D1(V2[i], 0.0);
-    v1[i] = D1(V1[i], col == 15 + i ? 1.0 : 0.0);
-  }
-  g2[0] = D1(P[0], col == 18 ? 1.0 : 0.0);
-  g2[1] = D1(P[1], col == 19 ? 1.0 : 0.0);
+  for (int i = 0; i < 3; ++i) v1[i] = D1(V1[i], 0.0);
+  g2[0] = D1(P[0], 0.0);
+  g2[1] = D1(P[1], 0.0);
 #pragma unroll
   for (int i = 0; i < 6; ++i) {
-    b[i] = D1(P[2 + i], col == 20 + i ? 1.0 : 0.0);
-    sf[i] = D1(P[8 + i], col == 26 + i ? 1.0 : 0.0);
+    b[i] = D1(P[2 + i], cc == 20 + i ? 1.0 : 0.0);
+    sf[i] = D1(P[8 + i], cc == 26 + i ? 1.0 : 0.0);
   }
-  ts = D1(P[14], col == 32 ? 1.0 : 0.0);
-  D1 raw[9];
-  const bool ok = imu::imu_raw_residual<D1>(a.buf, a.ftime[k], a.ftime[k + 1], x2, x1, v2, v1, g2, b, sf, ts, raw);
+  ts = D1(P[14], cc == 32 ? 1.0 : 0.0);
+  imu::AccelTangent at{t < 6 ? t % 3 : 0, t < 3 ? 1.0 : 0.0, (t >= 3 && t < 6) ? 1.0 : 0.0};
+  imu::Pose<D1> y;
+  const bool ok = imu::imu_integrate<D1>(a.buf, a.ftime[k], a.ftime[k + 1], x1, v1, g2, b, sf, ts, &y, at);
   const double* W = a.wsqrt + static_cast<int64_t>(k) * 81;
   double* rk = a.r + static_cast<int64_t>(k) * 9;
   double* Jk = a.J + static_cast<int64_t>(k) * 297;
+  const bool zero_rows = a.dp.rotation_only && (t < 3 || t >= 6);  // of row t, for the v2 columns
   if (!ok) {  // no measurements: zero residual (ceres-cost-functions.h:452-455)
-    if (lane == 0) {
+    if (t == 0) {
       for (int j = 0; j < 9; ++j) rk[j] = 0.0;
       a.cost[k] = 0.0;
     }
     for (int j = 0; j < 9; ++j) {
-      if (lane < 30) Jk[j * 33 + col] = 0.0;
-      if (lane >= 30) { Jk[j * 33 + 12] = 0.0; Jk[j * 33 + 13] = 0.0; Jk[j * 33 + 14] = 0.0; }
+      Jk[j * 33 + cc] = 0.0;
+      Jk[j * 33 + imu_col_acc(t)] = 0.0;
+      Jk[j * 33 + imu_col_end(t)] = 0.0;
     }
+    if (t < 9) { Jk[t * 33 + 12] = 0.0; Jk[t * 33 + 13] = 0.0; Jk[t * 33 + 14] = 0.0; }
     return;
   }
-  // residuals_vec = (r^T W)^T  (:476-477); rotation-only switch zeroes rows 0-2 and 6-8 (:479-482)
-  D1 rw[9];
-  double s = 0.0;
+  D1 x2[7], v2[3];
 #pragma unroll
-  for (int j = 0; j < 9; ++j) {
-    double va = 0.0, vv = 0.0;
+  for (int i = 0; i < 7; ++i) x2[i] = D1(X2[i], 0.0);
 #pragma unroll
-    for (int i = 0; i < 9; ++i) {
-      va += raw[i].a * W[i * 9 + j];
-      vv += raw[i].v * W[i * 9 + j];
+  for (int i = 0; i < 3; ++i) v2[i] = D1(V2[i], 0.0);
+  double sc = 1.0;
+  // e = 0: the chain's column; e = 1, 2: end-map-only columns, their (p, v) tangents assembled from the seeds and `at`
+#pragma unroll 1
+  for (int e = 0; e < 3; ++e) {
+    const int c = e == 0 ? cc : e == 1 ? imu_col_acc(t) : imu_col_end(t);
+    imu::Pose<D1> ye = y;
+    if (e > 0) {
+      double s[7];
+      se3_local_column(X2, c < 6 ? c : 0, s);
+#pragma unroll
+      for (int i = 0; i < 7; ++i) x2[i].v = c < 6 ? s[i] : 0.0;
+      se3_local_column(X1, (c >= 6 && c < 9) ? c - 6 : 0, s);
+      const bool tr = c >= 6 && c < 9, acc = e == 1 && t < 6;
+      const imu::Vec<double> dp0{tr ? s[4] : 0.0, tr ? s[5] : 0.0, tr ? s[6] : 0.0};
+      const imu::Vec<double> dv0{c == 15 ? 1.0 : 0.0, c == 16 ? 1.0 : 0.0, c == 17 ? 1.0 : 0.0};
+      const imu::Vec<D1> gv = imu::gravity_vector<D1>(D1(P[0], c == 18 ? 1.0 : 0.0), D1(P[1], c == 19 ? 1.0 : 0.0));
+      const imu::Vec<double> dg{gv.x.v, gv.y.v, gv.z.v};
+      const double T = at.dur;
+      const imu::Vec<double> dp = dp0 + imu::scale(dv0, T) - imu::scale(dg, 0.5 * T * T) +
+                                  (acc ? at.dp : imu::Vec<double>{0.0, 0.0, 0.0});
+      const imu::Vec<double> dv = dv0 - imu::scale(dg, T) + (acc ? at.dv : imu::Vec<double>{0.0, 0.0, 0.0});
+      ye.p = {D1(y.p.x.a, dp.x), D1(y.p.y.a, dp.y), D1(y.p.z.a, dp.z)};
+      ye.q = {D1(y.q.x.a, 0.0), D1(y.q.y.a, 0.0), D1(y.q.z.a, 0.0), D1(y.q.w.a, 0.0)};
+      ye.v = {D1(y.v.x.a, dv.x), D1(y.v.y.a, dv.y), D1(y.v.z.a, dv.z)};
     }
-    const bool off = a.dp.rotation_only && (j < 3 || j >= 6);
-    rw[j] = off ? D1(0.0, 0.0) : D1(va, vv);
-    s += rw[j].a * rw[j].a;
-  }
-  double sc = 1.0, cost = 0.5 * s;
-  if (a.apply_loss) {
-    double rho0, rho1;
-    cauchy(s, &rho0, &rho1);  // CauchyLoss(100), vicalibrator.h:133
-    cost = 0.5 * rho0 * a.mult;
-    sc = sqrt(rho1);
-  }
-  if (lane == 0) {
-#pragma unroll
-    for (int j = 0; j < 9; ++j) rk[j] = rw[j].a * sc;
-    a.cost[k] = cost;
-  }
-  const double m = (col >= 18 && col < 33) ? a.mask[col - 18] : 1.0;  // lanes 30, 31 carry no column
-  if (lane < 30) {
-#pragma unroll
-    for (int j = 0; j < 9; ++j) Jk[j * 33 + col] = rw[j].v * sc * m;
-  } else if (lane == 30) {
-    // d r / d v2 = -W[6+i][:]  (v_end - v2 enters rows 6-8 of the raw residual)
+    D1 raw[9];
+    imu::imu_end_residual<D1>(ye, x2, v2, raw);
+    // residuals_vec = (r^T W)^T  (:476-477); rotation-only switch zeroes rows 0-2 and 6-8 (:479-482)
+    D1 rw[9];
+    double s = 0.0;
 #pragma unroll
     for (int j = 0; j < 9; ++j) {
-      const bool off = a.dp.rotation_only && (j < 3 || j >= 6);
+      double va = 0.0, vv = 0.0;
 #pragma unroll
-      for (int i = 0; i < 3; ++i) Jk[j * 33 + 12 + i] = off ? 0.0 : -W[(6 + i) * 9 + j] * sc;
+      for (int i = 0; i < 9; ++i) {
+        va += raw[i].a * W[i * 9 + j];
+        vv += raw[i].v * W[i * 9 + j];
+      }
+      const bool off = a.dp.rotation_only && (j < 3 || j >= 6);
+      rw[j] = off ? D1(0.0, 0.0) : D1(va, vv);
+      s += rw[j].a * rw[j].a;
     }
+    if (e == 0) {  // the residual is the same on every column's pass
+      double cost = 0.5 * s;
+      if (a.apply_loss) {
+        double rho0, rho1;
+        cauchy(s, &rho0, &rho1);  // CauchyLoss(100), vicalibrator.h:133
+        cost = 0.5 * rho0 * a.mult;
+        sc = sqrt(rho1);
+      }
+      if (t == 0) {
+#pragma unroll
+        for (int j = 0; j < 9; ++j) rk[j] = rw[j].a * sc;
+        a.cost[k] = cost;
+      }
+    }
+    const double m = c >= 18 ? a.mask[c - 18] : 1.0;
+#pragma unroll
+    for (int j = 0; j < 9; ++j) Jk[j * 33 + c] = rw[j].v * sc * m;
+  }
+  // d r / d v2 = -W[6+i][:]  (v_end - v2 enters rows 6-8 of the raw residual): row t by team lane t
+  if (t < 9) {
+#pragma unroll
+    for (int i = 0; i < 3; ++i) Jk[t * 33 + 12 + i] = zero_rows ? 0.0 : -W[(6 + i) * 9 + t] * sc;
   }
 }
 
+// intervals kImuTeams * task + 0..2 by one warp
+template <class A>
+__device__ __forceinline__ void imu_eval_warp(const A& a, int task, int lane, const double* state) {
+  const int k = task * kImuTeams + lane / kImuTeam;
+  if (lane < kImuTeams * kImuTeam && k < a.ni) imu_eval_team(a, k, lane % kImuTeam, state);
+}
+
 __global__ void __launch_bounds__(32 * kImuWarps) imu_eval_kernel(ImuEvalArgs a) {
-  const int lane = threadIdx.x & 31;
-  const int k = blockIdx.x * kImuWarps + (threadIdx.x >> 5);
-  if (k >= a.ni || a.ctl->done) return;
-  imu_eval_interval(a, k, lane, a.states[a.which ? 1 - a.ctl->cur : a.ctl->cur]);
+  const int task = blockIdx.x * kImuWarps + (threadIdx.x >> 5);
+  if (task * kImuTeams >= a.ni || a.ctl->done) return;
+  imu_eval_warp(a, task, threadIdx.x & 31, a.states[a.which ? 1 - a.ctl->cur : a.ctl->cur]);
 }
 
 // ---------------------------------------------------------------- IMU -> frame blocks

@@ -1,8 +1,8 @@
 // eval_kernel — the evaluation half of an inertial trust-region iteration in ONE cooperative launch (one CTA of 256
 // threads per SM), grid barriers where the multi-launch engine has launch boundaries:
 //
-//   T  warp tasks from one queue (longest first): IMU residual + 9x33 Jacobian of an interval (lane per tangent
-//      direction, vc_imu.cuh) | reprojection evaluate + Gram build of a frame (build_frame_warp, vc_fused.cuh, as
+//   T  warp tasks from one queue (longest first): IMU residuals + 9x33 Jacobians of three intervals (a team of 10
+//      lanes each, vc_imu.cuh) | reprojection evaluate + Gram build of a frame (build_frame_warp, vc_fused.cuh, as
 //      lm_mega_kernel's phase B): frame block, E, gradient, per-(frame, camera) packed global block
 //   -- grid barrier
 //   A  per frame (one warp): J^T J of the two intervals touching the frame into B, U, E, gradient, and
@@ -110,6 +110,12 @@ __device__ __noinline__ void eval_weights(const WeightQueueArgs w, const double*
   }
 }
 
+// Phase T's IMU task: intervals 3 task + 0..2 by one warp.  A function of its own, as eval_weights: inlined, the
+// teams' registers join the kernel's and both spill more.
+__device__ __noinline__ void eval_imu_task(const ImuEvalView a, int task, int lane, const double* x) {
+  imu_eval_warp(a, task, lane, x);
+}
+
 // The evaluation of the rig `a` by the CTAs of `scope` (vc_mega.cuh): the cooperative grid (eval_mega_kernel) or one
 // thread-block cluster (eval_mega_batch_kernel; never sharded: the exchange is compiled out for it).
 template <class Scope>
@@ -153,16 +159,17 @@ __device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
 
   // ------------------------------------------------------------ T: task queue — IMU intervals first, then frames
   {
-    const ImuEvalView ia{a.dp, a.buf, a.ftime, a.wsqrt, a.mask + a.dp.imu_goff, a.imu_r, a.imu_J, a.imu_cost, ni, 1, a.dp.imu_mult};
+    const ImuEvalView ia{{a.dp.off_v, a.dp.off_imu, a.dp.rotation_only}, a.buf, a.ftime, a.wsqrt, a.mask + a.dp.imu_goff, a.imu_r, a.imu_J, a.imu_cost, ni, 1, a.dp.imu_mult};
     double* slab = smem + static_cast<size_t>(warp) * kWarpDoubles;
-    const unsigned n_tasks = static_cast<unsigned>(ni + nf);
+    const unsigned n_imu = static_cast<unsigned>((ni + kImuTeams - 1) / kImuTeams);
+    const unsigned n_tasks = n_imu + static_cast<unsigned>(nf);
     for (;;) {
       unsigned t = 0;
       if (lane == 0) t = atomicAdd(a.counter, 1u);
       t = __shfl_sync(0xffffffffu, t, 0);
       if (t >= n_tasks) break;
-      if (t < static_cast<unsigned>(ni)) imu_eval_interval(ia, static_cast<int>(t), lane, x);
-      else evm_build_frame(a, bt, x, static_cast<int>(t) - ni, slab, smCam, smRc, tri_lut, lane);
+      if (t < n_imu) eval_imu_task(ia, static_cast<int>(t), lane, x);
+      else evm_build_frame(a, bt, x, static_cast<int>(t - n_imu), slab, smCam, smRc, tri_lut, lane);
     }
   }
   mark(kEvProfTasks);

@@ -1,6 +1,6 @@
 // Device-side IMU residual math: RK4 integration of (p, q, v) through interpolated gyro / accel
-// samples, the SE3 log residual, and a one-direction dual number so a warp evaluates the 9x33
-// tangent Jacobian with one lane per direction.
+// samples, the SE3 log residual, a one-direction dual number for the tangent directions that reach the
+// attitude, and the (p, v)-only tangents that ride along the same chain in plain doubles (AccelTangent).
 //
 // Reference being reproduced:
 //   SwitchedFullImuCostFunction::operator()   ceres-cost-functions.h:402-484
@@ -198,29 +198,73 @@ template <class T> __device__ inline Pose<T> integrate_pose(const Pose<T>& y0, c
 }
 // ceres-cost-functions.h:79-105
 template <class T> __device__ inline void pose_derivative(const Pose<T>& y, Vec<T> g, const Meas<T>& z0, const Meas<T>& z1,
-                                                          Vec<T> bg, Vec<T> ba, const T sf[6], T dt, T k[9]) {
+                                                          Vec<T> bg, Vec<T> ba, const T sf[6], T dt, T k[9],
+                                                          Vec<T>* za_out = nullptr) {
   const T alpha = (z1.time - (z0.time + dt)) / (z1.time - z0.time), oma = T(1.0) - alpha;
   const Vec<T> zg = scale(z0.w, alpha) + scale(z1.w, oma);
   const Vec<T> za = scale(z0.a, alpha) + scale(z1.a, oma);
+  if (za_out) *za_out = za;
   k[0] = y.v.x; k[1] = y.v.y; k[2] = y.v.z;
   const Vec<T> w = qrot(y.q, Vec<T>{zg.x * sf[0] + bg.x, zg.y * sf[1] + bg.y, zg.z * sf[2] + bg.z});
   k[3] = w.x; k[4] = w.y; k[5] = w.z;
   const Vec<T> a = qrot(y.q, Vec<T>{za.x * sf[3] + ba.x, za.y * sf[4] + ba.y, za.z * sf[5] + ba.z}) - g;
   k[6] = a.x; k[7] = a.y; k[8] = a.z;
 }
-// ceres-cost-functions.h:138-177 (RK4)
-template <class T> __device__ inline Pose<T> integrate_imu(const Pose<T>& y0, const Meas<T>& z0, const Meas<T>& z1, Vec<T> bg,
-                                                           Vec<T> ba, const T sf[6], Vec<T> g) {
+// A (p, v)-only tangent carried beside the RK4 chain in plain doubles.  k[3..8] depend on q and the measurements but
+// never on p or v, so a direction that moves neither q, the gyro terms nor the sample times (pose1 translation, v1,
+// gravity, accelerometer bias and scale) never reaches q: along it k_v moves by R(q_s) du_s - dg at stage s, with
+// du_s = (fb + fz za_s[ax]) e_ax the derivative of the accelerometer term, and k_p by the velocity tangent.  This
+// accumulates the accelerometer part along the attitude path the chain integrates (RK4 per step:
+// dv += dt/6 (b1 + 2 b2 + 2 b3 + b4), dp += dt dv + dt^2/6 (b1 + b2 + b3)) and the integrated time `dur`; the seeds'
+// own part is linear in it (dp0 + dur dv0 - dur^2/2 dg, dv0 - dur dg) and is added by the caller.
+struct AccelTangent {
+  int ax;          // du = (fb + fz za[ax]) e_ax
+  double fb, fz;
+  double dur = 0.0;
+  Vec<double> dp{0.0, 0.0, 0.0}, dv{0.0, 0.0, 0.0};
+  Vec<double> b3, b6;  // b1 + b2 + b3 and b1 + 2 b2 + 2 b3 + b4 of the current step
+  template <class T_>
+  __device__ __forceinline__ void stage(int s, const Quat<T_>& q, const Vec<T_>& za) {
+    const double u = fb + fz * (ax == 0 ? val(za.x) : ax == 1 ? val(za.y) : val(za.z));
+    const Vec<double> b = qrot(Quat<double>{val(q.x), val(q.y), val(q.z), val(q.w)},
+                               Vec<double>{ax == 0 ? u : 0.0, ax == 1 ? u : 0.0, ax == 2 ? u : 0.0});
+    if (s == 0) {
+      b3 = b;
+      b6 = b;
+    } else if (s < 3) {
+      b3 = b3 + b;
+      b6 = b6 + scale(b, 2.0);
+    } else {
+      b6 = b6 + b;
+    }
+  }
+  __device__ __forceinline__ void step(double dt) {
+    dp = dp + scale(dv, dt) + scale(b3, dt * dt / 6.0);
+    dv = dv + scale(b6, dt / 6.0);
+    dur += dt;
+  }
+};
+
+// ceres-cost-functions.h:138-177 (RK4); `at` follows an AccelTangent along the step
+template <class T, class AT>
+__device__ inline Pose<T> integrate_imu(const Pose<T>& y0, const Meas<T>& z0, const Meas<T>& z1, Vec<T> bg, Vec<T> ba,
+                                        const T sf[6], Vec<T> g, AT& at) {
   if (val(z1.time) == val(z0.time)) return y0;
   const T dt = z1.time - z0.time;
   T k1[9], k2[9], k3[9], k4[9];
-  pose_derivative(y0, g, z0, z1, bg, ba, sf, T(0.0), k1);
+  Vec<T> za;
+  pose_derivative(y0, g, z0, z1, bg, ba, sf, T(0.0), k1, &za);
+  at.stage(0, y0.q, za);
   const Pose<T> y1 = integrate_pose(y0, k1, dt * T(0.5));
-  pose_derivative(y1, g, z0, z1, bg, ba, sf, dt / T(2.0), k2);
+  pose_derivative(y1, g, z0, z1, bg, ba, sf, dt / T(2.0), k2, &za);
+  at.stage(1, y1.q, za);
   const Pose<T> y2 = integrate_pose(y0, k2, dt * T(0.5));
-  pose_derivative(y2, g, z0, z1, bg, ba, sf, dt / T(2.0), k3);
+  pose_derivative(y2, g, z0, z1, bg, ba, sf, dt / T(2.0), k3, &za);
+  at.stage(2, y2.q, za);
   const Pose<T> y3 = integrate_pose(y0, k3, dt);
-  pose_derivative(y3, g, z0, z1, bg, ba, sf, dt, k4);
+  pose_derivative(y3, g, z0, z1, bg, ba, sf, dt, k4, &za);
+  at.stage(3, y3.q, za);
+  at.step(val(dt));
 #pragma unroll
   for (int i = 0; i < 9; ++i) k1[i] = k1[i] + T(2.0) * k2[i] + T(2.0) * k3[i] + k4[i];
   return integrate_pose(y0, k1, dt / T(6.0));
@@ -235,12 +279,11 @@ template <class T> __device__ inline Vec<T> gravity_vector(T p, T q) {
   return {cp * sq * mg, -sp * mg, cp * cq * mg};
 }
 
-// Unweighted residual (log(T_end * T_2^-1), v_end - v2); returns false when the interval has no
-// measurements (ceres-cost-functions.h:452-455).  `end` (optional) receives the integrated pose.
-template <class T>
-__device__ inline bool imu_raw_residual(const ImuBuf& buf, double t_start, double t_end, const T x2[7], const T x1[7],
-                                        const T v2[3], const T v1[3], const T g2[2], const T b[6], const T sf[6], T ts,
-                                        T r[9], Pose<T>* end = nullptr) {
+// The pose and velocity at t_end integrated from (x1, v1) at t_start (ceres-cost-functions.h:440-470); returns false
+// when the interval has no measurements (:452-455).  `at` follows an AccelTangent along the way.
+template <class T, class AT>
+__device__ inline bool imu_integrate(const ImuBuf& buf, double t_start, double t_end, const T x1[7], const T v1[3],
+                                     const T g2[2], const T b[6], const T sf[6], T ts, Pose<T>* end, AT& at) {
   // HasElement (interpolation-buffer.h:122-125)
   if (!(t_start >= buf.start_time + val(ts) && t_start <= buf.end_time + val(ts)) || buf.n == 0) return false;
   const Vec<T> g = gravity_vector<T>(g2[0], g2[1]);
@@ -251,10 +294,16 @@ __device__ inline bool imu_raw_residual(const ImuBuf& buf, double t_start, doubl
   bool more = true;
   while (more) {
     more = get_next<T>(buf, t_end, ts, &idx, &cur);
-    y = integrate_imu(y, prev, cur, bg, ba, sf, g);
+    y = integrate_imu(y, prev, cur, bg, ba, sf, g, at);
     prev = cur;
   }
-  if (end) *end = y;
+  *end = y;
+  return true;
+}
+
+// Unweighted residual of the integrated end state y: (log(T_end * T_2^-1), v_end - v2)
+template <class T>
+__device__ inline void imu_end_residual(const Pose<T>& y, const T x2[7], const T v2[3], T r[9]) {
   // T_end * T_2^-1
   const Quat<T> q2i = qconj(Quat<T>{x2[0], x2[1], x2[2], x2[3]});
   const Vec<T> t2i = qrot(q2i, Vec<T>{x2[4], x2[5], x2[6]});
@@ -264,7 +313,6 @@ __device__ inline bool imu_raw_residual(const ImuBuf& buf, double t_start, doubl
   r[6] = y.v.x - v2[0];
   r[7] = y.v.y - v2[1];
   r[8] = y.v.z - v2[2];
-  return true;
 }
 
 }  // namespace imu
