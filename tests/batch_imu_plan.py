@@ -1,5 +1,5 @@
 """Host model of vcgpu_solve_batch_inertial's launch plan (imu_batch_cluster_size and the grouping of
-run_solve_batch_inertial, vc_engine.inl), in plain Python.
+run_solve_batch_inertial, vc_batch.inl), in plain Python.
 
 A rig runs inside one thread-block cluster of the persistent inertial kernels.  How many CTAs the cluster has is a
 function of the rig alone: the fewest of 1, 2, 4, 8 whose elimination groups (GROUPS per CTA) take the chunks of level

@@ -1,4 +1,4 @@
-"""Host model of vcgpu_solve_batch's launch plan (batch_cluster_size and the grouping of run_solve_batch, vc_engine.inl),
+"""Host model of vcgpu_solve_batch's launch plan (batch_cluster_size and the grouping of run_solve_batch, vc_batch.inl),
 in plain Python.
 
 A rig runs inside one thread-block cluster.  How many CTAs the cluster has is a function of the rig alone: the fewest

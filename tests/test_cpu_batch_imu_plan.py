@@ -20,8 +20,8 @@ def test_cluster_size_boundaries():
     assert [cs(n) for n in (24, 200, 256)] == [2, 8, 8]
 
 
-def test_source_states_the_same_rule():
-    src = open(os.path.join(ROOT, "vicalib_b200", "csrc", "vc_engine.inl")).read()
+def test_batch_source_states_the_same_rule():
+    src = open(os.path.join(ROOT, "vicalib_b200", "csrc", "vc_batch.inl")).read()
     body = re.search(r"static int imu_batch_cluster_size\(int n_frames\) \{(.*?)\n\}", src, re.S).group(1)
     assert "const int chunks = (n_frames + kCsChunk - 1) / kCsChunk;" in body
     assert "while (size < 8 && size * kCsGroups < chunks) size *= 2;" in body

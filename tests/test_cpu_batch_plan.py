@@ -22,8 +22,8 @@ def test_cluster_size_boundaries():
     assert cs(10, 1) == 8
 
 
-def test_source_states_the_same_rule():
-    src = open(os.path.join(ROOT, "vicalib_b200", "csrc", "vc_engine.inl")).read()
+def test_batch_source_states_the_same_rule():
+    src = open(os.path.join(ROOT, "vicalib_b200", "csrc", "vc_batch.inl")).read()
     body = re.search(r"static int batch_cluster_size\(int n_frames, int warps\) \{(.*?)\n\}", src, re.S).group(1)
     assert "while (size < 8 && size * warps < n_frames) size *= 2;" in body
 

@@ -232,6 +232,8 @@ def _refused(handles, index):
 
 
 def test_refusals():
+    from vicalib_b200.capi import VcgpuError
+
     kw = dict(models=("poly3",), n_frames=30, grid=(10, 7))
     opts = dict(max_iters=4, **TOL0)
     fresh = Rig(seed=700, opts=opts, **kw).solo()
@@ -244,8 +246,8 @@ def test_refusals():
             r.g.set_flags(**changes["flags"])
         if "options" in changes:
             r.g.set_options(**changes["options"])
-        if "profiling" in changes:
-            r.g.set_profiling(changes["profiling"], False)
+        if "profiling" in changes or "flush" in changes:
+            r.g.set_profiling(changes.get("profiling", 0), changes.get("flush", False))
         return r
 
     _refused([], None)                                   # n = 0
@@ -255,10 +257,13 @@ def test_refusals():
             bad_with(options=dict(update_state_every_iteration=1)),
             bad_with(profiling=1), bad_with(profiling=2), bad_with(profiling=MULTI_LAUNCH),
             Rig(models=("poly3",), n_frames=12, grid=(14, 10), inertial=True, seed=703, flags=dict(inertial=1), opts=opts),
-            Rig(models=chain_plan.rig_with_globals(104, False), n_frames=12, grid=(14, 10), seed=704, opts=opts)]  # beyond the fit
+            Rig(models=chain_plan.rig_with_globals(104, False), n_frames=12, grid=(14, 10), seed=704, opts=opts),  # beyond the fit
+            bad_with(flush=True)]                        # L2 flushing
     for bad in bads:
         _refused([good[0].g, good[1].g, bad.g], 2)
         _refused([bad.g, good[0].g], 0)
+        with pytest.raises(VcgpuError):                  # the plan query refuses what the batch refuses
+            bad.g.batch_plan()
     # nothing ran: every handle of the refused batches solves alone as a fresh one does, in as many launches
     _same_bits(good[0].solo(), fresh, "after the refusals")
     _same_bits(good[1].solo(), ref1, "after the refusals")

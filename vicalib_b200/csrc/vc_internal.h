@@ -190,15 +190,10 @@ struct vcgpu_handle {
   unsigned long long* d_prof = nullptr;
   int dev_sms = 0, dev_smem_optin = 0;
   int mega_grid = 0, mega_warps[2] = {0, 0};  // [strategy]; 0 warps: does not fit / not supported, use the multi-launch engine
-  vc::MegaArgs* d_batch_args = nullptr;  // vcgpu_solve_batch: the rigs of a launch group (held by the group's first handle)
-  // vcgpu_solve_batch_inertial: the rigs of the batch as the solve [2 parities][n] and evaluation [start, iteration][n]
-  // batch kernels take them (held by the batch's first handle)
-  vc::ChainSolveArgs* d_batch_cs = nullptr;
-  vc::EvalMegaArgs* d_batch_ev = nullptr;
-  // vcgpu_get_covariance_batch: the batch's vision and inertial rigs as the covariance kernels take them (held by the
-  // batch's first handle), and this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
-  vc::CovArgs* d_batch_cov = nullptr;
-  vc::ChainCovArgs* d_batch_ccov = nullptr;
+  // the batch calls (vc_batch.inl): the kernel arguments of every rig of a batch this handle was handle 0 of, laid out
+  // by the call
+  unsigned char* d_batch_args = nullptr;
+  // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)
   bool imu_mega_ok = false;

@@ -5,14 +5,15 @@
 // loop (TrustRegionMinimizer + LevenbergMarquardtStrategy, SURVEY App. A.3) driven from the host
 // with every arithmetic step — the accept/reject decision included — on the device; the candidate
 // point is evaluated *with* its Jacobian blocks (speculatively) so an accepted step needs no second
-// pass.  Engines: vc_mega.cuh (persistent kernel, vision solves) and vc_engine.inl (multi-launch).
+// pass.  Engines: vc_mega.cuh (persistent kernel, vision solves) and vc_engine.inl (multi-launch); the batch
+// calls, one thread-block cluster per rig: vc_batch.inl.
 #include <algorithm>
+#include <array>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <numeric>
-#include <tuple>
 
 #include <nccl.h>
 
@@ -217,7 +218,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_batch_cs); dev_free(&h->d_batch_ev); dev_free(&h->d_batch_cov); dev_free(&h->d_batch_ccov); dev_free(&h->d_cov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_cov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -751,6 +752,7 @@ static int prepare(vcgpu_handle* h) {
 }
 
 #include "vc_engine.inl"
+#include "vc_batch.inl"
 
 extern "C" int vcgpu_solve(vcgpu_handle* h, vcgpu_iter_cb cb, void* user, vcgpu_summary* out) {
   if (!h) return VCGPU_ERR_INVALID;
@@ -969,26 +971,17 @@ extern "C" int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const dou
 extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   VC_TRY(prepare(h));
-  VC_TRY(ctl_reset(h, 0, 0));
-  VC_TRY(evaluate_into(h, 0, false, -1));
+  std::vector<double> mask, D2;
+  VC_TRY(cov_prelude(h, &mask, &D2));
   const DevProblem& dp = h->dp;
   const int G = dp.G;
   const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + G;
-  std::vector<double> mask;
-  fill_mask(h, &mask);
   const Blocks& b = h->blk[h->cur];
-  std::vector<double> gf0(nfp), gc0(G), D2(np, 0.0), col(G, 0.0), x(np);
+  // the gradient, which the unit right-hand sides replace, is put back after the solves
+  std::vector<double> gf0(nfp), gc0(G), sc(G), col(G, 0.0), x(np);
   CUDA_TRY(h, cudaMemcpyAsync(gf0.data(), b.gf, nfp * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(gc0.data(), b.gc, G * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  for (int k = 0; k < G; ++k) D2[nfp + k] = mask[k] != 0.0 ? 0.0 : 1.0;  // constant columns are empty: keep the system definite
-  // Jacobi-scaled like the trust-region steps (focal lengths next to distortion coefficients and a time offset: the raw
-  // J^T J does not survive an unpivoted Cholesky): cov = S (S H S)^-1 S
-  jacobi_scale_kernel<<<static_cast<int>((np + 255) / 256), 256, 0, h->stream>>>(dp, h->blk[0], h->blk[1], h->d_ctl, h->d_scale, nullptr);
-  ++h->launches;
-  std::vector<double> sc(G);
   CUDA_TRY(h, cudaMemcpyAsync(sc.data(), h->d_scale + nfp, G * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_scale + np, D2.data(), np * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(b.gf, 0, nfp * sizeof(double), h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   std::fill(cov, cov + static_cast<size_t>(G) * G, 0.0);
