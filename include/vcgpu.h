@@ -245,6 +245,20 @@ int vcgpu_get_covariance(vcgpu_handle* h, double* cov);
  * arguments per rig, held by handle 0. */
 int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov /* n pointers */,
                                int* status /* n, or NULL */);
+/* Marginal covariance of every frame's tangent (ceres::Covariance::GetCovarianceBlock(t_wp, t_wp), and (v_w, v_w) with
+ * the inertial terms on): the [frame f, frame f] blocks of (J^T J)^-1 at the current state, on the system
+ * vcgpu_get_covariance inverts (undamped J^T J, constant or unused globals taken out).  cov: n_frames blocks of fd x fd,
+ * row-major, in upload order; fd is 6, or 9 with the inertial terms on, and a block's rows follow the frame's rows of
+ * vcgpu_normal_equations' B.  Each block is exactly symmetric.  A vision frame no active observation sees gets a block
+ * of exactly 0.0, and the other blocks are those of the problem without it; so do the velocity rows and columns of a
+ * rotation-only run, which no residual reads.  Computed by a selected inversion of the
+ * frame elimination: no dense inverse of J^T J is formed.  Nothing on the handle changes: state, IMU weights and what a
+ * later vcgpu_solve computes stay as they were.
+ * VCGPU_ERR_NUMERIC: J^T J is not positive definite at the current state; cov is not written.  VCGPU_ERR_INVALID: a
+ * null argument, or frame shards (the call is one-GPU only).
+ * Device memory, kept on the handle: vision G^2 + 36 n_frames doubles; inertial (G + 9 t)^2 + 81 n_frames + about
+ * 8/7 n_frames (162 + 9 G) doubles, t <= 4 the nodes of the chain's top level. */
+int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov /* n_frames * fd * fd */);
 
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */

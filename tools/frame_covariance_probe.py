@@ -1,0 +1,67 @@
+"""Frame covariance next to the covariance of the globals, on the benchmark's target workload and on config 2.
+
+    python tools/frame_covariance_probe.py
+
+Prints the card, its power limit and SM clocks, then per workload (target: 2 x poly3 + IMU, 2000 frames, every IMU
+flag on; config2: 1 x poly3, 2000 frames), after K LM iterations: the wall time of vcgpu_get_frame_covariance and of
+vcgpu_get_covariance, each the best of RUNS alternating calls after a warm-up, and the device time of each call's kernels
+from one torch.profiler run of its own.  Reads device settings, changes none.
+"""
+import os
+import subprocess
+import sys
+import time
+
+import torch  # noqa: F401  (before libvcgpu.so: torch's CUDA library needs its own NCCL symbols first)
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from vicalib_b200 import synth
+from vicalib_b200.capi import Calibrator
+
+K, RUNS = 10, 5
+ALL_ON = dict(inertial=1, rotation_only=0, bias_active=1, scale_active=1, optimize_ts=1)
+try:  # read-only query: a number is only meaningful next to the card, its power limit and clocks
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True, timeout=30).stdout.strip()
+except (OSError, subprocess.SubprocessError):
+    card = "unknown (nvidia-smi not available)"
+print(f"card (name, power limit, SM clock now, SM clock max): {card}\n{K} LM iterations before the calls, best of {RUNS}")
+
+
+def wall(fn):
+    t = time.perf_counter()
+    fn()  # every call ends in a device synchronise (its copy back)
+    return time.perf_counter() - t
+
+
+def device_ms(fn):
+    from torch.profiler import ProfilerActivity, profile
+
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+    torch.cuda.synchronize()
+    us = sum(e.device_time_total for e in prof.key_averages() if e.device_time_total > 0 and e.key != "Memcpy DtoH (Device -> Pageable)"
+             and not e.key.startswith("Memcpy") and not e.key.startswith("Memset"))
+    return us / 1e3
+
+
+for name in ("target", "config2"):
+    p = synth.make_config(name)
+    g = Calibrator(device=0)
+    g.load(p)
+    g.set_flags(**(ALL_ON if p.inertial else {}))
+    g.set_options(max_iters=K, function_tol=0.0, gradient_tol=0.0, param_tol=0.0)
+    g.solve()
+    calls = {"frame_covariance": g.frame_covariance, "covariance": g.covariance}
+    for fn in calls.values():
+        fn()
+    best = {k: float("inf") for k in calls}
+    for _ in range(RUNS):
+        for k, fn in calls.items():
+            best[k] = min(best[k], wall(fn))
+    dev = {k: device_ms(fn) for k, fn in calls.items()}
+    fc = g.frame_covariance()
+    print(f"{name}: {p.n_frames} frames, fd {g.fd}, G {g.G}; frame blocks {fc.shape}, all finite {bool((fc == fc).all())}")
+    for k in calls:
+        print(f"  {k:17s} wall {best[k] * 1e3:9.2f} ms   kernels {dev[k]:9.2f} ms")
+    g.close()

@@ -25,6 +25,7 @@ EXPORTS = [
     "vcgpu_get_state", "vcgpu_num_residuals", "vcgpu_frame_dim", "vcgpu_num_globals", "vcgpu_eval_reproj",
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
+    "vcgpu_get_frame_covariance",
     "vcgpu_pose_pnp_ransac",
 ]
 
@@ -326,6 +327,14 @@ class Calibrator:
         G = self.G
         cov = np.zeros((G, G))
         self._chk(self.L.vcgpu_get_covariance(self.h, _p(cov)))
+        return cov
+
+    def frame_covariance(self):
+        """GetCovarianceBlock(t_wp, t_wp) (and (v_w, v_w) with the inertial terms on) of every frame:
+        (n_frames, fd, fd), each frame's tangent in the order of its rows in normal_equations()' B"""
+        fd = self.fd
+        cov = np.zeros((self.n_frames, fd, fd))
+        self._chk(self.L.vcgpu_get_frame_covariance(self.h, _p(cov)))
         return cov
 
     def phase_clocks(self):

@@ -323,6 +323,12 @@ __global__ void __launch_bounds__(256) sum_partials_kernel(const double* part, i
   }
 }
 
+// Blocks of the inverse of a level's system (vcgpu_get_frame_covariance, vc_frame_cov.cuh), in the scaled system: per
+// node Σ_kk [n][FD*FD], Σ_k,k+1 [n][FD*FD] (zero for the last node) and Σ_kg [n][FD*G]
+struct SigmaLevel {
+  double *kk, *kn, *kg;
+};
+
 // dense solve of [globals | top-level chain nodes]
 struct DenseArgs {
   DevProblem dp;
@@ -337,8 +343,10 @@ struct DenseArgs {
   int n_slots;         // frame blocks in the dense system (single GPU: top.n; sharded: one per rank)
   int slot_of[4];      // dense slot of each local top node
   int add_globals;     // 1: this rank contributes C + D and -g_c (exactly one rank does)
-  int mode;            // 0: assemble + solve; 1: assemble the local partial into buf only; 2: solve the (summed) buf
+  int mode;            // 0: assemble + solve; 1: assemble the local partial into buf only; 2: solve the (summed) buf;
+                       // 3: assemble + invert: the whole inverse into buf [N*N], the top nodes' blocks of it into sig
   double* buf;         // [N*N + N], N = G + n_slots*FD
+  SigmaLevel sig;      // mode 3
 };
 template <int FD>
 __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
@@ -413,6 +421,34 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
       if (k <= i) S[i * N + k] -= S[i * N + j] * S[k * N + j];
     }
     __syncthreads();
+  }
+  if (a.mode == 3) {
+    // N unit right-hand sides through the factor, one column per thread: L y = e_j (y is zero above row j), L^T x = y
+    double* X = a.buf;
+    for (int j = tid; j < N; j += 256) {
+      for (int i = j; i < N; ++i) {
+        double t = i == j ? 1.0 : 0.0;
+        for (int k = j; k < i; ++k) t -= S[i * N + k] * X[static_cast<int64_t>(k) * N + j];
+        X[static_cast<int64_t>(i) * N + j] = t / S[i * N + i];
+      }
+      for (int i = N - 1; i >= 0; --i) {
+        double t = i >= j ? X[static_cast<int64_t>(i) * N + j] : 0.0;
+        for (int k = i + 1; k < N; ++k) t -= S[k * N + i] * X[static_cast<int64_t>(k) * N + j];
+        X[static_cast<int64_t>(i) * N + j] = t / S[i * N + i];
+      }
+    }
+    __syncthreads();
+    if (bad && tid == 0) a.scalars[kScNotPD] = 1.0;
+    for (int e = tid; e < nt * FD * FD; e += 256) {
+      const int t = e / (FD * FD), r = (e / FD) % FD, q = e % FD, o = G + a.slot_of[t] * FD;
+      a.sig.kk[e] = X[static_cast<int64_t>(o + r) * N + o + q];
+      a.sig.kn[e] = t + 1 < nt ? X[static_cast<int64_t>(o + r) * N + G + a.slot_of[t + 1] * FD + q] : 0.0;
+    }
+    for (int e = tid; e < nt * FD * G; e += 256) {
+      const int t = e / (FD * G), r = (e / G) % FD, q = e % G, o = G + a.slot_of[t] * FD;
+      a.sig.kg[e] = X[static_cast<int64_t>(o + r) * N + q];
+    }
+    return;
   }
   if (tid < 32) {  // warp-cooperative triangular solves (column oriented), L L^T x = rhs
     const int lane = tid;

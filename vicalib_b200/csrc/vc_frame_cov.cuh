@@ -1,0 +1,248 @@
+// Marginal covariance of every frame's tangent (vcgpu_get_frame_covariance): the [f, f] blocks of (J^T J)^-1, by a
+// selected inversion of the frame elimination the solve already runs.  Everything here works in the Jacobi-scaled
+// system S H S that the eliminations factor; the last step unscales.
+//
+// Vision (fd = 6, block-diagonal frames): Σ_ff = B_f^-1 + W_f Σ_gg W_f^T with W_f = B_f^-1 E_f, the X that
+// frame_solve_kernel stores, and Σ_gg the inverse of the reduced system.
+//
+// Inertial (fd = 9, block-tridiagonal frames): the chain elimination (vc_chain.cuh) keeps, for every eliminated node p
+// of a level, its solution against the chunk's boundary y = (left separator, right separator, globals):
+// x_p = -Z_g - M_p x_y with M_p = Z_p[:, 0:2FD+G].  With the interior's block-tridiagonal matrix T (its inverse K)
+// and Σ_yy from the level above, the inverse restricted to the chunk is
+//   Σ_py = -M_p Σ_yy,   Σ_pq = K_pq + M_p Σ_yy M_q^T.
+// The walk starts at the inverse of the dense [globals | top nodes] system and goes down the levels; at every level it
+// keeps what the level below needs as its boundary: Σ_kk, Σ_k,k+1 and Σ_kg of every node (SigmaLevel).
+#pragma once
+#include "vc_chain.cuh"
+
+namespace vc {
+
+// ---------------------------------------------------------------- vision: one warp per frame
+struct FrameCovArgs {
+  DevProblem dp;
+  Blocks b[2];
+  const Ctl* ctl;
+  const double* scale;
+  const double* D2x;           // the frames' damping (0, or 1 on a frame no active observation sees)
+  const double* X;             // [nf][FD][G+1] of frame_solve_kernel: B_f^-1 [E_f | g_f]
+  const double* Sgg;           // [G*G] inverse of the reduced system
+  const uint8_t* frame_used;   // [nf]
+  double* out;                 // [nf][FD*FD]
+};
+constexpr int kFrameCovWarps = 4;
+
+template <int FD>
+__global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(FrameCovArgs a) {
+  constexpr int NP = FD * (FD + 1) / 2;  // lower triangle, row by row
+  const int lane = threadIdx.x & 31, f = blockIdx.x * kFrameCovWarps + (threadIdx.x >> 5);
+  if (f >= a.dp.n_frames) return;
+  double* out = a.out + static_cast<int64_t>(f) * FD * FD;
+  if (!a.frame_used[f]) {
+    for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
+    return;
+  }
+  const Blocks& b = a.b[a.ctl->cur];
+  const int G = a.dp.G, M = G + 1;
+  const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
+  const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+  // W Σ_gg W^T: the lanes split the columns q of P = W Σ_gg and sum P[r][q] W[c][q] over their own columns
+  double acc[NP];
+#pragma unroll
+  for (int t = 0; t < NP; ++t) acc[t] = 0.0;
+  for (int q = lane; q < G; q += 32) {
+    double p[FD];
+#pragma unroll
+    for (int r = 0; r < FD; ++r) p[r] = 0.0;
+    for (int k = 0; k < G; ++k) {
+      const double s = a.Sgg[static_cast<int64_t>(k) * G + q];
+#pragma unroll
+      for (int r = 0; r < FD; ++r) p[r] += Xf[r * M + k] * s;
+    }
+    int t = 0;
+#pragma unroll
+    for (int r = 0; r < FD; ++r)
+#pragma unroll
+      for (int c = 0; c <= r; ++c) acc[t++] += p[r] * Xf[c * M + q];
+  }
+#pragma unroll
+  for (int t = 0; t < NP; ++t)
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) acc[t] += __shfl_xor_sync(0xffffffffu, acc[t], o);
+  // B_f^-1: every lane factors the damped, scaled block (as frame_solve_kernel); lane c solves column c
+  const double* Bf = b.B + static_cast<int64_t>(f) * FD * FD;
+  double L[FD][FD], iL[FD];
+#pragma unroll
+  for (int i = 0; i < FD; ++i)
+#pragma unroll
+    for (int j = 0; j <= i; ++j) L[i][j] = Bf[i * FD + j] * sf[i] * sf[j] + (i == j ? a.D2x[static_cast<int64_t>(f) * FD + i] : 0.0);
+  frame_chol<FD>(L, iL);  // a failed pivot is flagged by frame_solve_kernel, which factored the same block
+  if (lane < FD) {
+    double x[FD];
+#pragma unroll
+    for (int i = 0; i < FD; ++i) {
+      double t = i == lane ? 1.0 : 0.0;
+#pragma unroll
+      for (int k = 0; k < i; ++k) t -= L[i][k] * x[k];
+      x[i] = t * iL[i];
+    }
+#pragma unroll
+    for (int i = FD - 1; i >= 0; --i) {
+      double t = x[i];
+#pragma unroll
+      for (int k = i + 1; k < FD; ++k) t -= L[k][i] * x[k];
+      x[i] = t * iL[i];
+    }
+    int t = 0;
+#pragma unroll
+    for (int r = 0; r < FD; ++r)
+#pragma unroll
+      for (int c = 0; c <= r; ++c, ++t)
+        if (c == lane) {
+          const double v = (x[r] + acc[t]) * (sf[r] * sf[c]);
+          out[r * FD + c] = v;
+          out[c * FD + r] = v;
+        }
+  }
+}
+
+// ---------------------------------------------------------------- inertial: one CTA per chunk of a level
+struct SelinvArgs {
+  int G, c;
+  ChainLevel cur;          // level l, as the elimination left it (A + addA, U, Z)
+  SigmaLevel sig, up;      // level l's blocks (written) and level l+1's (read)
+  const double* Sgg;       // Σ_gg, leading dimension ldg
+  int ldg;
+  double* scalars;
+};
+
+// dynamic shared memory of chain_selinv_kernel<FD> with chunks of c nodes: T [(c-1) FD]^2 | K [(c-1) FD]^2 |
+// P [(c-1) FD][2 FD + G]
+template <int FD>
+__host__ inline size_t chain_selinv_smem_bytes(int G, int c) {
+  const size_t nT = static_cast<size_t>(c - 1) * FD;
+  return (2 * nT * nT + nT * (2 * FD + static_cast<size_t>(G))) * sizeof(double);
+}
+
+// entry (k, q) of the boundary covariance Σ_yy of chunk j, y = (node j, node j+1 of level l+1, globals)
+template <int FD>
+__device__ __forceinline__ double selinv_boundary(const SelinvArgs& a, int j, bool hasR, int k, int q) {
+  const int G = a.G;
+  const int bk = k < FD ? 0 : k < 2 * FD ? 1 : 2, bq = q < FD ? 0 : q < 2 * FD ? 1 : 2;
+  if (!hasR && (bk == 1 || bq == 1)) return 0.0;
+  if (bk == 2 && bq == 2) return a.Sgg[static_cast<int64_t>(k - 2 * FD) * a.ldg + (q - 2 * FD)];
+  if (bq == 2) return a.up.kg[static_cast<int64_t>(j + bk) * FD * G + (k - bk * FD) * G + (q - 2 * FD)];
+  if (bk == 2) return a.up.kg[static_cast<int64_t>(j + bq) * FD * G + (q - bq * FD) * G + (k - 2 * FD)];
+  if (bk == bq) return a.up.kk[static_cast<int64_t>(j + bk) * FD * FD + (k - bk * FD) * FD + (q - bq * FD)];
+  if (bk == 0) return a.up.kn[static_cast<int64_t>(j) * FD * FD + k * FD + (q - FD)];
+  return a.up.kn[static_cast<int64_t>(j) * FD * FD + q * FD + (k - FD)];
+}
+
+template <int FD>
+__global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs a) {
+  extern __shared__ double sm[];
+  const int G = a.G, c = a.c, tid = threadIdx.x, ny = 2 * FD + G, w = ny + 1;
+  const ChainLevel& L = a.cur;
+  const int j = blockIdx.x, s = j * c, n = L.n;
+  const int m = min(c - 1, n - 1 - s);  // interior nodes s+1 .. s+m
+  const bool hasR = s + c < n;          // right separator: node s+m+1 here, node j+1 at level l+1
+  const int nT = m * FD;
+  double* T = sm;           // [nT][nT] the interior's block-tridiagonal matrix, then its Cholesky factor
+  double* K = T + nT * nT;  // [nT][nT] its inverse
+  double* P = K + nT * nT;  // [m][FD][ny] M_p Σ_yy
+  __shared__ int bad;
+  if (tid == 0) bad = 0;
+  for (int e = tid; e < nT * nT; e += kChainThreads) {
+    const int r = e / nT, q = e - r * nT, br = r / FD, bq = q / FD, rr = r - br * FD, qq = q - bq * FD;
+    const int64_t p = s + 1 + min(br, bq);
+    double v = 0.0;
+    if (br == bq) v = L.A[p * FD * FD + rr * FD + qq] + (L.addA ? L.addA[p * FD * FD + rr * FD + qq] : 0.0);
+    else if (bq == br + 1) v = L.U[(p + 1) * FD * FD + rr * FD + qq];  // H[p, p+1]
+    else if (br == bq + 1) v = L.U[(p + 1) * FD * FD + qq * FD + rr];  // H[p+1, p] = H[p, p+1]^T
+    T[e] = v;
+  }
+  for (int e = tid; e < nT * ny; e += kChainThreads) {
+    const int rp = e / ny, q = e - rp * ny;  // rp = i FD + r
+    const double* z = L.Z + (static_cast<int64_t>(s + 1) * FD + rp) * w;
+    double sum = 0.0;
+    for (int k = 0; k < ny; ++k) sum += z[k] * selinv_boundary<FD>(a, j, hasR, k, q);
+    P[e] = sum;
+  }
+  __syncthreads();
+  for (int jj = 0; jj < nT; ++jj) {  // T = L L^T, in place (lower triangle)
+    if (tid == 0) {
+      double d = T[jj * nT + jj];
+      if (!(d > 0.0)) { bad = 1; d = 1.0; }
+      T[jj * nT + jj] = sqrt(d);
+    }
+    __syncthreads();
+    const double dj = T[jj * nT + jj];
+    for (int i = jj + 1 + tid; i < nT; i += kChainThreads) T[i * nT + jj] /= dj;
+    __syncthreads();
+    const int rem = nT - jj - 1;
+    for (int e = tid; e < rem * rem; e += kChainThreads) {
+      const int i = jj + 1 + e / rem, k = jj + 1 + e % rem;
+      if (k <= i) T[i * nT + k] -= T[i * nT + jj] * T[k * nT + jj];
+    }
+    __syncthreads();
+  }
+  for (int col = tid; col < nT; col += kChainThreads) {  // K = T^-1, one column per thread
+    for (int i = col; i < nT; ++i) {
+      double t = i == col ? 1.0 : 0.0;
+      for (int k = col; k < i; ++k) t -= T[i * nT + k] * K[k * nT + col];
+      K[i * nT + col] = t / T[i * nT + i];
+    }
+    for (int i = nT - 1; i >= 0; --i) {
+      double t = i >= col ? K[i * nT + col] : 0.0;
+      for (int k = i + 1; k < nT; ++k) t -= T[k * nT + i] * K[k * nT + col];
+      K[i * nT + col] = t / T[i * nT + i];
+    }
+  }
+  __syncthreads();
+  if (bad && tid == 0) a.scalars[kScNotPD] = 1.0;
+  // the interior nodes: Σ_pp, Σ_p,p+1 (p+1 interior, or the right separator: -M_p Σ_y,right), Σ_pg = -(M_p Σ_yy)[:, g]
+  for (int e = tid; e < m * FD * FD; e += kChainThreads) {
+    const int i = e / (FD * FD), r = (e / FD) % FD, q = e % FD;
+    const int64_t p = s + 1 + i;
+    const double* Pr = P + (i * FD + r) * ny;
+    const double* zq = L.Z + (p * FD + q) * w;
+    double kk = K[(i * FD + r) * nT + i * FD + q];
+    for (int k = 0; k < ny; ++k) kk += Pr[k] * zq[k];
+    double kn = 0.0;
+    if (i + 1 < m) {
+      const double* zn = L.Z + ((p + 1) * FD + q) * w;
+      kn = K[(i * FD + r) * nT + (i + 1) * FD + q];
+      for (int k = 0; k < ny; ++k) kn += Pr[k] * zn[k];
+    } else if (hasR) {
+      kn = -Pr[FD + q];
+    }
+    a.sig.kk[p * FD * FD + r * FD + q] = kk;
+    a.sig.kn[p * FD * FD + r * FD + q] = kn;
+  }
+  for (int e = tid; e < m * FD * G; e += kChainThreads) {
+    const int i = e / (FD * G), r = (e / G) % FD, q = e % G;
+    a.sig.kg[(static_cast<int64_t>(s + 1 + i) * FD + r) * G + q] = -P[(i * FD + r) * ny + 2 * FD + q];
+  }
+  // the chunk's left separator: node j of level l+1; its next node is the first interior one (or the right separator)
+  for (int e = tid; e < FD * FD; e += kChainThreads) {
+    const int r = e / FD, q = e % FD;
+    a.sig.kk[static_cast<int64_t>(s) * FD * FD + e] = a.up.kk[static_cast<int64_t>(j) * FD * FD + e];
+    a.sig.kn[static_cast<int64_t>(s) * FD * FD + e] =
+        m > 0 ? -P[q * ny + r] : (hasR ? a.up.kn[static_cast<int64_t>(j) * FD * FD + e] : 0.0);
+  }
+  for (int e = tid; e < FD * G; e += kChainThreads)
+    a.sig.kg[static_cast<int64_t>(s) * FD * G + e] = a.up.kg[static_cast<int64_t>(j) * FD * G + e];
+}
+
+// Level 0's Σ_ff unscaled, s_f Σ_ff s_f, and exactly symmetric: both halves are written from the lower triangle.  Rows
+// and columns from `live` on (the velocities of a rotation-only run, which no residual reads) are 0.
+template <int FD>
+__global__ void __launch_bounds__(256) frame_cov_out_kernel(int n_frames, int live, const double* kk, const double* scale,
+                                                            double* out) {
+  const int64_t e = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= static_cast<int64_t>(n_frames) * FD * FD) return;
+  const int64_t f = e / (FD * FD);
+  const int r = static_cast<int>((e / FD) % FD), q = static_cast<int>(e % FD), hi = max(r, q), lo = min(r, q);
+  out[e] = hi < live ? kk[f * FD * FD + hi * FD + lo] * (scale[f * FD + hi] * scale[f * FD + lo]) : 0.0;
+}
+
+}  // namespace vc

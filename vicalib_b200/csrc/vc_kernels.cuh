@@ -696,6 +696,32 @@ __device__ __forceinline__ void schur_accumulate(double* Sacc, const double* sta
   }
 }
 
+// Cholesky factor of a frame block held in registers: the lower triangle of L is overwritten by the factor and iL gets
+// the reciprocals of its pivots.  A pivot that is not positive is taken as 1; the return value is false then.
+template <int FD>
+__device__ __forceinline__ bool frame_chol(double (&L)[FD][FD], double (&iL)[FD]) {
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < FD; ++j) {
+    double d = L[j][j];
+#pragma unroll
+    for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
+    if (!(d > 0.0)) { ok = false; d = 1.0; }
+    d = sqrt(d);
+    L[j][j] = d;
+    const double inv = 1.0 / d;
+    iL[j] = inv;
+#pragma unroll
+    for (int i = j + 1; i < FD; ++i) {
+      double t = L[i][j];
+#pragma unroll
+      for (int k = 0; k < j; ++k) t -= L[i][k] * L[j][k];
+      L[i][j] = t * inv;
+    }
+  }
+  return ok;
+}
+
 // One warp per frame: every lane factors the (damped, scaled) FD x FD block in registers and the
 // lanes split the right-hand-side columns [E | g]; the CTA then accumulates E^T X for its four
 // frames (schur_accumulate).
@@ -730,25 +756,7 @@ __global__ void __launch_bounds__(kSolveThreads) frame_solve_kernel(SolveArgs a)
           if (i == j) v += frame_damp<FD>(0.0, f, i, bij, s[i], rinv, a.D2x, nullptr, 0, a.dp.ghost && f == a.dp.n_frames - 1);
           L[i][j] = v;
         }
-      bool ok = true;
-#pragma unroll
-      for (int j = 0; j < FD; ++j) {
-        double d = L[j][j];
-#pragma unroll
-        for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
-        if (!(d > 0.0)) { ok = false; d = 1.0; }
-        d = sqrt(d);
-        L[j][j] = d;
-        const double inv = 1.0 / d;
-        iL[j] = inv;
-#pragma unroll
-        for (int i = j + 1; i < FD; ++i) {
-          double t = L[i][j];
-#pragma unroll
-          for (int k = 0; k < j; ++k) t -= L[i][k] * L[j][k];
-          L[i][j] = t * inv;
-        }
-      }
+      const bool ok = frame_chol<FD>(L, iL);
       if (!ok && lane == 0) a.scalars[kScNotPD] = 1.0;
       double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
       for (int c = lane; c < M; c += 32) {

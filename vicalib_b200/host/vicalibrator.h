@@ -476,6 +476,19 @@ class ViCalibrator {
     return cov;
   }
 
+  // GetCovarianceBlock(t_wp, t_wp) for every frame, and (v_w, v_w) when the inertial terms are on: the marginal
+  // covariance of each frame's tangent at the current solution, NumFrames() blocks of fd x fd row-major (fd: 6 | 9, the
+  // frame's rows of the normal equations).  A frame no active observation sees has a zero block.  Call after the solve
+  // has finished (not while IsRunning()).
+  std::vector<double> GetFrameCovariance(int* frame_dim = nullptr) {
+    int fd = 0;
+    Check(vcgpu_frame_dim(h_, &fd), "frame_dim");
+    std::vector<double> cov(NumFrames() * fd * fd, 0.0);
+    Check(vcgpu_get_frame_covariance(h_, cov.data()), "get_frame_covariance");
+    if (frame_dim) *frame_dim = fd;
+    return cov;
+  }
+
   // Pose seeds for AddFrame: what VicalibTask::AddSuperFrame computes per frame and camera with
   // calibu::PosePnPRansac(camera, ellipses, target.Circles3D(), ellipse_target_map, 0, 0, &t_cw) and
   // t_wp = t_cw.inverse() * t_ck (src/vicalib-task.cc:322-325, 341-349) — here for ALL views in one device call.
