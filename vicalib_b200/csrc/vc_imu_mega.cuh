@@ -55,7 +55,7 @@ struct ChainSolveArgs {
   const ChainLevel* lev;        // [n_levels] level descriptors (device memory)
   int n_levels;
   double* Spart;                // [grid][G*G+G] one Schur partial per CTA, packed (chain_sacc_doubles(G) entries used)
-  double* Ssum;                 // [G*G+G]
+  double* Ssum;                 // [G*G+G] summed Schur complement; chain_solve_kernel on one GPU: the dense system [RT][LD]
   double* delta;                // scaled step [nf*9 + G]
   double* scalars;
   double* state[2];
@@ -569,6 +569,70 @@ __device__ __forceinline__ void chain_backsub_level(const ChainLevel cur, int l,
   for (int t = gw; t < n_slots; t += nw) chain_backsub_node<FD>(cur, l, delta, nfp, G, t, lane);
 }
 
+// The back-substitution of every level on the cooperative grid, by whichever CTA calls it: items of kCsBsItem nodes at
+// level 0 and of one node per warp above it (the levels above have 28 and 224 nodes on the target: items of 16 would
+// leave most warps idle and double the rounds of those that work), levels top-down (the items of level l after all those of the levels above), off the counter sync[3].  An item of the
+// top level waits for sync[2] (1 once the dense solve has written the globals' and the top nodes' steps), an item of a
+// lower level for the count of finished items sync[4] to cover every level above — items are handed out in order, so
+// that count cannot include one of its own level before.  wait_all: return when every item is done (the update reads
+// every frame's step).  A function of its own with by-value arguments, as chain_weights_queue: inlined into the solve
+// kernel it raised the kernel's spills.  prof: CTA 0's phase clocks (thread 0 only, else null), t_prev the time of
+// its last mark; returns the time of the last mark here.
+template <int FD>
+__device__ __noinline__ unsigned long long chain_backsub_items(const ChainLevel* lev, int n_levels, double* delta, int64_t nfp, int G,
+                                                               unsigned long long* sync, bool wait_all, unsigned long long* wtask,
+                                                               unsigned long long* prof, unsigned long long t_prev) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  unsigned long long* ready = sync + 2;
+  unsigned long long* items = sync + 3;
+  unsigned long long* done = sync + 4;
+  auto item_nodes = [](int l) { return l == 0 ? kCsBsItem : kCsThreads / 32; };
+  auto level_items = [&](int l) { return (chain_backsub_slots(lev[l]) + item_nodes(l) - 1) / item_nodes(l); };
+  auto mark = [&](int l) {  // the time since the last mark to back-substitution level l's clock
+    if (prof) {
+      const unsigned long long t = global_ns();
+      prof[kCsProfBacksub + (n_levels - 2 - l)] += t - t_prev;
+      t_prev = t;
+    }
+  };
+  const int l_top = n_levels - 2;
+  int n_items = 0;
+  for (int l = l_top; l >= 0; --l) n_items += level_items(l);
+  int cl = l_top, n_cl = level_items(l_top);  // level of this CTA's current item, and its items
+  int before = 0;                             // items of the levels above cl
+  for (;;) {
+    if (tid == 0) *wtask = atomicAdd(items, 1ull);
+    __syncthreads();
+    const int it = static_cast<int>(*wtask);
+    if (it >= n_items) break;
+    while (it >= before + n_cl) {
+      mark(cl);
+      before += n_cl;
+      n_cl = level_items(--cl);
+    }
+    if (tid == 0) {
+      if (cl == l_top) spin_until(ready, 1ull);
+      else spin_until(done, static_cast<unsigned long long>(before));
+    }
+    __syncthreads();
+    const ChainLevel L = lev[cl];
+    const int nodes = item_nodes(cl);
+    for (int u = 0; u < nodes / (kCsThreads / 32); ++u)
+      chain_backsub_node<FD>(L, cl, delta, nfp, G, (it - before) * nodes + u * (kCsThreads / 32) + warp, lane);
+    __syncthreads();
+    if (tid == 0) {
+      __threadfence();
+      atomicAdd(done, 1ull);
+    }
+  }
+  mark(cl);
+  if (wait_all) {
+    if (tid == 0) spin_until(done, static_cast<unsigned long long>(n_items));
+    __syncthreads();
+  }
+  return t_prev;
+}
+
 // The deferred UpdateImuWeights as a function of its own (its own register allocation: inlined into the solve kernel
 // it is slower, with the solve's live values squeezed into the same 255 registers).  Everything by value — a
 // reference to the kernel's parameter block would force the whole block into local memory.
@@ -697,6 +761,82 @@ __device__ __noinline__ void dense_ldlt_tiles(double* S, int N, int LD, double* 
   }
   DenseTiles<T, 0>::run(R, S, N, LD, wd, bad, ti, tk);
   __syncthreads();
+}
+// entry k of the summed Schur complement: the nb CTAs' packed partials p[c * NS] added in CTA order, kCsRedLoads loads
+// in flight
+__device__ __forceinline__ double schur_entry(const double* p, int nb, int NS) {
+  double s = 0.0;
+  int c = 0;
+  for (; c + kCsRedLoads <= nb; c += kCsRedLoads) {
+    double v[kCsRedLoads];
+#pragma unroll
+    for (int u = 0; u < kCsRedLoads; ++u) v[u] = __ldcg(p + (c + u) * NS);
+#pragma unroll
+    for (int u = 0; u < kCsRedLoads; ++u) s += v[u];
+  }
+  for (; c < nb; ++c) s += __ldcg(p + c * NS);
+  return s;
+}
+// The [globals | top nodes] system of a run on one GPU as chain_solve's dense phase factors it — S [RT][LD] with the
+// right-hand side as row N and zeros everywhere else — written to a.Ssum, entries e0, e0 + stride, ...  First the
+// globals' block and right-hand side (an entry per thread of the solver CTAs, as the Schur reduction alone had: each
+// sums the nb partials), then the top nodes' blocks and the zeros.  Every entry is formed by the operations, in the
+// order, of the dense phase's own assembly (which sharded runs and clusters keep), so the system is bit for bit the same.
+__device__ __forceinline__ void dense_assemble(const ChainSolveArgs& a, const Blocks& b, double rinv, int nb, int e0, int stride) {
+  constexpr int FD = 9;
+  const int G = a.dp.G, NS = G * G + G;
+  const int64_t nfp = static_cast<int64_t>(a.dp.n_frames) * FD;
+  const ChainLevel& top = a.lev[a.n_levels - 1];
+  const int N = G + top.n * FD, LD = dense_ld(N), RT = dense_rows(N);
+  const double* sc = a.scale + nfp;
+  double* S = a.Ssum;
+  for (int e = e0; e < NS; e += stride) {
+    const int r = e / G, q = e - r * G;
+    const int k = r < G ? (q <= r ? r * (r + 1) / 2 + q : -1) : G * (G + 1) / 2 + q;
+    const double p = k >= 0 ? schur_entry(a.Spart + k, nb, NS) : 0.0;
+    const double cv = b.C[e];  // C | gc are contiguous
+    if (r < G) {
+      double v = cv * sc[r] * sc[q] - p;
+      if (r == q) v += global_damp(r, cv, sc[r], rinv, a.D2x, nfp);
+      S[r * LD + q] = v;
+    } else {
+      S[N * LD + q] = -cv * sc[q] + p;
+    }
+  }
+  const bool add = top.addA != nullptr;
+  auto entry = [&](int e) -> double {  // a top node's entry, or a zero
+    const int r = e / LD, c = e - r * LD;
+    double v = 0.0;
+    if (r <= N && c < N) {
+      const int tc = (c - G) / FD, cc = (c - G) - tc * FD;  // top node and row of column c (c >= G unless G <= r < N)
+      if (r == N) {
+        const int64_t o = static_cast<int64_t>(tc) * FD + cc;
+        v = -(__ldcg(top.g + o) + (add ? __ldcg(top.addg + o) : 0.0));
+      } else if (r < G) {  // E of top node tc, transposed
+        const int64_t o = static_cast<int64_t>(tc) * FD * G + cc * G + r;
+        v = __ldcg(top.E + o) + (add ? __ldcg(top.addE + o) : 0.0);
+      } else {
+        const int tr = (r - G) / FD, rr = (r - G) - tr * FD;
+        if (c < G) {
+          const int64_t o = static_cast<int64_t>(tr) * FD * G + rr * G + c;
+          v = __ldcg(top.E + o) + (add ? __ldcg(top.addE + o) : 0.0);
+        } else if (tc == tr) {
+          const int64_t o = static_cast<int64_t>(tr) * FD * FD + rr * FD + cc;
+          v = __ldcg(top.A + o) + (add ? __ldcg(top.addA + o) : 0.0);
+        } else if (tc == tr + 1) {
+          v = __ldcg(top.U + static_cast<int64_t>(tc) * FD * FD + rr * FD + cc);  // H[tr, tc]
+        } else if (tr == tc + 1) {
+          v = __ldcg(top.U + static_cast<int64_t>(tr) * FD * FD + cc * FD + rr);  // H[tc, tr] transposed
+        }
+      }
+    }
+    return v;
+  };
+  for (int e = e0; e < RT * LD; e += stride) {
+    const int r = e / LD, c = e - r * LD;
+    if (c < G && (r < G || r == N)) continue;  // written above
+    S[e] = entry(e);
+  }
 }
 // One damped solve of the frame-chain + globals system and (optionally) the state update of the rig `a`, by the CTAs
 // of `scope` (vc_mega.cuh): the cooperative grid (chain_solve_kernel) or one thread-block cluster (chain_solve_batch_kernel).
@@ -846,28 +986,23 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
   // CTA order, kCsRedLoads loads in flight (neighbouring threads read neighbouring entries), and writes it unpacked:
   // lower triangle, upper triangle 0, then the right-hand side.  32-bit offsets (grid x (G^2 + G) < 2^31 for G <= 127):
   // 64-bit ones cost the kernel more spills.
-  for (int e = bid * kCsThreads + tid; e < NS; e += ns * kCsThreads) {
-    const int r = e / G, q = e - r * G;
-    const int k = r < G ? (q <= r ? r * (r + 1) / 2 + q : -1) : G * (G + 1) / 2 + q;
-    double s = 0.0;
-    if (k >= 0) {
-      const double* p = a.Spart + k;
-      int c = 0;
-      for (; c + kCsRedLoads <= nb; c += kCsRedLoads) {
-        double v[kCsRedLoads];
-#pragma unroll
-        for (int u = 0; u < kCsRedLoads; ++u) v[u] = __ldcg(p + (c + u) * NS);
-#pragma unroll
-        for (int u = 0; u < kCsRedLoads; ++u) s += v[u];
-      }
-      for (; c < nb; ++c) s += __ldcg(p + c * NS);
+  // On the grid on one GPU the same threads assemble the dense system as CTA 0 factors it, in its padded [RT][LD]
+  // layout, in a.Ssum (sized for it): the operations of the assembly CTA 0 does otherwise, in the same order, so the
+  // system is bit for bit the same, and CTA 0 copies it in one round of asynchronous copies.
+  const bool sharded = Scope::kSharded && a.x.nranks > 1;
+  const bool assemble = kQueue && !sharded;
+  if (assemble) {
+    dense_assemble(a, b, rinv, nb, bid * kCsThreads + tid, ns * kCsThreads);
+  } else {
+    for (int e = bid * kCsThreads + tid; e < NS; e += ns * kCsThreads) {
+      const int r = e / G, q = e - r * G;
+      const int k = r < G ? (q <= r ? r * (r + 1) / 2 + q : -1) : G * (G + 1) / 2 + q;
+      a.Ssum[e] = k >= 0 ? schur_entry(a.Spart + k, nb, NS) : 0.0;
     }
-    a.Ssum[e] = s;
   }
   mark(kCsProfReduce);
   barrier(ns);
   // ------------------------------------------------------------ sharded: the ranks' partial systems meet here
-  const bool sharded = Scope::kSharded && a.x.nranks > 1;
   const int TB = chain_top_block(G);
   if (sharded) {
     const ChainLevel& top = a.lev[a.n_levels - 1];
@@ -937,6 +1072,10 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
     double* wd = S + RT * LD;  // 1 / d_j
     const double* sc = a.scale + nfp;
     if (tid == 0) bad_dense = 0;
+    if (assemble) {  // assembled by the Schur reduction (dense_assemble)
+      for (int e = tid; e < RT * LD; e += kCsThreads) cp_async8(S + e, a.Ssum + e);
+      cp_async_wait_all();
+    } else {
     for (int e = tid; e < RT * LD; e += kCsThreads) S[e] = 0.0;
     __syncthreads();
     if (sharded) {
@@ -1012,6 +1151,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
       }
       for (int e = tid; e < FD; e += kCsThreads)
         rhs[o + e] = -(__ldcg(top.g + static_cast<int64_t>(t) * FD + e) + (add ? __ldcg(top.addg + static_cast<int64_t>(t) * FD + e) : 0.0));
+    }
     }
     }
     // right-looking L D L^T on the lower triangle, the right-hand side riding along as row N.  The matrix lives in
@@ -1113,10 +1253,18 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
         for (int q = 0; q < 4; ++q) a.step_part[4 * static_cast<int64_t>(nb) + q] = g4[q];
       }
     }
+    if constexpr (kQueue) {  // the back-substitution may start: the globals' and the top nodes' steps are in a.delta
+      __syncthreads();
+      if (tid == 0) {
+        __threadfence();
+        atomicAdd(a.sync + 2, 1ull);
+      }
+    }
   }
   if constexpr (kCov) return;  // the other CTAs: nothing after the elimination
   if (prof) { const long long t = clock64(); a.prof[55] += static_cast<unsigned long long>(t - dt0); }
   mark(kCsProfDense);
+  if constexpr (kQueue) break;  // every level of the back-substitution is handed out in the closing phases
   if (a.n_levels <= 2) break;  // the next barrier is the one the whole grid meets at
   barrier(ns);
   // ------------------------------------------------------------ back-substitution, top-down, levels >= 1
@@ -1140,11 +1288,16 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
       continue;
     }
     // ---------------------------------------------------------- closing phases.  The CTAs that stayed with the solve
-    // get here when the levels above level 0 are back-substituted, the CTAs that left when the weights queue is empty.
-    // Nobody waits for everybody: level 0 is handed out in items of kCsBsItem nodes, off a counter, to whoever is here
-    // once the levels above are done — a CTA still busy with its last weights task holds up neither the
-    // back-substitution nor the update of the others (the queue used to keep them all at a grid barrier).  Which warp
-    // does a node changes nothing in its result, and the update keeps its fixed frames per CTA.
+    // get here when they are done with the solve, the CTAs that left when the weights queue is empty.  Nobody waits for
+    // everybody: the back-substitution is handed out in items of kCsBsItem nodes, off a counter, to whoever is here —
+    // a CTA still busy with its last weights task holds up neither the back-substitution nor the update of the others.
+    // On the grid every level is handed out so (chain_backsub_items).  A cluster hands out level 0 only, once its CTAs
+    // are done with the levels above.  Which warp does a node changes nothing in its result, and the update keeps its
+    // fixed frames per CTA.
+    if constexpr (kQueue) {
+      if (a.n_levels >= 2) t_prev = chain_backsub_items<FD>(a.lev, a.n_levels, a.delta, nfp, G, a.sync, a.do_update != 0, &wtask,
+                                                            prof ? a.prof : nullptr, t_prev);
+    } else {
     unsigned long long* ready = a.sync + 2;  // CTAs that stayed with the solve and are done with the levels above
     unsigned long long* items = a.sync + 3;  // level-0 items handed out
     unsigned long long* done = a.sync + 4;   // level-0 items finished
@@ -1179,6 +1332,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
         if (tid == 0) spin_until(done, static_cast<unsigned long long>(n_items));
         __syncthreads();
       }
+    }
     }
     if (!a.do_update) continue;
     // ---------------------------------------------------------- x (+) step of every frame, one thread each (the top
