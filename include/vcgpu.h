@@ -259,6 +259,20 @@ int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* cons
  * Device memory, kept on the handle: vision G^2 + 36 n_frames doubles; inertial (G + 9 t)^2 + 81 n_frames + about
  * 8/7 n_frames (162 + 9 G) doubles, t <= 4 the nodes of the chain's top level. */
 int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov /* n_frames * fd * fd */);
+/* vcgpu_get_frame_covariance of n independent rigs in one call, one thread-block cluster per rig; vision and inertial
+ * rigs may be mixed.  cov[i] receives rig i's blocks exactly as vcgpu_get_frame_covariance lays them out (n_frames_i
+ * blocks of fd_i x fd_i; equal to its result to rounding, each block exactly symmetric, the same exact zeros).  Each rig
+ * takes the cluster size its batch solve takes, a function of the rig alone, so its blocks are the same bits whatever
+ * else is in the batch and in whatever order.  Per handle, on its own stream, the point is evaluated; then one launch
+ * runs per group of like rigs; then one copy back per handle.  Nothing on the handle changes: state, IMU weights and what
+ * a later vcgpu_solve or batch solve computes stay as they were.
+ * status, VCGPU_ERR_NUMERIC and VCGPU_ERR_INVALID: as vcgpu_get_covariance_batch (the same refusals: n <= 0, a null or
+ * repeated handle, a null cov[i], handles on different devices, frame shards, any vcgpu_set_profiling bit or L2 flushing,
+ * and a rig the cluster kernels do not fit, which includes inertial G >= 68 on an H100).
+ * Device memory: per handle the workspace of vcgpu_get_frame_covariance and that of vcgpu_get_covariance_batch, and a few
+ * KB of kernel arguments per rig, held by handle 0. */
+int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov /* n pointers */,
+                                     int* status /* n, or NULL */);
 
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */

@@ -25,7 +25,7 @@ EXPORTS = [
     "vcgpu_get_state", "vcgpu_num_residuals", "vcgpu_frame_dim", "vcgpu_num_globals", "vcgpu_eval_reproj",
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
-    "vcgpu_get_frame_covariance",
+    "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch",
     "vcgpu_pose_pnp_ransac",
 ]
 
@@ -63,8 +63,8 @@ ITER_CB = C.CFUNCTYPE(C.c_int, C.POINTER(Iteration), C.c_void_p)
 
 
 class VcgpuError(RuntimeError):
-    """A negative return code of the library.  covariance_batch also sets `status` (one code per rig) and
-    `covariances` (the matrices written, None for the rigs whose system is not positive definite)."""
+    """A negative return code of the library.  covariance_batch and frame_covariance_batch also set `status` (one code
+    per rig) and `covariances` (the arrays written, None for the rigs whose system is not positive definite)."""
 
     status = None
     covariances = None
@@ -384,17 +384,31 @@ def covariance_batch(calibrators, out=None):
     rigs may be mixed), each rig in its own thread-block cluster.  Returns one G x G array per calibrator, in order;
     out: optional list of C-contiguous float64 (G, G) arrays to write into.  Raises VcgpuError; where some rigs' systems
     are not positive definite, the error's `status` gives every rig's code and `covariances` the other rigs' matrices."""
-    n = len(calibrators)
-    L = lib()
     if out is None:
         out = [None if g is None else np.zeros((g.G, g.G)) for g in calibrators]
+    return _covariances(lib().vcgpu_get_covariance_batch, "covariance_batch", calibrators, out)
+
+
+def frame_covariance_batch(calibrators, out=None):
+    """vcgpu_get_frame_covariance_batch: Calibrator.frame_covariance() of every Calibrator of the list (vision and
+    inertial rigs may be mixed), each rig in its own thread-block cluster.  Returns one (n_frames, fd, fd) array per
+    calibrator, in order; out: optional list of C-contiguous float64 arrays of that shape to write into.  Raises
+    VcgpuError as covariance_batch does."""
+    if out is None:
+        out = [None if g is None else np.zeros((g.n_frames, g.fd, g.fd)) for g in calibrators]
+    return _covariances(lib().vcgpu_get_frame_covariance_batch, "frame_covariance_batch", calibrators, out)
+
+
+def _covariances(entry, name, calibrators, out):
+    n = len(calibrators)
+    L = lib()
     for a in out:
         if a is not None and (a.dtype != np.float64 or not a.flags.c_contiguous):
-            raise ValueError("covariance_batch: out arrays must be C-contiguous float64")
+            raise ValueError(f"{name}: out arrays must be C-contiguous float64")
     hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
     ptrs = (C.c_void_p * max(n, 1))(*[None if a is None else a.ctypes.data for a in out])
     status = (C.c_int * max(n, 1))()
-    rc = L.vcgpu_get_covariance_batch(hs, C.c_int(n), ptrs, status)
+    rc = entry(hs, C.c_int(n), ptrs, status)
     if rc != 0:
         msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
         e = VcgpuError(f"vcgpu error {rc}: {msg}")

@@ -31,20 +31,14 @@ struct FrameCovArgs {
 };
 constexpr int kFrameCovWarps = 4;
 
+// Frame f's block B_f^-1 + X_f Σ_gg X_f^T, unscaled, by one warp (frame_cov_vision_kernel, cov_frame_mega_batch_kernel).
+// b, D2x: the blocks of the normal equations and the frames' damping; sf: frame f's Jacobi scale; Xf: X_f = B_f^-1 E_f,
+// [FD][ldx].  (B_f's address is formed after the product: held across it, it costs frame_cov_vision_kernel two registers.)
 template <int FD>
-__global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(FrameCovArgs a) {
+__device__ __forceinline__ void frame_cov_block(const Blocks& b, const double* D2x, int f, const double* sf, const double* Xf, int ldx,
+                                                const double* Sgg, int G, int lane, double* out) {
   constexpr int NP = FD * (FD + 1) / 2;  // lower triangle, row by row
-  const int lane = threadIdx.x & 31, f = blockIdx.x * kFrameCovWarps + (threadIdx.x >> 5);
-  if (f >= a.dp.n_frames) return;
-  double* out = a.out + static_cast<int64_t>(f) * FD * FD;
-  if (!a.frame_used[f]) {
-    for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
-    return;
-  }
-  const Blocks& b = a.b[a.ctl->cur];
-  const int G = a.dp.G, M = G + 1;
-  const double* Xf = a.X + static_cast<int64_t>(f) * FD * M;
-  const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+  const int M = ldx;
   // W Σ_gg W^T: the lanes split the columns q of P = W Σ_gg and sum P[r][q] W[c][q] over their own columns
   double acc[NP];
 #pragma unroll
@@ -54,7 +48,7 @@ __global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(F
 #pragma unroll
     for (int r = 0; r < FD; ++r) p[r] = 0.0;
     for (int k = 0; k < G; ++k) {
-      const double s = a.Sgg[static_cast<int64_t>(k) * G + q];
+      const double s = Sgg[static_cast<int64_t>(k) * G + q];
 #pragma unroll
       for (int r = 0; r < FD; ++r) p[r] += Xf[r * M + k] * s;
     }
@@ -74,8 +68,8 @@ __global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(F
 #pragma unroll
   for (int i = 0; i < FD; ++i)
 #pragma unroll
-    for (int j = 0; j <= i; ++j) L[i][j] = Bf[i * FD + j] * sf[i] * sf[j] + (i == j ? a.D2x[static_cast<int64_t>(f) * FD + i] : 0.0);
-  frame_chol<FD>(L, iL);  // a failed pivot is flagged by frame_solve_kernel, which factored the same block
+    for (int j = 0; j <= i; ++j) L[i][j] = Bf[i * FD + j] * sf[i] * sf[j] + (i == j ? D2x[static_cast<int64_t>(f) * FD + i] : 0.0);
+  frame_chol<FD>(L, iL);  // a failed pivot is flagged by the elimination, which factored the same block
   if (lane < FD) {
     double x[FD];
 #pragma unroll
@@ -105,6 +99,20 @@ __global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(F
   }
 }
 
+template <int FD>
+__global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(FrameCovArgs a) {
+  const int lane = threadIdx.x & 31, f = blockIdx.x * kFrameCovWarps + (threadIdx.x >> 5);
+  if (f >= a.dp.n_frames) return;
+  double* out = a.out + static_cast<int64_t>(f) * FD * FD;
+  if (!a.frame_used[f]) {
+    for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
+    return;
+  }
+  const Blocks& b = a.b[a.ctl->cur];
+  const int G = a.dp.G, M = G + 1;
+  frame_cov_block<FD>(b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, a.X + static_cast<int64_t>(f) * FD * M, M, a.Sgg, G, lane, out);
+}
+
 // ---------------------------------------------------------------- inertial: one CTA per chunk of a level
 struct SelinvArgs {
   int G, c;
@@ -115,77 +123,81 @@ struct SelinvArgs {
   double* scalars;
 };
 
-// dynamic shared memory of chain_selinv_kernel<FD> with chunks of c nodes: T [(c-1) FD]^2 | K [(c-1) FD]^2 |
-// P [(c-1) FD][2 FD + G]
+// shared memory of one chunk of c nodes (chain_selinv_chunk): T [(c-1) FD]^2 | K [(c-1) FD]^2 | P [(c-1) FD][2 FD + G]
 template <int FD>
-__host__ inline size_t chain_selinv_smem_bytes(int G, int c) {
+__host__ __device__ inline size_t chain_selinv_smem_bytes(int G, int c) {
   const size_t nT = static_cast<size_t>(c - 1) * FD;
   return (2 * nT * nT + nT * (2 * FD + static_cast<size_t>(G))) * sizeof(double);
 }
 
-// entry (k, q) of the boundary covariance Σ_yy of chunk j, y = (node j, node j+1 of level l+1, globals)
+// entry (k, q) of the boundary covariance Σ_yy of chunk j, y = (node j, node j+1 of level l+1, globals).  Level l+1's
+// blocks and Σ_gg are read through L2: in a cluster's walk other CTAs wrote them in the same launch.
 template <int FD>
 __device__ __forceinline__ double selinv_boundary(const SelinvArgs& a, int j, bool hasR, int k, int q) {
   const int G = a.G;
   const int bk = k < FD ? 0 : k < 2 * FD ? 1 : 2, bq = q < FD ? 0 : q < 2 * FD ? 1 : 2;
   if (!hasR && (bk == 1 || bq == 1)) return 0.0;
-  if (bk == 2 && bq == 2) return a.Sgg[static_cast<int64_t>(k - 2 * FD) * a.ldg + (q - 2 * FD)];
-  if (bq == 2) return a.up.kg[static_cast<int64_t>(j + bk) * FD * G + (k - bk * FD) * G + (q - 2 * FD)];
-  if (bk == 2) return a.up.kg[static_cast<int64_t>(j + bq) * FD * G + (q - bq * FD) * G + (k - 2 * FD)];
-  if (bk == bq) return a.up.kk[static_cast<int64_t>(j + bk) * FD * FD + (k - bk * FD) * FD + (q - bq * FD)];
-  if (bk == 0) return a.up.kn[static_cast<int64_t>(j) * FD * FD + k * FD + (q - FD)];
-  return a.up.kn[static_cast<int64_t>(j) * FD * FD + q * FD + (k - FD)];
+  if (bk == 2 && bq == 2) return __ldcg(a.Sgg + static_cast<int64_t>(k - 2 * FD) * a.ldg + (q - 2 * FD));
+  if (bq == 2) return __ldcg(a.up.kg + static_cast<int64_t>(j + bk) * FD * G + (k - bk * FD) * G + (q - 2 * FD));
+  if (bk == 2) return __ldcg(a.up.kg + static_cast<int64_t>(j + bq) * FD * G + (q - bq * FD) * G + (k - 2 * FD));
+  if (bk == bq) return __ldcg(a.up.kk + static_cast<int64_t>(j + bk) * FD * FD + (k - bk * FD) * FD + (q - bq * FD));
+  if (bk == 0) return __ldcg(a.up.kn + static_cast<int64_t>(j) * FD * FD + k * FD + (q - FD));
+  return __ldcg(a.up.kn + static_cast<int64_t>(j) * FD * FD + q * FD + (k - FD));
 }
 
-template <int FD>
-__global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs a) {
-  extern __shared__ double sm[];
-  const int G = a.G, c = a.c, tid = threadIdx.x, ny = 2 * FD + G, w = ny + 1;
+// Chunk j of level l (separator s = j c, interior nodes s+1 .. s+m) by NT threads: this thread is `tid` of them, sync()
+// is their barrier, sm their workspace (chain_selinv_smem_bytes), *bad their pivot flag.  node_A(p, e) and node_U(p, e)
+// give entry e of H[p, p] and of H[p-1, p] at level l as the elimination saw them (A + addA and U, or at level 0 of a
+// cluster, which never stores them, the scaled and damped normal equations).  The caller separates two chunks that
+// share a workspace with sync().
+template <int FD, int NT, class Sync, class NodeA, class NodeU>
+__device__ __forceinline__ void chain_selinv_chunk(const SelinvArgs& a, int j, double* sm, int tid, int* bad, Sync sync, NodeA node_A,
+                                                   NodeU node_U) {
+  const int G = a.G, c = a.c, ny = 2 * FD + G, w = ny + 1;
   const ChainLevel& L = a.cur;
-  const int j = blockIdx.x, s = j * c, n = L.n;
+  const int s = j * c, n = L.n;
   const int m = min(c - 1, n - 1 - s);  // interior nodes s+1 .. s+m
   const bool hasR = s + c < n;          // right separator: node s+m+1 here, node j+1 at level l+1
   const int nT = m * FD;
   double* T = sm;           // [nT][nT] the interior's block-tridiagonal matrix, then its Cholesky factor
   double* K = T + nT * nT;  // [nT][nT] its inverse
   double* P = K + nT * nT;  // [m][FD][ny] M_p Σ_yy
-  __shared__ int bad;
-  if (tid == 0) bad = 0;
-  for (int e = tid; e < nT * nT; e += kChainThreads) {
+  if (tid == 0) *bad = 0;
+  for (int e = tid; e < nT * nT; e += NT) {
     const int r = e / nT, q = e - r * nT, br = r / FD, bq = q / FD, rr = r - br * FD, qq = q - bq * FD;
     const int64_t p = s + 1 + min(br, bq);
     double v = 0.0;
-    if (br == bq) v = L.A[p * FD * FD + rr * FD + qq] + (L.addA ? L.addA[p * FD * FD + rr * FD + qq] : 0.0);
-    else if (bq == br + 1) v = L.U[(p + 1) * FD * FD + rr * FD + qq];  // H[p, p+1]
-    else if (br == bq + 1) v = L.U[(p + 1) * FD * FD + qq * FD + rr];  // H[p+1, p] = H[p, p+1]^T
+    if (br == bq) v = node_A(p, rr * FD + qq);
+    else if (bq == br + 1) v = node_U(p + 1, rr * FD + qq);  // H[p, p+1]
+    else if (br == bq + 1) v = node_U(p + 1, qq * FD + rr);  // H[p+1, p] = H[p, p+1]^T
     T[e] = v;
   }
-  for (int e = tid; e < nT * ny; e += kChainThreads) {
+  for (int e = tid; e < nT * ny; e += NT) {
     const int rp = e / ny, q = e - rp * ny;  // rp = i FD + r
     const double* z = L.Z + (static_cast<int64_t>(s + 1) * FD + rp) * w;
     double sum = 0.0;
     for (int k = 0; k < ny; ++k) sum += z[k] * selinv_boundary<FD>(a, j, hasR, k, q);
     P[e] = sum;
   }
-  __syncthreads();
+  sync();
   for (int jj = 0; jj < nT; ++jj) {  // T = L L^T, in place (lower triangle)
     if (tid == 0) {
       double d = T[jj * nT + jj];
-      if (!(d > 0.0)) { bad = 1; d = 1.0; }
+      if (!(d > 0.0)) { *bad = 1; d = 1.0; }
       T[jj * nT + jj] = sqrt(d);
     }
-    __syncthreads();
+    sync();
     const double dj = T[jj * nT + jj];
-    for (int i = jj + 1 + tid; i < nT; i += kChainThreads) T[i * nT + jj] /= dj;
-    __syncthreads();
+    for (int i = jj + 1 + tid; i < nT; i += NT) T[i * nT + jj] /= dj;
+    sync();
     const int rem = nT - jj - 1;
-    for (int e = tid; e < rem * rem; e += kChainThreads) {
+    for (int e = tid; e < rem * rem; e += NT) {
       const int i = jj + 1 + e / rem, k = jj + 1 + e % rem;
       if (k <= i) T[i * nT + k] -= T[i * nT + jj] * T[k * nT + jj];
     }
-    __syncthreads();
+    sync();
   }
-  for (int col = tid; col < nT; col += kChainThreads) {  // K = T^-1, one column per thread
+  for (int col = tid; col < nT; col += NT) {  // K = T^-1, one column per thread
     for (int i = col; i < nT; ++i) {
       double t = i == col ? 1.0 : 0.0;
       for (int k = col; k < i; ++k) t -= T[i * nT + k] * K[k * nT + col];
@@ -197,10 +209,10 @@ __global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs 
       K[i * nT + col] = t / T[i * nT + i];
     }
   }
-  __syncthreads();
-  if (bad && tid == 0) a.scalars[kScNotPD] = 1.0;
+  sync();
+  if (*bad && tid == 0) a.scalars[kScNotPD] = 1.0;
   // the interior nodes: Σ_pp, Σ_p,p+1 (p+1 interior, or the right separator: -M_p Σ_y,right), Σ_pg = -(M_p Σ_yy)[:, g]
-  for (int e = tid; e < m * FD * FD; e += kChainThreads) {
+  for (int e = tid; e < m * FD * FD; e += NT) {
     const int i = e / (FD * FD), r = (e / FD) % FD, q = e % FD;
     const int64_t p = s + 1 + i;
     const double* Pr = P + (i * FD + r) * ny;
@@ -218,31 +230,47 @@ __global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs 
     a.sig.kk[p * FD * FD + r * FD + q] = kk;
     a.sig.kn[p * FD * FD + r * FD + q] = kn;
   }
-  for (int e = tid; e < m * FD * G; e += kChainThreads) {
+  for (int e = tid; e < m * FD * G; e += NT) {
     const int i = e / (FD * G), r = (e / G) % FD, q = e % G;
     a.sig.kg[(static_cast<int64_t>(s + 1 + i) * FD + r) * G + q] = -P[(i * FD + r) * ny + 2 * FD + q];
   }
   // the chunk's left separator: node j of level l+1; its next node is the first interior one (or the right separator)
-  for (int e = tid; e < FD * FD; e += kChainThreads) {
+  for (int e = tid; e < FD * FD; e += NT) {
     const int r = e / FD, q = e % FD;
-    a.sig.kk[static_cast<int64_t>(s) * FD * FD + e] = a.up.kk[static_cast<int64_t>(j) * FD * FD + e];
+    a.sig.kk[static_cast<int64_t>(s) * FD * FD + e] = __ldcg(a.up.kk + static_cast<int64_t>(j) * FD * FD + e);
     a.sig.kn[static_cast<int64_t>(s) * FD * FD + e] =
-        m > 0 ? -P[q * ny + r] : (hasR ? a.up.kn[static_cast<int64_t>(j) * FD * FD + e] : 0.0);
+        m > 0 ? -P[q * ny + r] : (hasR ? __ldcg(a.up.kn + static_cast<int64_t>(j) * FD * FD + e) : 0.0);
   }
-  for (int e = tid; e < FD * G; e += kChainThreads)
-    a.sig.kg[static_cast<int64_t>(s) * FD * G + e] = a.up.kg[static_cast<int64_t>(j) * FD * G + e];
+  for (int e = tid; e < FD * G; e += NT)
+    a.sig.kg[static_cast<int64_t>(s) * FD * G + e] = __ldcg(a.up.kg + static_cast<int64_t>(j) * FD * G + e);
+}
+
+// One CTA per chunk of level l (vcgpu_get_frame_covariance: the multi-launch chain kernels stored every level's blocks)
+template <int FD>
+__global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs a) {
+  extern __shared__ double sm[];
+  __shared__ int bad;
+  const ChainLevel& L = a.cur;
+  chain_selinv_chunk<FD, kChainThreads>(
+      a, blockIdx.x, sm, threadIdx.x, &bad, [] { __syncthreads(); },
+      [&](int64_t p, int e) { return L.A[p * FD * FD + e] + (L.addA ? L.addA[p * FD * FD + e] : 0.0); },
+      [&](int64_t p, int e) { return L.U[p * FD * FD + e]; });
 }
 
 // Level 0's Σ_ff unscaled, s_f Σ_ff s_f, and exactly symmetric: both halves are written from the lower triangle.  Rows
 // and columns from `live` on (the velocities of a rotation-only run, which no residual reads) are 0.
 template <int FD>
+__device__ __forceinline__ double frame_cov_out_entry(int64_t e, int live, const double* kk, const double* scale) {
+  const int64_t f = e / (FD * FD);
+  const int r = static_cast<int>((e / FD) % FD), q = static_cast<int>(e % FD), hi = max(r, q), lo = min(r, q);
+  return hi < live ? kk[f * FD * FD + hi * FD + lo] * (scale[f * FD + hi] * scale[f * FD + lo]) : 0.0;
+}
+template <int FD>
 __global__ void __launch_bounds__(256) frame_cov_out_kernel(int n_frames, int live, const double* kk, const double* scale,
                                                             double* out) {
   const int64_t e = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (e >= static_cast<int64_t>(n_frames) * FD * FD) return;
-  const int64_t f = e / (FD * FD);
-  const int r = static_cast<int>((e / FD) % FD), q = static_cast<int>(e % FD), hi = max(r, q), lo = min(r, q);
-  out[e] = hi < live ? kk[f * FD * FD + hi * FD + lo] * (scale[f * FD + hi] * scale[f * FD + lo]) : 0.0;
+  out[e] = frame_cov_out_entry<FD>(e, live, kk, scale);
 }
 
 }  // namespace vc

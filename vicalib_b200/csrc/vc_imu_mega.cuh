@@ -24,6 +24,7 @@
 #include <type_traits>
 
 #include "vc_chain.cuh"
+#include "vc_frame_cov.cuh"
 #include "vc_kernels.cuh"
 #include "vc_mega.cuh"
 #include "vc_xchg.cuh"
@@ -846,7 +847,9 @@ __device__ __forceinline__ void dense_assemble(const ChainSolveArgs& a, const Bl
 // kCov (chain_cov_batch_kernel, with a.D2x set): the elimination, the Schur reduction and the dense factorisation only;
 // in place of the dense phase's right-hand side, the G unit right-hand sides of the globals give the globals' block of
 // the [globals | top nodes] inverse, unscaled into cov (G x G; mask: 0 on constant globals).  No step, no state update.
-template <class Scope, bool kCov = false>
+// kFrame (with kCov; chain_frame_cov_batch_kernel): no right-hand side at all; the factorisation stays in CTA 0's shared
+// memory for the caller (the L D L^T factor S [RT][LD], then 1 / d at S + RT LD).
+template <class Scope, bool kCov = false, bool kFrame = false>
 __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope, const double* mask = nullptr, double* cov = nullptr) {
   extern __shared__ double smem[];
   constexpr int FD = 9;
@@ -1172,6 +1175,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
         if (tid == 0) a.scalars[kScNotPD] = 1.0;
         return;
       }
+      if constexpr (kFrame) return;
       for (int j = warp; j < G; j += kCsThreads / 32) {
         double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
         if (mask[j] != 0.0) warp_inverse_column<kCovQ, true>(S, LD, wd, N, j, lane, x);
@@ -1399,6 +1403,98 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_cov_batch_kernel(const Ch
   ClusterScope scope;
   const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
   chain_solve<ClusterScope, true>(a.s, scope, a.mask, a.cov);
+}
+
+// ------------------------------------------------------------------ frame covariance (vcgpu_get_frame_covariance_batch)
+// The walk takes two chunks per CTA at a time, one per group of kCsGroup threads, where their workspaces fit in what the
+// solve asks for; else one per CTA, and the request grows to one chunk's workspace.
+__host__ __device__ inline int chain_walk_chunks(int G) {
+  return 2 * chain_selinv_smem_bytes<9>(G, kCsChunk) <= chain_solve_smem_doubles(G) * sizeof(double) ? 2 : 1;
+}
+__host__ __device__ inline size_t chain_frame_cov_smem_bytes(int G) {
+  const size_t solve = chain_solve_smem_doubles(G) * sizeof(double), walk = chain_walk_chunks(G) * chain_selinv_smem_bytes<9>(G, kCsChunk);
+  return solve > walk ? solve : walk;
+}
+// a rig as chain_frame_cov_batch_kernel takes it: the solve's arguments (D2x: the frame damping of
+// vcgpu_get_frame_covariance; scalars[kScNotPD] zeroed), every level's Σ blocks, the inverse of [globals | top nodes]
+// [N*N] and the blocks written [nf][81], rows and columns from `live` on 0
+struct ChainFrameCovArgs {
+  ChainSolveArgs s;
+  SigmaLevel sig[kMaxChainLevels];
+  double* inv;
+  double* out;
+  int live;
+};
+// A batch of inertial rigs, one thread-block cluster each: cluster k writes the frame covariance of args[k].  The
+// elimination and the dense factorisation of chain_solve; CTA 0's warps solve the N unit right-hand sides (the whole
+// inverse of [globals | top nodes], as dense_solve_kernel's mode 3 gives it) and leave the top nodes' blocks; then the
+// levels top-down, a cluster barrier between two, their chunks spread over the CTAs (chain_selinv_chunk); then level 0
+// unscaled.
+__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainFrameCovArgs* __restrict__ args) {
+  extern __shared__ double smem[];
+  constexpr int FD = 9;
+  ClusterScope scope;
+  const ChainFrameCovArgs& a = args[blockIdx.x / scope.nb()];
+  chain_solve<ClusterScope, true, true>(a.s, scope);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, grp = tid / kCsGroup, gtid = tid - grp * kCsGroup;
+  const int bid = scope.bid(), nb = scope.nb();
+  const int G = a.s.dp.G, nl = a.s.n_levels, nf = a.s.dp.n_frames;
+  const ChainLevel top = a.s.lev[nl - 1];
+  const int nt = top.n, N = G + nt * FD;
+  if (bid == 0) {
+    const int LD = dense_ld(N), RT = dense_rows(N);
+    for (int j = warp; j < N; j += kCsThreads / 32) {
+      double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
+      warp_inverse_column<kCovQ, true>(smem, LD, smem + RT * LD, N, j, lane, x);
+#pragma unroll
+      for (int q = 0; q < kCovQ; ++q)
+        if (32 * q + lane < N) a.inv[static_cast<int64_t>(32 * q + lane) * N + j] = x[q];
+    }
+    __syncthreads();
+    const SigmaLevel& t = a.sig[nl - 1];
+    for (int e = tid; e < nt * FD * FD; e += kCsThreads) {
+      const int k = e / (FD * FD), r = (e / FD) % FD, q = e % FD, o = G + k * FD;
+      t.kk[e] = a.inv[static_cast<int64_t>(o + r) * N + o + q];
+      t.kn[e] = k + 1 < nt ? a.inv[static_cast<int64_t>(o + r) * N + o + FD + q] : 0.0;
+    }
+    for (int e = tid; e < nt * FD * G; e += kCsThreads) {
+      const int k = e / (FD * G), r = (e / G) % FD, q = e % G;
+      t.kg[e] = a.inv[static_cast<int64_t>(G + k * FD + r) * N + q];
+    }
+  }
+  scope.sync();
+  __shared__ int bad[kCsGroups];
+  const bool two = chain_walk_chunks(G) == 2;
+  const size_t ws = chain_selinv_smem_bytes<FD>(G, kCsChunk) / sizeof(double);
+  for (int l = nl - 2; l >= 0; --l) {
+    SelinvArgs sa;
+    sa.G = G; sa.c = kCsChunk; sa.cur = a.s.lev[l]; sa.sig = a.sig[l]; sa.up = a.sig[l + 1];
+    sa.Sgg = a.inv; sa.ldg = N; sa.scalars = a.s.scalars;
+    NodeSrc src;
+    src.L = l > 0 ? &a.s.lev[l] : nullptr;
+    src.b = a.s.b[a.s.ctl->cur]; src.scale = a.s.scale; src.D2x = a.s.D2x; src.rinv = 0.0; src.G = G; src.nf = nf;
+    src.sepdiag = nullptr; src.rank = 0; src.ghost = 0;
+    auto node_A = [&](int64_t p, int e) { return src_A<FD>(src, p, e); };
+    auto node_U = [&](int64_t p, int e) { return src_U<FD>(src, p, e); };
+    const int n_chunks = a.s.lev[l + 1].n;
+    if (two) {
+      auto sync = [grp] { group_sync(grp); };
+      for (int j = bid * kCsGroups + grp; j < n_chunks; j += nb * kCsGroups) {
+        chain_selinv_chunk<FD, kCsGroup>(sa, j, smem + grp * ws, gtid, &bad[grp], sync, node_A, node_U);
+        sync();
+      }
+    } else {
+      auto sync = [] { __syncthreads(); };
+      for (int j = bid; j < n_chunks; j += nb) {
+        chain_selinv_chunk<FD, kCsThreads>(sa, j, smem, tid, &bad[0], sync, node_A, node_U);
+        sync();
+      }
+    }
+    scope.sync();
+  }
+  const double* kk = a.sig[0].kk;
+  for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < static_cast<int64_t>(nf) * FD * FD; e += static_cast<int64_t>(nb) * kCsThreads)
+    a.out[e] = frame_cov_out_entry<FD>(e, a.live, kk, a.s.scale);
 }
 
 }  // namespace vc

@@ -41,6 +41,7 @@
 #pragma once
 #include <cooperative_groups.h>
 
+#include "vc_frame_cov.cuh"
 #include "vc_dogleg.cuh"
 #include "vc_fused.cuh"
 #include "vc_kernels.cuh"
@@ -928,22 +929,27 @@ struct CovArgs {
   const double* mask;   // [G] 0: constant global
   double* part;         // [cluster CTAs][G*G + G] CTA partials of the Schur sum
   double* tot;          // [G*G + G] their total
-  double* cov;          // [G*G] the covariance, row-major
+  double* cov;          // [G*G] the covariance, row-major (frame mode: Σ_gg, the whole scaled inverse)
   double* notpd;        // set to 1 where a pivot fails (zeroed before the launch)
+  // frame mode (cov_frame_mega_batch_kernel): D2x also 1 on the frames no active observation sees (frame_used 0), whose
+  // blocks of fcov [nf][36] are 0
+  const uint8_t* frame_used;
+  double* fcov;
 };
 // dynamic shared memory of cov_mega_batch_kernel: per warp its frame's scaled [E | g] and X, the reduced system, pivots
 __host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
   return static_cast<size_t>(n_warps) * 12 * (G + 1) + static_cast<size_t>(G) * G + 2 * static_cast<size_t>(G);
 }
 
-// A batch of vision rigs, one thread-block cluster each: cluster k writes the covariance of args[k].  Frames are owned as
-// in mega_solve (frame f -> CTA f mod cluster size, warp (f / size) mod warps); every CTA forms and factors the reduced
-// system (the same bits everywhere), then the cluster's warps share the right-hand sides.
-__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(const CovArgs* __restrict__ args) {
+// One vision rig by one thread-block cluster.  Frames are owned as in mega_solve (frame f -> CTA f mod cluster size, warp
+// (f / size) mod warps); every CTA forms and factors the reduced system (the same bits everywhere), then the cluster's
+// warps share the right-hand sides.  kFrames = false: the covariance of the globals.  kFrames = true: all G unit
+// right-hand sides give Σ_gg; after a cluster barrier one warp per frame refactors B_f, forms X_f = B_f^-1 E_f again
+// and writes B_f^-1 + X_f Σ_gg X_f^T (frame_cov_block).
+template <bool kFrames>
+__device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
   extern __shared__ double smem[];
   constexpr int FD = 6;
-  ClusterScope scope;
-  const CovArgs& a = args[blockIdx.x / scope.nb()];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nthreads = blockDim.x, nwarps = nthreads >> 5;
   const int bid = scope.bid(), nb = scope.nb();
   const int G = a.G, M = G + 1, NS = G * G + G, nf = a.n_frames;
@@ -957,72 +963,74 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(cons
   for (int e = tid; e < NS; e += nthreads) S[e] = 0.0;
   if (tid == 0) bad = 0;
   bool frame_bad = false;
+  // this warp's frame f: its damped, scaled block factored in registers, then its scaled [E | 0] and X into the warp's
+  // slots of wmem
+  auto frame_x = [&](int f) {
+    double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
+    double* Xw = Esw + FD * M;
+    const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+    const double* Bf = a.b.B + static_cast<int64_t>(f) * FD * FD;
+    const double* Ef = a.b.E + static_cast<int64_t>(f) * FD * G;
+    double s[FD], L[FD][FD], iL[FD];
+#pragma unroll
+    for (int i = 0; i < FD; ++i) s[i] = sf[i];
+#pragma unroll
+    for (int i = 0; i < FD; ++i)
+#pragma unroll
+      for (int j = 0; j <= i; ++j) {
+        const double bij = Bf[i * FD + j];
+        double v = bij * s[i] * s[j];
+        if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], 0.0, a.D2x, nullptr, 0, false);
+        L[i][j] = v;
+      }
+#pragma unroll
+    for (int j = 0; j < FD; ++j) {
+      double d = L[j][j];
+#pragma unroll
+      for (int q = 0; q < j; ++q) d -= L[j][q] * L[j][q];
+      if (!(d > 0.0)) { frame_bad = true; d = 1.0; }
+      const double inv = rsqrt(d);
+      L[j][j] = d * inv;
+      iL[j] = inv;
+#pragma unroll
+      for (int i = j + 1; i < FD; ++i) {
+        double t = L[i][j];
+#pragma unroll
+        for (int q = 0; q < j; ++q) t -= L[i][q] * L[j][q];
+        L[i][j] = t * inv;
+      }
+    }
+    for (int c = lane; c < M; c += 32) {
+      double x[FD];
+      const double scc = c < G ? scg[c] : 1.0;
+#pragma unroll
+      for (int i = 0; i < FD; ++i) {
+        const double r = (c < G ? Ef[i * G + c] : 0.0) * s[i] * scc;  // the right-hand side plays no part
+        Esw[i * M + c] = r;
+        x[i] = r;
+      }
+#pragma unroll
+      for (int i = 0; i < FD; ++i) {
+        double t = x[i];
+#pragma unroll
+        for (int q = 0; q < i; ++q) t -= L[i][q] * x[q];
+        x[i] = t * iL[i];
+      }
+#pragma unroll
+      for (int i = FD - 1; i >= 0; --i) {
+        double t = x[i];
+#pragma unroll
+        for (int q = i + 1; q < FD; ++q) t -= L[q][i] * x[q];
+        x[i] = t * iL[i];
+      }
+#pragma unroll
+      for (int i = 0; i < FD; ++i) Xw[i * M + c] = x[i];
+    }
+  };
   for (int base = 0; base < nk; base += nwarps) {
     const int k = base + warp;
     __syncthreads();
-    if (k < nk) {
-      const int f = bid + k * nb;
-      double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
-      double* Xw = Esw + FD * M;
-      const double* sf = a.scale + static_cast<int64_t>(f) * FD;
-      const double* Bf = a.b.B + static_cast<int64_t>(f) * FD * FD;
-      const double* Ef = a.b.E + static_cast<int64_t>(f) * FD * G;
-      double s[FD], L[FD][FD], iL[FD];
-#pragma unroll
-      for (int i = 0; i < FD; ++i) s[i] = sf[i];
-#pragma unroll
-      for (int i = 0; i < FD; ++i)
-#pragma unroll
-        for (int j = 0; j <= i; ++j) {
-          const double bij = Bf[i * FD + j];
-          double v = bij * s[i] * s[j];
-          if (i == j) v = frame_damp<FD>(v, f, i, bij, s[i], 0.0, a.D2x, nullptr, 0, false);
-          L[i][j] = v;
-        }
-#pragma unroll
-      for (int j = 0; j < FD; ++j) {
-        double d = L[j][j];
-#pragma unroll
-        for (int q = 0; q < j; ++q) d -= L[j][q] * L[j][q];
-        if (!(d > 0.0)) { frame_bad = true; d = 1.0; }
-        const double inv = rsqrt(d);
-        L[j][j] = d * inv;
-        iL[j] = inv;
-#pragma unroll
-        for (int i = j + 1; i < FD; ++i) {
-          double t = L[i][j];
-#pragma unroll
-          for (int q = 0; q < j; ++q) t -= L[i][q] * L[j][q];
-          L[i][j] = t * inv;
-        }
-      }
-      for (int c = lane; c < M; c += 32) {
-        double x[FD];
-        const double scc = c < G ? scg[c] : 1.0;
-#pragma unroll
-        for (int i = 0; i < FD; ++i) {
-          const double r = (c < G ? Ef[i * G + c] : 0.0) * s[i] * scc;  // the right-hand side plays no part
-          Esw[i * M + c] = r;
-          x[i] = r;
-        }
-#pragma unroll
-        for (int i = 0; i < FD; ++i) {
-          double t = x[i];
-#pragma unroll
-          for (int q = 0; q < i; ++q) t -= L[i][q] * x[q];
-          x[i] = t * iL[i];
-        }
-#pragma unroll
-        for (int i = FD - 1; i >= 0; --i) {
-          double t = x[i];
-#pragma unroll
-          for (int q = i + 1; q < FD; ++q) t -= L[q][i] * x[q];
-          x[i] = t * iL[i];
-        }
-#pragma unroll
-        for (int i = 0; i < FD; ++i) Xw[i * M + c] = x[i];
-      }
-    }
+    if (k < nk) frame_x(bid + k * nb);
     __syncthreads();
     schur_accumulate<FD>(S, wmem, 2 * FD * M, min(nwarps, nk - base), G, tid, nthreads);
   }
@@ -1044,11 +1052,46 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(cons
     if (bid == 0 && tid == 0) *a.notpd = 1.0;
     return;
   }
-  for (int j = bid * nwarps + warp; j < G; j += nb * nwarps) {
-    double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
-    if (a.mask[j] != 0.0) warp_inverse_column<kCovQ, false>(S, G, invd, G, j, lane, x);
-    cov_store_column<kCovQ>(x, scg, a.mask, G, j, lane, a.cov);
+  if constexpr (!kFrames) {
+    for (int j = bid * nwarps + warp; j < G; j += nb * nwarps) {
+      double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
+      if (a.mask[j] != 0.0) warp_inverse_column<kCovQ, false>(S, G, invd, G, j, lane, x);
+      cov_store_column<kCovQ>(x, scg, a.mask, G, j, lane, a.cov);
+    }
+  } else {
+    for (int j = bid * nwarps + warp; j < G; j += nb * nwarps) {
+      double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
+      warp_inverse_column<kCovQ, false>(S, G, invd, G, j, lane, x);
+#pragma unroll
+      for (int q = 0; q < kCovQ; ++q)
+        if (32 * q + lane < G) a.cov[static_cast<int64_t>(32 * q + lane) * G + j] = x[q];
+    }
+    scope.sync();
+    for (int k = warp; k < nk; k += nwarps) {
+      const int f = bid + k * nb;
+      double* out = a.fcov + static_cast<int64_t>(f) * FD * FD;
+      if (!a.frame_used[f]) {
+        for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
+        continue;
+      }
+      frame_x(f);
+      __syncwarp();
+      const double* Xw = wmem + static_cast<size_t>(warp) * 2 * FD * M + FD * M;
+      frame_cov_block<FD>(a.b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, Xw, M, a.cov, G, lane, out);
+      __syncwarp();
+    }
   }
+}
+
+// A batch of vision rigs, one thread-block cluster each: cluster k writes the covariance of args[k].
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(const CovArgs* __restrict__ args) {
+  ClusterScope scope;
+  cov_mega<false>(args[blockIdx.x / scope.nb()], scope);
+}
+// ... the frame covariance of args[k] (vcgpu_get_frame_covariance_batch)
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_mega_batch_kernel(const CovArgs* __restrict__ args) {
+  ClusterScope scope;
+  cov_mega<true>(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

@@ -1008,22 +1008,20 @@ extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
   return rc;
 }
 
-// The frames' blocks of vcgpu_get_frame_covariance (vc_frame_cov.cuh) into out [nf][fd*fd] on the device.
+// The frames' blocks of vcgpu_get_frame_covariance (vc_frame_cov.cuh) into w.out [nf][fd*fd] on the device.
 // Vision: the solve's frame elimination and Schur sum, the inverse of the reduced system, then one warp per frame.
-static int frame_cov_vision(vcgpu_handle* h, const double* D2x, double** out) {
+static int frame_cov_vision(vcgpu_handle* h, const double* D2x, const FrameCovSpace& w) {
   const DevProblem& dp = h->dp;
   const int G = dp.G;
-  VC_TRY(dev_alloc(h, &h->d_fcov, static_cast<size_t>(G) * G + static_cast<size_t>(dp.n_frames) * 36));
-  *out = h->d_fcov + static_cast<size_t>(G) * G;
   VC_TRY(vision_frame_solve(h, D2x));
   DenseArgs da{};
   da.dp = dp; da.bs[0] = h->blk[0]; da.bs[1] = h->blk[1]; da.ctl = h->d_ctl; da.scale = h->d_scale; da.D2x = D2x;
-  da.Ssum = h->d_Ssum; da.delta = h->d_delta; da.scalars = h->d_scalars; da.add_globals = 1; da.mode = 3; da.buf = h->d_fcov;
+  da.Ssum = h->d_Ssum; da.delta = h->d_delta; da.scalars = h->d_scalars; da.add_globals = 1; da.mode = 3; da.buf = w.inv;
   VC_TRY(kernel_smem_optin(h));
   dense_solve_kernel<6><<<1, 256, vc::chain_dense_smem_bytes(G), h->stream>>>(da);
   vc::FrameCovArgs fa;
   fa.dp = dp; fa.b[0] = h->blk[0]; fa.b[1] = h->blk[1]; fa.ctl = h->d_ctl; fa.scale = h->d_scale; fa.D2x = D2x; fa.X = h->d_X;
-  fa.Sgg = h->d_fcov; fa.frame_used = h->d_frame_used; fa.out = *out;
+  fa.Sgg = w.inv; fa.frame_used = h->d_frame_used; fa.out = w.out;
   vc::frame_cov_vision_kernel<6><<<(dp.n_frames + vc::kFrameCovWarps - 1) / vc::kFrameCovWarps, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
   h->launches += 2;
   CUDA_TRY(h, cudaGetLastError());
@@ -1031,40 +1029,26 @@ static int frame_cov_vision(vcgpu_handle* h, const double* D2x, double** out) {
 }
 // Inertial: the chain elimination, the inverse of [globals | top nodes], then the levels top-down (chain_selinv_kernel);
 // rows and columns from `live` on are 0.
-// The workspace is the dense inverse [N*N], the frames' blocks and, per level of n nodes, n (2 * 81 + 9 G) doubles.
-static int frame_cov_inertial(vcgpu_handle* h, const double* D2x, int live, double** out) {
+static int frame_cov_inertial(vcgpu_handle* h, const double* D2x, int live, const FrameCovSpace& w) {
   constexpr int FD = 9;
   vc::ImuDev* d = imu_dev(h);
   const DevProblem& dp = h->dp;
-  const int G = dp.G, nl = static_cast<int>(d->levels.size()), N = G + d->levels.back().n * FD;
-  size_t total = static_cast<size_t>(N) * N + static_cast<size_t>(dp.n_frames) * FD * FD;
-  for (const vc::ChainLevel& L : d->levels) total += static_cast<size_t>(L.n) * (2 * FD * FD + FD * G);
-  VC_TRY(dev_alloc(h, &h->d_fcov, total));
-  double* p = h->d_fcov + static_cast<size_t>(N) * N;
-  *out = p;
-  p += static_cast<size_t>(dp.n_frames) * FD * FD;
-  std::vector<vc::SigmaLevel> sig(nl);
-  for (int l = 0; l < nl; ++l) {
-    const size_t n = d->levels[l].n;
-    sig[l].kk = p; p += n * FD * FD;
-    sig[l].kn = p; p += n * FD * FD;
-    sig[l].kg = p; p += n * FD * G;
-  }
+  const int G = dp.G, nl = static_cast<int>(d->levels.size());
   VC_TRY(imu_chain_eliminate(h, D2x));
-  VC_TRY(imu_chain_dense(h, D2x, h->d_fcov, &sig.back()));
+  VC_TRY(imu_chain_dense(h, D2x, w.inv, &w.sig.back()));
   const size_t sm = vc::chain_selinv_smem_bytes<FD>(G, kChainC);
   if (nl > 1 && sm > h->selinv_smem_max)
     return fail(h, VCGPU_ERR_INVALID, "frame covariance: G = " + std::to_string(G) + " needs " + std::to_string(sm) +
                                           " B of shared memory per block, the device allows " + std::to_string(h->selinv_smem_max));
   for (int l = nl - 2; l >= 0; --l) {
     vc::SelinvArgs sa;
-    sa.G = G; sa.c = kChainC; sa.cur = d->levels[l]; sa.sig = sig[l]; sa.up = sig[l + 1];
-    sa.Sgg = h->d_fcov; sa.ldg = N; sa.scalars = h->d_scalars;
+    sa.G = G; sa.c = kChainC; sa.cur = d->levels[l]; sa.sig = w.sig[l]; sa.up = w.sig[l + 1];
+    sa.Sgg = w.inv; sa.ldg = w.N; sa.scalars = h->d_scalars;
     vc::chain_selinv_kernel<FD><<<d->levels[l + 1].n, vc::kChainThreads, sm, h->stream>>>(sa);
     ++h->launches;
   }
   const int64_t ne = static_cast<int64_t>(dp.n_frames) * FD * FD;
-  vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, sig[0].kk, h->d_scale, *out);
+  vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, w.sig[0].kk, h->d_scale, w.out);
   ++h->launches;
   CUDA_TRY(h, cudaGetLastError());
   return VCGPU_OK;
@@ -1081,22 +1065,24 @@ extern "C" int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov) {
   VC_TRY(cov_prelude(h, &mask, &D2));
   const DevProblem& dp = h->dp;
   const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + dp.G;
-  // A frame no active observation sees has an empty block, and so do the velocities of a rotation-only run (no residual
-  // reads them): a unit damping on those tangents leaves them out of the other blocks, and their rows come back 0.
-  const int live = dp.inertial && h->flags.rotation_only ? 6 : dp.fd;
   std::vector<double> D2f(D2);
-  for (int64_t i = 0; i < nfp; ++i)
-    if (!h->h_frame_used[i / dp.fd] || i % dp.fd >= live) D2f[i] = 1.0;
+  const int live = frame_cov_damping(h, &D2f);
   CUDA_TRY(h, cudaMemcpyAsync(h->d_scale + np, D2f.data(), np * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
-  double* d_out = nullptr;
-  const int rc = dp.inertial ? frame_cov_inertial(h, h->d_scale + np, live, &d_out) : frame_cov_vision(h, h->d_scale + np, &d_out);
+  FrameCovSpace w;
+  int rc = frame_cov_space(h, &w);
+  if (rc == VCGPU_OK) rc = dp.inertial ? frame_cov_inertial(h, h->d_scale + np, live, w) : frame_cov_vision(h, h->d_scale + np, w);
   h->blocks_valid = false;  // as vcgpu_get_covariance: the Jacobi scale is the next solve's to set
   if (rc != VCGPU_OK) return rc;
   VC_TRY(read_scalars(h));
   if (h->h_scalars[kScNotPD] > 0) return fail(h, VCGPU_ERR_NUMERIC, "frame covariance: J^T J is singular at the current state");
-  CUDA_TRY(h, cudaMemcpy(cov, d_out, static_cast<size_t>(nfp) * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
+  CUDA_TRY(h, cudaMemcpy(cov, w.out, static_cast<size_t>(nfp) * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
   return VCGPU_OK;
+}
+extern "C" int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_frame_covariance_batch");
+  return run_frame_covariance_batch(handles, n, cov, status);
 }
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp
