@@ -195,6 +195,34 @@ int vcgpu_cost(vcgpu_handle* h, double* cost);
 /* RemoveOutliers (vicalibrator.h:859-916): drops observations with |r| > threshold * rmse[cam] */
 int vcgpu_remove_outliers(vcgpu_handle* h, const double* rmse, double threshold, int64_t* n_removed);
 int vcgpu_get_obs_active(vcgpu_handle* h, uint8_t* active /*n_obs, caller order*/);
+/* vcgpu_evaluate of every camera of n rigs in one call.  Per rig i: cam_cost[i][c] = 1/2 sum |r|^2 over camera c's
+ * active observations (loss-free, as vcgpu_evaluate(h, c)), and cam_blocks[i][c] their count (cam_blocks, or an entry of
+ * it, may be NULL); residuals_or_null[i] (the array or an entry may be NULL) gets 2 doubles per active observation in
+ * vcgpu_evaluate(h, -1, ...)'s layout, caller order.  The residuals are the bits vcgpu_evaluate returns and the counts
+ * are equal; a cost equals vcgpu_evaluate's to rounding (the device sums in another order).  One launch covers every rig:
+ * tiles of 256 consecutive observations of one camera, one CTA each, a tiling that is a function of the rig alone, so a
+ * rig's costs are the same bits whatever else is in the batch and in whatever order.  Per handle, on its own stream,
+ * the uploads of vcgpu_evaluate; then the launch and one download of the costs, and one of each rig's residuals.
+ * Nothing on the handle changes but what vcgpu_evaluate changes: state, IMU weights and what a later vcgpu_solve or batch
+ * solve computes stay as they were.
+ * Returns VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in
+ * vcgpu_last_error of every non-null handle, for: n <= 0, a null or repeated handle, a null cam_cost[i], handles on
+ * different devices, and frame shards.
+ * Device memory, held by handle 0: 8 bytes per tile and 96 bytes per rig of workspace, and 240 bytes per rig and
+ * 24 per tile of kernel arguments; with residuals, per handle 2 n_obs doubles (and n_obs int32 when the caller's order
+ * is not sorted by camera and frame). */
+int vcgpu_evaluate_batch(vcgpu_handle* const* handles, int n, double* const* cam_cost /* n pointers to n_cams */,
+                         int64_t* const* cam_blocks /* n pointers to n_cams, or NULL */,
+                         double* const* residuals_or_null /* n pointers to 2 * active observations, or NULL */);
+/* vcgpu_remove_outliers of n rigs in one call: rmse[i] holds rig i's n_cams values; an active observation of camera c
+ * leaves the problem where |r| > threshold * rmse[i][c], exactly the set vcgpu_remove_outliers removes (the device forms
+ * |r| without a fused multiply-add, as the host does).  n_removed: n counts, or NULL.  The residuals are computed as
+ * vcgpu_evaluate_batch computes them, in the same launch layout; the marks come back in one download.  A rig that loses
+ * nothing is left exactly as it was.  Refusals as vcgpu_evaluate_batch, with a null rmse[i] in place of a null
+ * cam_cost[i].  Device memory: vcgpu_evaluate_batch's, and one byte per active observation of every rig, held by
+ * handle 0. */
+int vcgpu_remove_outliers_batch(vcgpu_handle* const* handles, int n, const double* const* rmse /* n pointers */, double threshold,
+                                int64_t* n_removed /* n, or NULL */);
 /* UpdateImuWeights (vicalibrator.h:723-799) */
 int vcgpu_update_imu_weights(vcgpu_handle* h);
 int vcgpu_get_imu_weights(vcgpu_handle* h, double* w_sqrt /*(n_frames-1)*81*/);

@@ -25,7 +25,7 @@ EXPORTS = [
     "vcgpu_get_state", "vcgpu_num_residuals", "vcgpu_frame_dim", "vcgpu_num_globals", "vcgpu_eval_reproj",
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
-    "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch",
+    "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch", "vcgpu_evaluate_batch", "vcgpu_remove_outliers_batch",
     "vcgpu_pose_pnp_ransac",
 ]
 
@@ -417,3 +417,43 @@ def _covariances(entry, name, calibrators, out):
             e.covariances = [out[i] if status[i] == 0 else None for i in range(n)]
         raise e
     return list(out)
+
+
+def evaluate_batch(calibrators, residuals=False):
+    """vcgpu_evaluate_batch: Calibrator.evaluate(c) of every camera of every Calibrator of the list, in one launch.
+    Returns one (cost[n_cams], blocks[n_cams]) per calibrator, in order; residuals=True adds a third entry, the
+    residuals of Calibrator.evaluate(-1, residuals=True)."""
+    n = len(calibrators)
+    L = lib()
+    cost = [np.zeros(max(g.n_cams, 1)) for g in calibrators]
+    blocks = [np.zeros(max(g.n_cams, 1), dtype=np.int64) for g in calibrators]
+    res = [np.zeros(max(2 * g.n_obs, 1)) for g in calibrators] if residuals else None
+    hs = (C.c_void_p * max(n, 1))(*[g.h for g in calibrators])
+    cp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in cost])
+    bp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in blocks])
+    rp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in res]) if residuals else None
+    _batch_check(L, L.vcgpu_evaluate_batch(hs, C.c_int(n), cp, bp, rp), calibrators)
+    out = []
+    for g, c, b, k in zip(calibrators, cost, blocks, range(n)):
+        c, b = c[: g.n_cams], b[: g.n_cams]
+        out.append((c, b, res[k][: 2 * int(b.sum())]) if residuals else (c, b))
+    return out
+
+
+def remove_outliers_batch(calibrators, rmses, threshold):
+    """vcgpu_remove_outliers_batch: Calibrator.remove_outliers(rmses[i], threshold) of every Calibrator of the list,
+    in one launch.  Returns the removed counts, in order."""
+    n = len(calibrators)
+    L = lib()
+    rmse = [_c(r) for r in rmses]
+    hs = (C.c_void_p * max(n, 1))(*[g.h for g in calibrators])
+    rp = (C.c_void_p * max(n, 1))(*[r.ctypes.data for r in rmse])
+    removed = np.zeros(max(n, 1), dtype=np.int64)
+    _batch_check(L, L.vcgpu_remove_outliers_batch(hs, C.c_int(n), rp, C.c_double(threshold), _p(removed)), calibrators)
+    return [int(x) for x in removed[:n]]
+
+
+def _batch_check(L, rc, calibrators):
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        raise VcgpuError(f"vcgpu error {rc}: {msg}")

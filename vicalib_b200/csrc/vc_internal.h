@@ -167,7 +167,7 @@ struct vcgpu_handle {
   // The others are constant to the solve and left out of x_norm (as Ceres drops parameter blocks no residual uses)
   std::vector<uint8_t> h_frame_used;
   uint8_t* d_frame_used = nullptr;
-  double* d_r = nullptr;          // [2][n_obs] loss-corrected residuals
+  double* d_r = nullptr;          // [2][n_obs] loss-corrected residuals (vcgpu_evaluate_batch: [n_obs][2] loss-free, caller order)
   double* d_J = nullptr;          // per camera: [2*(12+K)][n_obs_cam] column SoA, loss-corrected (two-pass path / hooks only)
   int64_t j_doubles = 0;
   double* d_cost_part = nullptr;  // per eval block partial costs
@@ -193,6 +193,11 @@ struct vcgpu_handle {
   // the batch calls (vc_batch.inl): the kernel arguments of every rig of a batch this handle was handle 0 of, laid out
   // by the call
   unsigned char* d_batch_args = nullptr;
+  // vcgpu_evaluate_batch / vcgpu_remove_outliers_batch of a batch this handle was handle 0 of: the tiles' partials, the
+  // per-camera costs and tickets, and every rig's outlier marks (vc_batch.inl: run_evaluate_batch)
+  unsigned char* d_eval = nullptr;
+  // vcgpu_evaluate_batch with residuals: [n_obs] each sorted observation's place in caller order, when that is not its own
+  int32_t* d_rank = nullptr;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

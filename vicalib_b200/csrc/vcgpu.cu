@@ -30,6 +30,7 @@
 #include "vc_imu_mega.cuh"
 #include "vc_imu_eval_mega.cuh"
 #include "vc_pnp.cuh"
+#include "vc_eval_batch.cuh"
 
 using namespace vc;
 
@@ -219,7 +220,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -846,6 +847,18 @@ extern "C" int vcgpu_remove_outliers(vcgpu_handle* h, const double* rmse, double
   if (removed) h->dirty = true;
   if (n_removed) *n_removed = removed;
   return VCGPU_OK;
+}
+extern "C" int vcgpu_evaluate_batch(vcgpu_handle* const* handles, int n, double* const* cam_cost, int64_t* const* cam_blocks,
+                                    double* const* residuals_or_null) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!cam_cost) return batch_refuse(handles, n, 0, "null cam_cost array", "vcgpu_evaluate_batch");
+  return run_evaluate_batch(handles, n, EvalBatchOut{cam_cost, cam_blocks, residuals_or_null, nullptr, 0.0, nullptr});
+}
+extern "C" int vcgpu_remove_outliers_batch(vcgpu_handle* const* handles, int n, const double* const* rmse, double threshold,
+                                           int64_t* n_removed) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!rmse) return batch_refuse(handles, n, 0, "null rmse array", "vcgpu_remove_outliers_batch");
+  return run_evaluate_batch(handles, n, EvalBatchOut{nullptr, nullptr, nullptr, rmse, threshold, n_removed});
 }
 extern "C" int vcgpu_get_obs_active(vcgpu_handle* h, uint8_t* active) {
   if (!h || !active) return VCGPU_ERR_INVALID;
