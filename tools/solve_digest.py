@@ -5,11 +5,12 @@
 Solves the workload (default config2) with LM and DOGLEG on the persistent kernel and on the multi-launch engine
 (vcgpu_set_profiling's multi-launch bit), and 8 rigs of config 1's shape with one vcgpu_solve_batch per strategy; then
 the inertial LM solve on the persistent inertial kernels: the target workload (weights held) and config3 with live
-weights; then one vcgpu_solve_batch_inertial of four rigs of cluster sizes 1, 2, 4 and 8 (live weights on one), and one
-vcgpu_get_covariance_batch of two vision rigs and those four.  Prints, per case, the iterations, the final cost and
-last trust-region radius as hex floats and a SHA-256 of the final state (inertial: with velocities, IMU parameters and
-the weights), per covariance its status and a SHA-256 of the matrix; with out.npz also stores the states, costs, radii
-and matrices.  Equal lines mean bit-for-bit equal results.
+weights; then one vcgpu_solve_batch_inertial of four rigs of cluster sizes 1, 2, 4 and 8 (live weights on one), one
+vcgpu_get_covariance_batch and one vcgpu_get_frame_covariance_batch of two vision rigs and those four, and
+vcgpu_get_covariance and vcgpu_get_frame_covariance of one vision rig and one inertial rig of them.  Prints, per case,
+the iterations, the final cost and last trust-region radius as hex floats and a SHA-256 of the final state (inertial:
+with velocities, IMU parameters and the weights), per covariance its status and a SHA-256 of the matrix or blocks; with
+out.npz also stores the states, costs, radii and matrices.  Equal lines mean bit-for-bit equal results.
 """
 import hashlib
 import os
@@ -19,7 +20,8 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from vicalib_b200 import synth
-from vicalib_b200.capi import Calibrator, VcgpuError, covariance_batch, solve_batch, solve_batch_inertial
+from vicalib_b200.capi import (Calibrator, VcgpuError, covariance_batch, frame_covariance_batch, solve_batch,
+                               solve_batch_inertial)
 
 wl = sys.argv[1] if len(sys.argv) > 1 else "config2"
 KEYS = ("intr", "q_ck", "p_ck", "T_wp")
@@ -79,17 +81,30 @@ for i, models in enumerate((("poly3",), ("fov", "kb4"))):
     g.load(synth.make_problem(models=models, n_frames=20 + 20 * i, grid=(10, 7), seed=1200 + i))
     vis_rigs.append(g)
 cov_rigs = [vis_rigs[0], imu_rigs[0], imu_rigs[3], vis_rigs[1], imu_rigs[1], imu_rigs[2]]
-try:
-    covs, status = covariance_batch(cov_rigs), [0] * len(cov_rigs)
-except VcgpuError as e:
-    if getattr(e, "status", None) is None:
-        raise
-    covs, status = e.covariances, e.status
-for i, (c, st) in enumerate(zip(covs, status)):
-    name = f"covariance batch rig {i}"
+
+
+def report_cov(name, c, st):
     if c is not None:
         out[name] = c
     print(f"{name:24s} status {st:2d}  cov {hashlib.sha256(c.tobytes()).hexdigest()[:16] if c is not None else '-'}")
+
+
+for what, batch in (("covariance", covariance_batch), ("frame covariance", frame_covariance_batch)):
+    try:
+        covs, status = batch(cov_rigs), [0] * len(cov_rigs)
+    except VcgpuError as e:
+        if getattr(e, "status", None) is None:
+            raise
+        covs, status = e.covariances, e.status
+    for i, (c, st) in enumerate(zip(covs, status)):
+        report_cov(f"{what} batch rig {i}", c, st)
+for i in (0, 4):  # a vision rig and an inertial one
+    for what, call in (("covariance", Calibrator.covariance), ("frame covariance", Calibrator.frame_covariance)):
+        try:
+            c, st = call(cov_rigs[i]), 0
+        except VcgpuError as e:
+            c, st = None, int(str(e).split()[2].rstrip(":"))
+        report_cov(f"{what} rig {i}", c, st)
 for g in imu_rigs + vis_rigs:
     g.close()
 if len(sys.argv) > 2:

@@ -1397,6 +1397,12 @@ struct ChainCovArgs {
   ChainSolveArgs s;
   const double* mask;
   double* cov;
+  // frame mode (chain_frame_cov_batch_kernel; D2x: the frame damping of vcgpu_get_frame_covariance): every level's Σ
+  // blocks, the inverse of [globals | top nodes] [N*N] and the blocks written [nf][81], rows and columns from `live` on 0
+  SigmaLevel sig[kMaxChainLevels];
+  double* inv;
+  double* out;
+  int live;
 };
 // A batch of inertial rigs, one thread-block cluster each: cluster k writes the covariance of args[k] (vcgpu_get_covariance_batch).
 __global__ void __launch_bounds__(kCsThreads, 1) chain_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
@@ -1415,26 +1421,16 @@ __host__ __device__ inline size_t chain_frame_cov_smem_bytes(int G) {
   const size_t solve = chain_solve_smem_doubles(G) * sizeof(double), walk = chain_walk_chunks(G) * chain_selinv_smem_bytes<9>(G, kCsChunk);
   return solve > walk ? solve : walk;
 }
-// a rig as chain_frame_cov_batch_kernel takes it: the solve's arguments (D2x: the frame damping of
-// vcgpu_get_frame_covariance; scalars[kScNotPD] zeroed), every level's Σ blocks, the inverse of [globals | top nodes]
-// [N*N] and the blocks written [nf][81], rows and columns from `live` on 0
-struct ChainFrameCovArgs {
-  ChainSolveArgs s;
-  SigmaLevel sig[kMaxChainLevels];
-  double* inv;
-  double* out;
-  int live;
-};
 // A batch of inertial rigs, one thread-block cluster each: cluster k writes the frame covariance of args[k].  The
 // elimination and the dense factorisation of chain_solve; CTA 0's warps solve the N unit right-hand sides (the whole
 // inverse of [globals | top nodes], as dense_solve_kernel's mode 3 gives it) and leave the top nodes' blocks; then the
 // levels top-down, a cluster barrier between two, their chunks spread over the CTAs (chain_selinv_chunk); then level 0
 // unscaled.
-__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainFrameCovArgs* __restrict__ args) {
+__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
   extern __shared__ double smem[];
   constexpr int FD = 9;
   ClusterScope scope;
-  const ChainFrameCovArgs& a = args[blockIdx.x / scope.nb()];
+  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
   chain_solve<ClusterScope, true, true>(a.s, scope);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, grp = tid / kCsGroup, gtid = tid - grp * kCsGroup;
   const int bid = scope.bid(), nb = scope.nb();

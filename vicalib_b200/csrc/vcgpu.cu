@@ -779,7 +779,7 @@ extern "C" int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int
 extern "C" int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_covariance_batch");
-  return run_covariance_batch(handles, n, cov, status);
+  return run_cov_batch(handles, n, cov, status, false);
 }
 extern "C" int vcgpu_iterate(vcgpu_handle* h, int n, vcgpu_summary* out) {
   if (!h || n <= 0) return VCGPU_ERR_INVALID;
@@ -986,7 +986,8 @@ extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   VC_TRY(prepare(h));
   std::vector<double> mask, D2;
-  VC_TRY(cov_prelude(h, &mask, &D2));
+  VC_TRY(cov_prelude(h, false, &D2));
+  fill_mask(h, &mask);
   const DevProblem& dp = h->dp;
   const int G = dp.G;
   const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + G;
@@ -1074,13 +1075,11 @@ extern "C" int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   if (h->nranks > 1) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_frame_covariance is one-GPU only: frame shards are not supported");
   VC_TRY(prepare(h));
-  std::vector<double> mask, D2;
-  VC_TRY(cov_prelude(h, &mask, &D2));
+  std::vector<double> D2;
+  int live = 0;
+  VC_TRY(cov_prelude(h, true, &D2, &live));
   const DevProblem& dp = h->dp;
   const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + dp.G;
-  std::vector<double> D2f(D2);
-  const int live = frame_cov_damping(h, &D2f);
-  CUDA_TRY(h, cudaMemcpyAsync(h->d_scale + np, D2f.data(), np * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
   FrameCovSpace w;
   int rc = frame_cov_space(h, &w);
@@ -1095,7 +1094,7 @@ extern "C" int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov) {
 extern "C" int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_frame_covariance_batch");
-  return run_frame_covariance_batch(handles, n, cov, status);
+  return run_cov_batch(handles, n, cov, status, true);
 }
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp
