@@ -245,6 +245,34 @@ int vcgpu_num_globals(vcgpu_handle* h, int* out); /* sum_c (6 + K_c) (+15 with i
 int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t* cam_id, const int64_t* start, const int32_t* count,
                           const double* pix, const double* pw, int robust_its, double robust_tol, double* T_cw /*n_views*7*/,
                           double* rmse_or_null, int32_t* n_used_or_null);
+/* one rig's views for vcgpu_pose_pnp_ransac_batch: exactly vcgpu_pose_pnp_ransac's view arguments and outputs */
+typedef struct {
+  int n_views;
+  const int32_t* cam_id;   /* n_views */
+  const int64_t* start;    /* n_views */
+  const int32_t* count;    /* n_views */
+  const double* pix;       /* [..][2] */
+  const double* pw;        /* [..][3] */
+  double* T_cw;            /* n_views * 7 */
+  double* rmse_or_null;    /* n_views, or NULL */
+  int32_t* n_used_or_null; /* n_views, or NULL */
+} vcgpu_pnp_views;
+/* vcgpu_pose_pnp_ransac of n rigs in one call: views[i] are rig i's views, seen by handles[i]'s cameras (those of
+ * vcgpu_set_cameras).  Every rig's outputs are the bits vcgpu_pose_pnp_ransac(handles[i], ...) writes for the same views,
+ * whatever else is in the batch and in whatever order: a view's RANSAC draws are seeded by its index within its rig.
+ * A rig with n_views = 0 is allowed and gets nothing written.  One launch covers every view of every rig, one warp per
+ * view; every rig's views and correspondences are packed into one upload and all outputs come back in one download, all
+ * on handle 0's stream.  The correspondences of a view are copied per view, so views may share correspondences.
+ * Returns VCGPU_ERR_INVALID before anything is uploaded or launched and writes nothing, with a message naming the rig's
+ * index (and for a bad view the view's index) in vcgpu_last_error of every non-null handle, for: n <= 0, a null views,
+ * a null or repeated handle, handles on different devices, a handle without cameras, n_views < 0, a rig with views and
+ * a null cam_id, start, count, pix, pw or T_cw, and a view vcgpu_pose_pnp_ransac refuses (cam_id outside the handle's
+ * cameras, start < 0 or count < 0).
+ * Memory, held by handle 0 and grown to the largest batch, never freed per call: on the device 672 bytes per rig, 92
+ * per view and 57 per correspondence; in page-locked host memory the same without the scratch, 40 bytes per
+ * correspondence instead of 57. */
+int vcgpu_pose_pnp_ransac_batch(vcgpu_handle* const* handles, int n, const vcgpu_pnp_views* views, int robust_its,
+                                double robust_tol);
 
 /* GetSolutionCovariance (vicalibrator.h:802-857; compiled out upstream behind COMPUTE_VICALIB_COVARIANCE): the
  * [globals, globals] block of (J^T J)^-1 at the current state, tangent space, G x G row-major with G = vcgpu_num_globals:

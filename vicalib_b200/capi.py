@@ -26,7 +26,7 @@ EXPORTS = [
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
     "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch", "vcgpu_evaluate_batch", "vcgpu_remove_outliers_batch",
-    "vcgpu_pose_pnp_ransac",
+    "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch",
 ]
 
 
@@ -53,6 +53,13 @@ class Summary(C.Structure):
     _fields_ = [("iterations", C.c_int), ("successful_steps", C.c_int), ("termination", C.c_int),
                 ("num_residuals", C.c_int), ("initial_cost", C.c_double), ("final_cost", C.c_double),
                 ("device_seconds", C.c_double), ("kernel_launches", C.c_int)]
+
+
+class PnpViews(C.Structure):
+    """vcgpu_pnp_views: one rig's views and outputs of vcgpu_pose_pnp_ransac_batch"""
+    _fields_ = [("n_views", C.c_int), ("cam_id", C.c_void_p), ("start", C.c_void_p), ("count", C.c_void_p),
+                ("pix", C.c_void_p), ("pw", C.c_void_p), ("T_cw", C.c_void_p), ("rmse_or_null", C.c_void_p),
+                ("n_used_or_null", C.c_void_p)]
 
 
 class Config(C.Structure):
@@ -451,6 +458,27 @@ def remove_outliers_batch(calibrators, rmses, threshold):
     removed = np.zeros(max(n, 1), dtype=np.int64)
     _batch_check(L, L.vcgpu_remove_outliers_batch(hs, C.c_int(n), rp, C.c_double(threshold), _p(removed)), calibrators)
     return [int(x) for x in removed[:n]]
+
+
+def pose_pnp_batch(entries, robust_its=0, robust_tol=0.0):
+    """vcgpu_pose_pnp_ransac_batch: Calibrator.pose_pnp_ransac of every rig in one launch.  entries: one
+    (Calibrator, (cam_id, start, count, pix, pw)) per rig, the view arguments of Calibrator.pose_pnp_ransac.  Returns one
+    (T_cw [n, 7], rmse [n], n_used [n]) per rig, in order; each is the bits the rig's own call returns."""
+    n = len(entries)
+    L = lib()
+    keep, outs = [], []
+    views = (PnpViews * max(n, 1))()
+    for k, (g, (cam_id, start, count, pix, pw)) in enumerate(entries):
+        ins = [_c(cam_id, np.int32), _c(start, np.int64), _c(count, np.int32), _c(pix), _c(pw)]
+        m = len(ins[0])
+        out = (np.zeros((m, 7)), np.zeros(m), np.zeros(m, dtype=np.int32))
+        keep.append(ins)
+        outs.append(out)
+        views[k] = PnpViews(m, *[a.ctypes.data for a in ins], *[a.ctypes.data for a in out])
+    hs = (C.c_void_p * max(n, 1))(*[g.h for g, _ in entries])
+    _batch_check(L, L.vcgpu_pose_pnp_ransac_batch(hs, C.c_int(n), views, C.c_int(robust_its), C.c_double(robust_tol)),
+                 [g for g, _ in entries])
+    return outs
 
 
 def _batch_check(L, rc, calibrators):

@@ -198,6 +198,10 @@ struct vcgpu_handle {
   unsigned char* d_eval = nullptr;
   // vcgpu_evaluate_batch with residuals: [n_obs] each sorted observation's place in caller order, when that is not its own
   int32_t* d_rank = nullptr;
+  // vcgpu_pose_pnp_ransac_batch of a batch this handle was handle 0 of: the packed inputs, outputs and scratch
+  // (d_pnp), and the packed inputs and outputs in page-locked host memory (h_pnp) (vc_batch.inl: run_pnp_batch)
+  unsigned char* d_pnp = nullptr;
+  std::vector<unsigned char, PinnedAlloc<unsigned char>> h_pnp;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

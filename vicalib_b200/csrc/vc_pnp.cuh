@@ -12,6 +12,7 @@
 //   robust_its > 0: RANSAC over 4-point homographies (deterministic sample sequence), steps 2-4 on the inliers.
 // CPU restatement: oracle/pnp.py.  The frame pose handed to the solve is T_wp = T_cw^-1 * T_ck (vicalib-task.cc:341-349).
 #pragma once
+#include "vc_internal.h"
 #include "vc_math.cuh"
 
 namespace vc {
@@ -291,36 +292,28 @@ __device__ inline void mat_to_quat(const double m[9], double q[4]) {
   for (int k = 0; k < 4; ++k) q[k] *= n;
 }
 
-__global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
-  __shared__ WarpMem wm[kWarps];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int v = blockIdx.x * kWarps + warp;
-  if (v >= a.n_views) return;
-  WarpMem* sm = &wm[warp];
-  const int cnt = a.count[v];
-  const int64_t s0 = a.start[v];
-  const double* pw = a.pw + 3 * s0;
-  double* xy = a.xy + 2 * s0;
-  unsigned char* use = a.use + s0;
-  const int cam = a.cam[v], model = a.model[cam];
-  const double* intr = a.intr + 10 * cam;
-  if (lane == 0) { a.n_used[v] = 0; a.rmse[v] = 0.0; }
-  if (lane < 7) a.T_cw[7 * static_cast<int64_t>(v) + lane] = lane == 3 ? 1.0 : 0.0;
+// One view on one warp: cnt correspondences pix [cnt][2] / pw [cnt][3] of a camera of `model` / `intr`, scratch xy
+// [cnt][2] / use [cnt]; the RANSAC draws are seeded by (seed, draw).  Writes T_cw [7], *rmse and *n_used.
+__device__ __forceinline__ void pose_pnp_view(int seed, int cnt, const double* pix, const double* pw, int model, const double* intr,
+                                              int robust_its, double robust_tol, double* xy, unsigned char* use, WarpMem* sm,
+                                              int lane, double* T_cw, double* rmse, int32_t* n_used) {
+  if (lane == 0) { *n_used = 0; *rmse = 0.0; }
+  if (lane < 7) T_cw[lane] = lane == 3 ? 1.0 : 0.0;
   if (cnt < 4) return;
   for (int i = lane; i < cnt; i += 32) {
-    unproject(model, intr, a.pix[2 * (s0 + i)], a.pix[2 * (s0 + i) + 1], &xy[2 * i], &xy[2 * i + 1]);
+    unproject(model, intr, pix[2 * i], pix[2 * i + 1], &xy[2 * i], &xy[2 * i + 1]);
     use[i] = 1;
   }
   __syncwarp();
   double H[9];
   int n_use = cnt;
-  if (a.robust_its > 0) {
+  if (robust_its > 0) {
     double Hbest[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
     int best = -1;
-    for (int it = 0; it < a.robust_its; ++it) {
+    for (int it = 0; it < robust_its; ++it) {
       // 4 distinct indices from a linear congruential sequence seeded by (view, draw): the same on every lane
       int idx[4];
-      unsigned s = static_cast<unsigned>(v) * 2654435761u + static_cast<unsigned>(it) * 40503u + 12345u;
+      unsigned s = static_cast<unsigned>(seed) * 2654435761u + static_cast<unsigned>(it) * 40503u + 12345u;
       int got = 0;
       while (got < 4) {
         s = s * 1664525u + 1013904223u;
@@ -337,7 +330,7 @@ __global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
         const double X = pw[3 * i], Y = pw[3 * i + 1];
         const double qz = H[6] * X + H[7] * Y + H[8];
         const double ex = (H[0] * X + H[1] * Y + H[2]) / qz - xy[2 * i], ey = (H[3] * X + H[4] * Y + H[5]) / qz - xy[2 * i + 1];
-        inl += sqrt(ex * ex + ey * ey) < a.robust_tol ? 1 : 0;
+        inl += sqrt(ex * ex + ey * ey) < robust_tol ? 1 : 0;
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) inl += __shfl_xor_sync(0xffffffffu, inl, o);
@@ -353,7 +346,7 @@ __global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
       const double X = pw[3 * i], Y = pw[3 * i + 1];
       const double qz = Hbest[6] * X + Hbest[7] * Y + Hbest[8];
       const double ex = (Hbest[0] * X + Hbest[1] * Y + Hbest[2]) / qz - xy[2 * i], ey = (Hbest[3] * X + Hbest[4] * Y + Hbest[5]) / qz - xy[2 * i + 1];
-      const int ok = sqrt(ex * ex + ey * ey) < a.robust_tol ? 1 : 0;
+      const int ok = sqrt(ex * ex + ey * ey) < robust_tol ? 1 : 0;
       use[i] = static_cast<unsigned char>(ok);
       n_use += ok;
     }
@@ -447,12 +440,62 @@ __global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
   }
   double q[4];
   mat_to_quat(R, q);
-  if (lane < 4) a.T_cw[7 * static_cast<int64_t>(v) + lane] = q[lane];
-  else if (lane < 7) a.T_cw[7 * static_cast<int64_t>(v) + lane] = t[lane - 4];
+  if (lane < 4) T_cw[lane] = q[lane];
+  else if (lane < 7) T_cw[lane] = t[lane - 4];
   if (lane == 0) {
-    a.n_used[v] = n_use;
-    a.rmse[v] = sqrt(cost / n_use);
+    *n_used = n_use;
+    *rmse = sqrt(cost / n_use);
   }
+}
+
+// vcgpu_pose_pnp_ransac: one warp per view of one handle, seeded by the view's index
+__global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
+  __shared__ WarpMem wm[kWarps];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int v = blockIdx.x * kWarps + warp;
+  if (v >= a.n_views) return;
+  const int64_t s0 = a.start[v];
+  const int cam = a.cam[v];
+  pose_pnp_view(v, a.count[v], a.pix + 2 * s0, a.pw + 3 * s0, a.model[cam], a.intr + 10 * cam, a.robust_its, a.robust_tol,
+                a.xy + 2 * s0, a.use + s0, &wm[warp], lane, a.T_cw + 7 * static_cast<int64_t>(v), a.rmse + v, a.n_used + v);
+}
+
+// vcgpu_pose_pnp_ransac_batch: one warp per view of every rig of the batch, the views of a rig one after the other and
+// each view's correspondences packed behind the previous view's.  A view reads its camera from its rig's table and
+// seeds its RANSAC draws with its index within its rig, so a rig's poses are the bits its vcgpu_pose_pnp_ransac gives.
+struct BatchRig {
+  int32_t model[kMaxCams];
+  double intr[kMaxCams][10];
+};
+struct BatchView {
+  int64_t at;     // first correspondence of the view in pix / pw / xy / use
+  int32_t rig;    // index into rigs
+  int32_t index;  // the view's index within its rig: the RANSAC seed
+  int32_t cam, count;
+};
+struct BatchArgs {
+  int64_t n_views;
+  const BatchRig* rigs;
+  const BatchView* views;
+  const double* pix;   // [N][2]
+  const double* pw;    // [N][3]
+  int robust_its;
+  double robust_tol;
+  double* xy;          // [N][2] scratch
+  unsigned char* use;  // [N] scratch
+  double* T_cw;        // [n_views][7]
+  double* rmse;        // [n_views]
+  int32_t* n_used;     // [n_views]
+};
+__global__ void __launch_bounds__(32 * kWarps) pose_pnp_batch_kernel(BatchArgs a) {
+  __shared__ WarpMem wm[kWarps];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int64_t v = static_cast<int64_t>(blockIdx.x) * kWarps + warp;
+  if (v >= a.n_views) return;
+  const BatchView w = a.views[v];
+  const BatchRig& r = a.rigs[w.rig];
+  pose_pnp_view(w.index, w.count, a.pix + 2 * w.at, a.pw + 3 * w.at, r.model[w.cam], r.intr[w.cam], a.robust_its, a.robust_tol,
+                a.xy + 2 * w.at, a.use + w.at, &wm[warp], lane, a.T_cw + 7 * v, a.rmse + v, a.n_used + v);
 }
 
 }  // namespace pnp

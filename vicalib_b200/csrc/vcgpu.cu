@@ -220,7 +220,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -1158,6 +1158,13 @@ extern "C" int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t
   if (rmse) std::copy(hr.begin(), hr.end(), rmse);
   if (n_used) std::copy(hu.begin(), hu.end(), n_used);
   return VCGPU_OK;
+}
+
+extern "C" int vcgpu_pose_pnp_ransac_batch(vcgpu_handle* const* handles, int n, const vcgpu_pnp_views* views, int robust_its,
+                                           double robust_tol) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!views) return batch_refuse(handles, n, 0, "null views array", "vcgpu_pose_pnp_ransac_batch");
+  return run_pnp_batch(handles, n, views, robust_its, robust_tol);
 }
 
 extern "C" int vcgpu_eval_imu(vcgpu_handle* h, double* r, double* J) {
