@@ -146,7 +146,7 @@ int vcgpu_solve(vcgpu_handle* h, vcgpu_iter_cb cb, void* user, vcgpu_summary* ou
  * of that launch); kernel_launches counts the rig's own start-point launches plus that one.
  * Returns VCGPU_ERR_INVALID before anything is launched, with a message naming the index in vcgpu_last_error of every
  * non-null handle of the batch, for: n <= 0, a null or repeated handle, handles on different devices, and a handle
- * that has inertial terms on, frame shards, a vcgpu_set_profiling bit (1, 2, 4) or L2 flushing set,
+ * that has inertial terms on, frame shards, a vcgpu_set_profiling bit (1, 4) or L2 flushing set,
  * update_state_every_iteration set, no active observation, or a rig too large for the persistent vision kernel.
  * There is no sequential fallback: call vcgpu_solve on such a handle.  A refused batch leaves its handles as they were.
  * Device memory: nothing beyond what each handle holds for vcgpu_solve, which includes a 32 MiB totals buffer per
@@ -172,7 +172,7 @@ int vcgpu_batch_plan(vcgpu_handle* h, int* cluster_size, int* warps, int* reside
  * Returns VCGPU_ERR_INVALID before any kernel is launched, with a message naming the index in vcgpu_last_error of
  * every non-null handle of the batch, for: n <= 0, a null or repeated handle, handles on different devices, and a
  * handle without inertial terms (vision rigs: vcgpu_solve_batch), with strategy 1 (inertial DOGLEG runs on the
- * multi-launch engine), frame shards, a vcgpu_set_profiling bit or L2 flushing set, update_state_every_iteration set,
+ * multi-launch engine), frame shards, a vcgpu_set_profiling bit (1, 4, 8) or L2 flushing set, update_state_every_iteration set,
  * or a rig the persistent inertial kernels do not fit (G >= 68 on an H100).  There is no sequential fallback: call
  * vcgpu_solve on such a handle.  A refused batch leaves its handles as they were.
  * Device memory: nothing beyond what each handle holds for vcgpu_solve, and n x ~5 KB of kernel arguments held by
@@ -188,18 +188,21 @@ int vcgpu_iterate(vcgpu_handle* h, int n_iterations, vcgpu_summary* out);
 
 /* Problem::Evaluate with residual_blocks = camera `cam` (or all visual blocks if cam < 0),
  * apply_loss_function = false: cost = 1/2 sum |r|^2, residuals in caller observation order
- * (2 per active observation of that camera)  (vicalibrator.h:873-887, 958-966) */
+ * (2 per active observation of that camera)  (vicalibrator.h:873-887, 958-966).  Runs as vcgpu_evaluate_batch of this
+ * handle alone: the cost of cam < 0 is the sum of the per-camera costs, and the handle keeps that call's device memory.
+ * Unlike the batch call it takes frame shards, each evaluating its own observations.  VCGPU_ERR_INVALID: cam >= the
+ * number of cameras. */
 int vcgpu_evaluate(vcgpu_handle* h, int cam, double* cost, double* residuals_or_null, int64_t* n_blocks);
 /* total robustified cost 1/2 sum rho(|r|^2) over all active residual blocks at the current state */
 int vcgpu_cost(vcgpu_handle* h, double* cost);
-/* RemoveOutliers (vicalibrator.h:859-916): drops observations with |r| > threshold * rmse[cam] */
+/* RemoveOutliers (vicalibrator.h:859-916): drops observations with |r| > threshold * rmse[cam].  Runs as
+ * vcgpu_remove_outliers_batch of this handle alone, and takes frame shards. */
 int vcgpu_remove_outliers(vcgpu_handle* h, const double* rmse, double threshold, int64_t* n_removed);
 int vcgpu_get_obs_active(vcgpu_handle* h, uint8_t* active /*n_obs, caller order*/);
 /* vcgpu_evaluate of every camera of n rigs in one call.  Per rig i: cam_cost[i][c] = 1/2 sum |r|^2 over camera c's
  * active observations (loss-free, as vcgpu_evaluate(h, c)), and cam_blocks[i][c] their count (cam_blocks, or an entry of
  * it, may be NULL); residuals_or_null[i] (the array or an entry may be NULL) gets 2 doubles per active observation in
- * vcgpu_evaluate(h, -1, ...)'s layout, caller order.  The residuals are the bits vcgpu_evaluate returns and the counts
- * are equal; a cost equals vcgpu_evaluate's to rounding (the device sums in another order).  One launch covers every rig:
+ * vcgpu_evaluate(h, -1, ...)'s layout, caller order.  The residuals are the bits vcgpu_eval_reproj returns.  One launch covers every rig:
  * tiles of 256 consecutive observations of one camera, one CTA each, a tiling that is a function of the rig alone, so a
  * rig's costs are the same bits whatever else is in the batch and in whatever order.  Per handle, on its own stream,
  * the uploads of vcgpu_evaluate; then the launch and one download of the costs, and one of each rig's residuals.
@@ -215,8 +218,8 @@ int vcgpu_evaluate_batch(vcgpu_handle* const* handles, int n, double* const* cam
                          int64_t* const* cam_blocks /* n pointers to n_cams, or NULL */,
                          double* const* residuals_or_null /* n pointers to 2 * active observations, or NULL */);
 /* vcgpu_remove_outliers of n rigs in one call: rmse[i] holds rig i's n_cams values; an active observation of camera c
- * leaves the problem where |r| > threshold * rmse[i][c], exactly the set vcgpu_remove_outliers removes (the device forms
- * |r| without a fused multiply-add, as the host does).  n_removed: n counts, or NULL.  The residuals are computed as
+ * leaves the problem where |r| > threshold * rmse[i][c], |r| = sqrt(r0 * r0 + r1 * r1) formed without a fused
+ * multiply-add.  n_removed: n counts, or NULL.  The residuals are computed as
  * vcgpu_evaluate_batch computes them, in the same launch layout; the marks come back in one download.  A rig that loses
  * nothing is left exactly as it was.  Refusals as vcgpu_evaluate_batch, with a null rmse[i] in place of a null
  * cam_cost[i].  Device memory: vcgpu_evaluate_batch's, and one byte per active observation of every rig, held by
@@ -241,7 +244,8 @@ int vcgpu_num_globals(vcgpu_handle* h, int* out); /* sum_c (6 + K_c) (+15 with i
  * robust_its > 0: RANSAC over 4-point homographies with inlier tolerance robust_tol (normalised image coordinates);
  * the reference calls it with 0, 0.  Out: T_cw[v] = (qx qy qz qw tx ty tz), p_c = R p_w + t; rmse[v] in normalised
  * coordinates; n_used[v] = points in the final fit (0: fewer than 4 usable points, T_cw[v] = identity).
- * The frame pose the solve is seeded with is T_wp = T_cw^-1 * T_ck (vicalib-task.cc:341-349). */
+ * The frame pose the solve is seeded with is T_wp = T_cw^-1 * T_ck (vicalib-task.cc:341-349).
+ * Runs as vcgpu_pose_pnp_ransac_batch of this handle alone: the same refusals and memory, which the handle keeps. */
 int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t* cam_id, const int64_t* start, const int32_t* count,
                           const double* pix, const double* pw, int robust_its, double robust_tol, double* T_cw /*n_views*7*/,
                           double* rmse_or_null, int32_t* n_used_or_null);
@@ -295,7 +299,7 @@ int vcgpu_get_covariance(vcgpu_handle* h, double* cov);
  * message names the failing indices.
  * Returns VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in
  * vcgpu_last_error of every non-null handle, for: n <= 0, a null or repeated handle, a null cov[i], handles on
- * different devices, frame shards, any vcgpu_set_profiling bit or L2 flushing, and a rig the cluster kernels do not
+ * different devices, frame shards, any vcgpu_set_profiling bit (1, 4, 8) or L2 flushing, and a rig the cluster kernels do not
  * fit (vision: the persistent vision kernel's fit, or no active observation; inertial: G >= 68 on an H100).
  * Device memory: per handle G^2 + 16 doubles (vision rigs also 9 (G^2 + G) of workspace), and a few KB of kernel
  * arguments per rig, held by handle 0. */
@@ -323,7 +327,7 @@ int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov /* n_frames * fd * f
  * runs per group of like rigs; then one copy back per handle.  Nothing on the handle changes: state, IMU weights and what
  * a later vcgpu_solve or batch solve computes stay as they were.
  * status, VCGPU_ERR_NUMERIC and VCGPU_ERR_INVALID: as vcgpu_get_covariance_batch (the same refusals: n <= 0, a null or
- * repeated handle, a null cov[i], handles on different devices, frame shards, any vcgpu_set_profiling bit or L2 flushing,
+ * repeated handle, a null cov[i], handles on different devices, frame shards, any vcgpu_set_profiling bit (1, 4, 8) or L2 flushing,
  * and a rig the cluster kernels do not fit, which includes inertial G >= 68 on an H100).
  * Device memory: per handle the workspace of vcgpu_get_frame_covariance and that of vcgpu_get_covariance_batch, and a few
  * KB of kernel arguments per rig, held by handle 0. */
@@ -346,9 +350,9 @@ int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const double* D2, do
 
 /* ---- measurement hooks (bench.py) ------------------------------------------------------------
  * profile (bit mask): 1 = bracket every kernel stage of the multi-launch engine with CUDA events on the
- *          launching stream; 2 = two-pass path that materialises the Jacobian in HBM; 4 = multi-launch engine
- *          even where the persistent kernel applies; 8 = persistent kernel records per-phase device clocks
- *          (read back through vcgpu_get_stage_times)
+ *          launching stream; 4 = multi-launch engine even where the persistent kernel applies; 8 = persistent kernel
+ *          records per-phase device clocks (read back through vcgpu_get_stage_times).  Any other bit: VCGPU_ERR_INVALID,
+ *          and the handle is left as it was.
  * flush_l2: overwrite a 256 MiB scratch buffer before every iteration and time iterations
  *           individually, so no iteration starts with its inputs resident in the 50 MB L2 */
 enum {
@@ -356,7 +360,7 @@ enum {
   VCGPU_STAGE_FRAME_SOLVE = 1,  /* per-frame Cholesky + Schur contribution (or IMU chain elimination) */
   VCGPU_STAGE_GLOBAL_SOLVE = 2, /* dense reduced system */
   VCGPU_STAGE_BACKSUB = 3,      /* back-substitution + x (+) delta */
-  VCGPU_STAGE_EVAL_REPROJ = 4,  /* reprojection residual + Jacobian */
+  VCGPU_STAGE_EVAL_REPROJ = 4,  /* unused: the reprojection evaluation is part of VCGPU_STAGE_BUILD */
   VCGPU_STAGE_BUILD = 5,        /* per-frame block normal equations */
   VCGPU_STAGE_REDUCE = 6,       /* global block tree reduction, level 1 */
   VCGPU_STAGE_FINALIZE = 7,     /* level 2 + cost + gradient norms */

@@ -255,7 +255,7 @@ def test_refusals():
     _refused([good[0].g, good[1].g, good[0].g], 2)       # a repeated handle
     bads = [bad_with(flags=dict(visual=0)),              # no active observation
             bad_with(options=dict(update_state_every_iteration=1)),
-            bad_with(profiling=1), bad_with(profiling=2), bad_with(profiling=MULTI_LAUNCH),
+            bad_with(profiling=1), bad_with(profiling=MULTI_LAUNCH),
             Rig(models=("poly3",), n_frames=12, grid=(14, 10), inertial=True, seed=703, flags=dict(inertial=1), opts=opts),
             Rig(models=chain_plan.rig_with_globals(104, False), n_frames=12, grid=(14, 10), seed=704, opts=opts),  # beyond the fit
             bad_with(flush=True)]                        # L2 flushing
@@ -269,9 +269,14 @@ def test_refusals():
     _same_bits(good[1].solo(), ref1, "after the refusals")
     s = bads[1].g.solve()  # update_state_every_iteration: vcgpu_solve takes it
     assert s["iterations"] == 4
-    for bad in bads[2:5]:
+    # bit 2 is no profiling bit: set_profiling refuses it and leaves the handle solving as a fresh twin does
+    two = Rig(seed=702, opts=opts, **kw)
+    with pytest.raises(VcgpuError):
+        two.g.set_profiling(2, False)
+    _same_bits(two.solo(), Rig(seed=702, opts=opts, **kw).solo(), "set_profiling(2) refused")
+    for bad in bads[2:4]:
         bad.g.set_profiling(0, False)
-    after = _batch(bads[2:5])  # and, the bit cleared, the batch does
+    after = _batch(bads[2:4] + [Rig(seed=702, opts=opts, **kw)])  # and, the bit cleared, the batch does
     for a in after[1:]:
         _same_bits(a, after[0], "the same rig three times")
 

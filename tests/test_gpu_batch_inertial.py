@@ -278,7 +278,7 @@ def test_refusals():
         return r
 
     specs = [dict(flags=dict(inertial=0)), dict(options=dict(strategy=1)), dict(options=dict(update_state_every_iteration=1)),
-             dict(profiling=1), dict(profiling=2), dict(profiling=4), dict(profiling=8), dict(flush=True),
+             dict(profiling=1), dict(profiling=4), dict(profiling=8), dict(flush=True),
              dict(models=chain_plan.rig_with_globals(68), n_frames=12, grid=(14, 10))]
     assert chain_plan.rig_globals(specs[-1]["models"]) == 68
     _refused([], None)                                   # n = 0

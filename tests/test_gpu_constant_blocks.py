@@ -1,6 +1,6 @@
 """GPU: constant parameter blocks on every solve engine, against the CPU oracle (or a dense numpy solve where noted).
 
-- Normal equations with fixed intrinsics on each build path (fused, materialised, multi-launch inertial, eval_mega_kernel),
+- Normal equations with fixed intrinsics on each build path (fused, multi-launch inertial, eval_mega_kernel),
   and with residual-block multiplicities: 1e-10 relative per block family; the intrinsic columns of E and rows and
   columns of C and gc exactly 0.
 - The damped arrow solve with constant columns against numpy.linalg.solve with those columns deleted, where the LM
@@ -18,7 +18,7 @@ from vicalib_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
-MATERIALISE, MULTI_LAUNCH = 2, 4  # vcgpu_set_profiling bits 1 and 2
+MULTI_LAUNCH = 4  # vcgpu_set_profiling bit 2
 STAGES = [
     dict(inertial=1, rotation_only=1, bias_active=0, scale_active=0, optimize_ts=1),
     dict(inertial=1, rotation_only=0, bias_active=1, scale_active=0, optimize_ts=1),
@@ -73,7 +73,7 @@ def _check_ne(o, g, models, bar=1e-10):
 VISION_MODELS = [("linear",), ("fov",), ("poly2",), ("poly3",), ("kb4",), ("poly3", "fov", "kb4")]
 
 
-@pytest.mark.parametrize("mode", [0, MATERIALISE], ids=["fused", "materialised"])
+@pytest.mark.parametrize("mode", [0], ids=["fused"])
 @pytest.mark.parametrize("models", VISION_MODELS, ids=["+".join(m) for m in VISION_MODELS])
 def test_vision_normal_equations_fixed_intrinsics(models, mode):
     p = synth.make_problem(models=models, n_frames=12, grid=(14, 10), seed=7 + len(models))
@@ -105,7 +105,7 @@ def test_eight_cameras_fixed_intrinsics():
     assert not ne["E"][:, :, ic].any() and not ne["C"][ic].any() and not ne["gc"][ic].any()
 
 
-@pytest.mark.parametrize("mode", [0, MATERIALISE, MULTI_LAUNCH], ids=["fused", "materialised", "multi_launch"])
+@pytest.mark.parametrize("mode", [0, MULTI_LAUNCH], ids=["fused", "multi_launch"])
 @pytest.mark.parametrize("inertial", [False, True], ids=["vision", "inertial"])
 def test_multiplicities(inertial, mode):
     """visual_mult = 3, imu_mult = 2: the residual-block multiplicities of the staged flow scale every Gram build"""
@@ -212,7 +212,6 @@ def _engine(s, inertial, persistent):
 
 SOLVE_CASES = [
     ("vision_fix", cb.vision_problem, cb.FIX, 0, 0), ("vision_fix", cb.vision_problem, cb.FIX, 0, MULTI_LAUNCH),
-    ("vision_fix", cb.vision_problem, cb.FIX, 0, MATERIALISE),
     ("vision_fix", cb.vision_problem, cb.FIX, 1, 0), ("vision_fix", cb.vision_problem, cb.FIX, 1, MULTI_LAUNCH),
     ("inertial_fix", cb.inertial_problem, cb.INERTIAL_FIX, 0, 0),
     ("inertial_fix", cb.inertial_problem, cb.INERTIAL_FIX, 0, MULTI_LAUNCH),
@@ -222,7 +221,7 @@ SOLVE_CASES = [
     ("rotation_only", cb.inertial_problem, cb.STAGE_ROT_ONLY, 0, MULTI_LAUNCH),
     ("rotation_only", cb.inertial_problem, cb.STAGE_ROT_ONLY, 1, 0),
 ]
-_MODE = {0: "persistent", MULTI_LAUNCH: "multi_launch", MATERIALISE: "materialised"}
+_MODE = {0: "persistent", MULTI_LAUNCH: "multi_launch"}
 
 
 @pytest.mark.parametrize("name,make,flags,strategy,mode", SOLVE_CASES,

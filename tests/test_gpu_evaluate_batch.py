@@ -1,9 +1,10 @@
-"""GPU: vcgpu_evaluate_batch and vcgpu_remove_outliers_batch (eval_batch_kernel, one launch over tiles of every rig)
-against the per-handle vcgpu_evaluate and vcgpu_remove_outliers.  Residuals and counts must be the same bits, costs
-within 1e-13 relative (the device sums in another order), removal sets equal.  A rig's tiling is a function of the rig
-alone, so its outputs must not move, bit for bit, with the rest of the batch.  Not covered: handles on different
-devices and frame-sharded handles (both need more than one GPU); their refusals are argument checks next to the ones
-tested here.
+"""GPU: vcgpu_evaluate_batch and vcgpu_remove_outliers_batch (eval_batch_kernel, one launch over tiles of every rig),
+and the per-handle vcgpu_evaluate and vcgpu_remove_outliers, which run it as a batch of one.  The reference is code
+they do not share: the residuals of vcgpu_eval_reproj at the active observations, their per-camera costs summed in
+numpy and the outlier sets formed from them in numpy.  Residuals and counts must be the same bits, costs within 1e-13
+relative (the device sums in another order), removal sets equal.  A rig's tiling is a function of the rig alone, so
+its outputs must not move, bit for bit, with the rest of the batch.  Not covered: handles on different devices and
+frame-sharded handles (both need more than one GPU); their refusals are argument checks next to the ones tested here.
 """
 import ctypes as C
 
@@ -27,7 +28,24 @@ def _rig(models, n_frames, seed, inertial=False, grid=(10, 7), problem=None):
     g.load(p)
     if inertial:
         g.set_flags(**ALL_ON)
+    g.obs_cam = np.asarray(p.obs_cam)  # for _reference
     return g, p
+
+
+def _reference(g, obs_cam):
+    """(cost[n_cams], blocks[n_cams], residuals) of the active observations, caller order, from vcgpu_eval_reproj"""
+    act = g.obs_active().astype(bool)
+    r = g.eval_reproj(jac=False)[0][act]
+    cam = np.asarray(obs_cam)[act]
+    cost = np.array([0.5 * np.sum(r[cam == c, 0] * r[cam == c, 0] + r[cam == c, 1] * r[cam == c, 1]) for c in range(g.n_cams)])
+    return cost, np.array([(cam == c).sum() for c in range(g.n_cams)], dtype=np.int64), r.ravel()
+
+
+def _outliers(g, obs_cam, rmse, threshold):
+    """the active observations RemoveOutliers drops, formed in numpy from the residuals of vcgpu_eval_reproj"""
+    r = g.eval_reproj(jac=False)[0]
+    err = np.sqrt(r[:, 0] * r[:, 0] + r[:, 1] * r[:, 1])
+    return g.obs_active().astype(bool) & (err > threshold * np.asarray(rmse)[np.asarray(obs_cam)])
 
 
 def _per_handle(g):
@@ -76,7 +94,9 @@ def test_parity_mixed_batch():
                 g.solve(free_running=True)
         got = evaluate_batch(rigs, residuals=True)
         for k, (g, out) in enumerate(zip(rigs, got)):
-            _check(out, _per_handle(g), (state, k))
+            ref = _reference(g, g.obs_cam)
+            _check(out, ref, (state, k))
+            _check(_per_handle(g), ref, (state, k, "per handle"))
         assert got[-1][1].sum() == 0 and got[-2][1][1] == 0 and got[-2][1][0] > 0
     # without residuals, the same costs
     plain = evaluate_batch(rigs)
@@ -145,11 +165,14 @@ def test_outliers_match_per_handle():
     for g, s, r, p in zip(batch, solo, rmses, ps):
         assert np.array_equal(r, _rmse(s))
         assert _margin(g, p, r, threshold) > 1e-12
+    drop = [_outliers(g, p.obs_cam, r, threshold) for g, r, p in zip(batch, rmses, ps)]
+    keep = [g.obs_active().astype(bool) & ~d for g, d in zip(batch, drop)]
     counts = remove_outliers_batch(batch, rmses, threshold)
-    for g, s, r, bad, n in zip(batch, solo, rmses, bads, counts):
-        assert n == s.remove_outliers(r, threshold) and n >= len(bad)
+    for g, s, r, bad, n, d, k in zip(batch, solo, rmses, bads, counts, drop, keep):
+        assert n == s.remove_outliers(r, threshold) == d.sum() and n >= len(bad)
         act = g.obs_active()
         assert np.array_equal(act, s.obs_active())
+        assert np.array_equal(act.astype(bool), k)
         assert not act[bad].any()
 
 
@@ -260,14 +283,18 @@ def test_north_star_sized_rig():
         g.solve(free_running=True)
         gs.append(g)
     g, twin = gs
-    ref = _per_handle(g)
+    ref = _reference(g, p.obs_cam)
     _check(evaluate_batch([g], residuals=True)[0], ref, "target")
+    _check(_per_handle(g), ref, "target, per handle")
     rmse = _rmse(g)
     threshold = 2.5
     assert _margin(g, p, rmse, threshold) > 1e-12
+    drop = _outliers(g, p.obs_cam, rmse, threshold)
+    keep = g.obs_active().astype(bool) & ~drop
     n = remove_outliers_batch([g], [rmse], threshold)[0]
-    assert n == twin.remove_outliers(rmse, threshold) and n > 0
+    assert n == twin.remove_outliers(rmse, threshold) == drop.sum() and n > 0
     assert np.array_equal(g.obs_active(), twin.obs_active())
+    assert np.array_equal(g.obs_active().astype(bool), keep)
 
 
 # ------------------------------------------------------------------ 7. refusals

@@ -1,6 +1,8 @@
 """GPU: vcgpu_pose_pnp_ransac_batch (pose_pnp_batch_kernel, one warp per view of every rig) against
-vcgpu_pose_pnp_ransac on the same handle and views.  T_cw, rmse and n_used must be the same bits, whatever else is in
-the batch and in whatever order: the batch seeds a view's RANSAC draws with its index within its rig.  Not covered:
+vcgpu_pose_pnp_ransac on the same handle and views, which is a batch of one: what the comparisons check is the packing
+of many rigs and the seeding (test_gpu_pnp.py checks the poses against the oracle).  T_cw, rmse and n_used must be the
+same bits, whatever else is in the batch and in whatever order: the batch seeds a view's RANSAC draws with its index
+within its rig.  Not covered:
 handles on different devices (that needs more than one GPU); its refusal is an argument check next to the ones tested
 here.
 """

@@ -304,6 +304,8 @@ class Calibrator:
               "finalize", "imu_eval", "imu_weights", "grid_sync", "eval_tasks", "imu_accumulate"]
 
     def set_profiling(self, profile=True, flush_l2=False):
+        """profile bits: 1 stage events (multi-launch engine), 4 multi-launch engine, 8 persistent-kernel phase clocks;
+        any other bit raises VcgpuError and leaves the handle as it was"""
         self._chk(self.L.vcgpu_set_profiling(self.h, C.c_int(int(profile)), C.c_int(int(flush_l2))))
 
     def fp64_peak(self, device=0):

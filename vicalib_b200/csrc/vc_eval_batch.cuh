@@ -1,5 +1,5 @@
-// vcgpu_evaluate_batch and vcgpu_remove_outliers_batch: the loss-free reprojection residuals of every camera of many rigs
-// in one launch, reduced per (rig, camera) on the device.
+// vcgpu_evaluate, vcgpu_remove_outliers and their batches: the loss-free reprojection residuals (reproj_residual) of
+// every camera of one or many rigs in one launch, reduced per (rig, camera) on the device.
 //
 // The work is cut into tiles of kEvalTile consecutive observations of one (rig, camera) in the rig's sorted (camera,
 // frame) order, one CTA per tile.  The tiling is a function of the rig alone, so a large rig spreads over the whole GPU
@@ -22,10 +22,10 @@ struct EvalBatchRig {
   const int32_t* frame;
   const double *pw, *pc;     // AoS [n][3], [n][2]
   const int32_t* rank;       // sorted index -> index among the active observations in caller order; null: the same
-  double* res;               // null, or [2 * n_obs]: vcgpu_evaluate(cam = -1)'s layout
+  double* res;               // null, or [2 * n_obs]: the active observations' residuals in caller order
   uint8_t* mark;             // null, or [n_obs] sorted: 1 where |r| > limit[camera]
   int model[kMaxCams], obs_start[kMaxCams], n_obs[kMaxCams];
-  double limit[kMaxCams];    // threshold * rmse[c], formed on the host as vcgpu_remove_outliers forms it
+  double limit[kMaxCams];    // threshold * rmse[c], formed on the host
 };
 // tile `tile` of the n_tiles of camera `cam` of rig `rig`; its partial goes to part[part0 + tile], the camera's cost and
 // ticket counter are entry `sum`
@@ -38,23 +38,13 @@ struct EvalBatchArgs {
   unsigned* counter;   // tickets per (rig, camera) entry, zero at launch
 };
 
-// the loss-free residual of sorted observation i: eval_reproj_kernel<MODEL, false>'s arithmetic, operation for operation
+// the residual of sorted observation i of camera c of rig g
 template <int MODEL>
 __device__ __forceinline__ void eval_batch_residual(const EvalBatchRig& g, const double* state, int c, int64_t i, double* r0, double* r1) {
-  const double* cam = state + g.off_cam + kCamStateStride * c;
-  const double* T = state + 7 * static_cast<int64_t>(g.frame[i]);
-  const Q4 q{T[0], T[1], T[2], T[3]};
-  const V3 t{T[4], T[5], T[6]};
-  const V3 pw{g.pw[3 * i], g.pw[3 * i + 1], g.pw[3 * i + 2]};
-  const V3 pk = qrot(qconj(q), pw - t);  // T_wk^-1 * p_w
-  const Q4 qc{cam[0], cam[1], cam[2], cam[3]};
+  V3 pk;
   double R[9];
-  qmat(qc, R);
-  const V3 pc = mat_mul(R, pk) + V3{cam[4], cam[5], cam[6]};
-  double z[2];
-  Cam<MODEL>::project(pc, cam + 7, z, nullptr, nullptr);
-  *r0 = z[0] - g.pc[2 * i];
-  *r1 = z[1] - g.pc[2 * i + 1];
+  reproj_residual<MODEL>(state + 7 * static_cast<int64_t>(g.frame[i]), state + g.off_cam + kCamStateStride * c, g.pw + 3 * i, g.pc + 2 * i,
+                         r0, r1, &pk, R, nullptr, nullptr);
 }
 
 // sum of v over the CTA in a fixed order (lanes by shuffle, then warps in order); the result is valid in thread 0
@@ -88,7 +78,8 @@ __global__ void __launch_bounds__(kEvalTile) eval_batch_kernel(EvalBatchArgs a) 
       case kPoly3: eval_batch_residual<kPoly3>(g, state, c, i, &r0, &r1); break;
       default: eval_batch_residual<kKb4>(g, state, c, i, &r0, &r1); break;
     }
-    // not contracted into an FMA: the outlier test must see the square vcgpu_remove_outliers forms on the host
+    // not contracted into an FMA: |r| is sqrt(r0 * r0 + r1 * r1) with every operation rounded, as RemoveOutliers forms it
+    // (vicalibrator.h:890-893)
     s = __dadd_rn(__dmul_rn(r0, r0), __dmul_rn(r1, r1));
     if (g.res) {
       const int64_t o = g.rank ? static_cast<int64_t>(g.rank[i]) : i;

@@ -117,7 +117,7 @@ struct vcgpu_handle {
   long launches = 0, collectives = 0;
   std::unordered_map<void*, size_t> capacity;  // bytes held by each dev_alloc()ed pointer slot
   // measurement hooks
-  bool profiling = false, flush_l2 = false, materialize = false;
+  bool profiling = false, flush_l2 = false;
   bool multi_launch = false;  // force the multi-launch engine (A/B against the persistent kernel)
   bool phase_clocks = false;  // persistent kernel: per-phase %globaltimer deltas into the stage times
   cudaEvent_t st_ev[VCGPU_STAGE_COUNT][2] = {};
@@ -167,11 +167,10 @@ struct vcgpu_handle {
   // The others are constant to the solve and left out of x_norm (as Ceres drops parameter blocks no residual uses)
   std::vector<uint8_t> h_frame_used;
   uint8_t* d_frame_used = nullptr;
-  double* d_r = nullptr;          // [2][n_obs] loss-corrected residuals (vcgpu_evaluate_batch: [n_obs][2] loss-free, caller order)
-  double* d_J = nullptr;          // per camera: [2*(12+K)][n_obs_cam] column SoA, loss-corrected (two-pass path / hooks only)
+  double* d_r = nullptr;          // loss-free residuals: vcgpu_eval_reproj [2][n_obs] sorted, the evaluate calls [n_obs][2] caller order
+  double* d_J = nullptr;          // vcgpu_eval_reproj, per camera: [2*(12+K)][n_obs_cam] column SoA, loss-free
   int64_t j_doubles = 0;
-  double* d_cost_part = nullptr;  // per eval block partial costs
-  int n_cost_part = 0;
+  double* d_cost_part = nullptr;  // [n_frames] per-frame partial costs of the fused build
   double* d_Cg = nullptr;         // [n_groups][kCgStride]
   double* d_Cpart = nullptr;      // [kReduceBlocks][G*G+G]
   vc::Blocks blk[2];
@@ -193,12 +192,12 @@ struct vcgpu_handle {
   // the batch calls (vc_batch.inl): the kernel arguments of every rig of a batch this handle was handle 0 of, laid out
   // by the call
   unsigned char* d_batch_args = nullptr;
-  // vcgpu_evaluate_batch / vcgpu_remove_outliers_batch of a batch this handle was handle 0 of: the tiles' partials, the
+  // vcgpu_evaluate / vcgpu_remove_outliers, or their batch calls with this handle as handle 0: the tiles' partials, the
   // per-camera costs and tickets, and every rig's outlier marks (vc_batch.inl: run_evaluate_batch)
   unsigned char* d_eval = nullptr;
-  // vcgpu_evaluate_batch with residuals: [n_obs] each sorted observation's place in caller order, when that is not its own
+  // vcgpu_evaluate(_batch) with residuals: [n_obs] each sorted observation's place in caller order, when that is not its own
   int32_t* d_rank = nullptr;
-  // vcgpu_pose_pnp_ransac_batch of a batch this handle was handle 0 of: the packed inputs, outputs and scratch
+  // vcgpu_pose_pnp_ransac, or its batch call with this handle as handle 0: the packed inputs, outputs and scratch
   // (d_pnp), and the packed inputs and outputs in page-locked host memory (h_pnp) (vc_batch.inl: run_pnp_batch)
   unsigned char* d_pnp = nullptr;
   std::vector<unsigned char, PinnedAlloc<unsigned char>> h_pnp;

@@ -53,189 +53,78 @@ __device__ __forceinline__ double global_damp(int k, double Ckk, double scale, d
   return D2x ? D2x[nfp + k] : lm_damp(Ckk, scale, rinv);
 }
 
-// ---------------------------------------------------------------- reprojection evaluate (two-pass path + hooks)
+// ---------------------------------------------------------------- loss-free reprojection residual
+// One observation: the target point pw seen from the frame pose T (T_wk, 7 doubles) through the camera cam (q_ck 4 |
+// p_ck 3 | intrinsics), less the detected pixel z.  Also the pose chain's intermediates pk = T_wk^-1 pw and R = R(q_ck),
+// and, where not null, the projection's derivatives dzp = dz/dp_c [2][3] and dzi = dz/d intrinsics [2][K].
+template <int MODEL>
+__device__ __forceinline__ void reproj_residual(const double* T, const double* cam, const double* pw, const double* z, double* r0,
+                                                double* r1, V3* pk, double R[9], double* dzp, double* dzi) {
+  const Q4 q{T[0], T[1], T[2], T[3]};
+  const V3 t{T[4], T[5], T[6]};
+  *pk = qrot(qconj(q), V3{pw[0], pw[1], pw[2]} - t);  // T_wk^-1 * p_w
+  const Q4 qc{cam[0], cam[1], cam[2], cam[3]};
+  qmat(qc, R);
+  const V3 pc = mat_mul(R, *pk) + V3{cam[4], cam[5], cam[6]};
+  double zp[2];
+  Cam<MODEL>::project(pc, cam + 7, zp, dzp, dzi);
+  *r0 = zp[0] - z[0];
+  *r1 = zp[1] - z[1];
+}
+
+// ---------------------------------------------------------------- reprojection residuals and Jacobians (vcgpu_eval_reproj)
 struct EvalArgs {
   const double* state[2];
-  const Ctl* ctl;
-  int which;
+  const Ctl* ctl;          // the evaluated buffer is pick(ctl, 0)
   int64_t cam_off;         // offset of this camera's 17 state doubles
   const int32_t* frame;    // per observation (camera-local arrays from here on)
   const double *pw, *pc;   // AoS [n][3], [n][2]
   const double* mask;      // 6+K column mask (w_ck, p_ck, intr)
   double *r0, *r1;
   double* J;               // column c at J + c*n
-  double* cost_part;       // one per block
   int n;
-  int apply_loss;          // 1: SoftLOne corrector + robust cost; 0: raw residuals, cost 1/2|r|^2
-  double mult;
 };
 
 template <int MODEL, bool JAC>
 __global__ void __launch_bounds__(256) eval_reproj_kernel(EvalArgs a) {
   constexpr int K = Cam<MODEL>::K, NT = 12 + K;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const double* state = a.state[pick(a.ctl, a.which)];
-  const double* cam = state + a.cam_off;
-  double cost = 0.0;
-  if (i < a.n) {
-    const double* T = state + 7 * static_cast<int64_t>(a.frame[i]);
-    const Q4 q{T[0], T[1], T[2], T[3]};
-    const V3 t{T[4], T[5], T[6]};
-    const V3 pw{a.pw[3 * i], a.pw[3 * i + 1], a.pw[3 * i + 2]};
-    const V3 pk = qrot(qconj(q), pw - t);  // T_wk^-1 * p_w
-    const Q4 qc{cam[0], cam[1], cam[2], cam[3]};
-    double R[9];
-    qmat(qc, R);
-    const V3 pc = mat_mul(R, pk) + V3{cam[4], cam[5], cam[6]};
-    double z[2], dzp[6], dzi[2 * K];
-    Cam<MODEL>::project(pc, cam + 7, z, JAC ? dzp : nullptr, JAC ? dzi : nullptr);
-    double r0 = z[0] - a.pc[2 * i], r1 = z[1] - a.pc[2 * i + 1];
-    const double s = r0 * r0 + r1 * r1;
-    double sc = 1.0;
-    if (a.apply_loss) {
-      double rho0, rho1;
-      soft_l_one(s, &rho0, &rho1);
-      cost = 0.5 * rho0 * a.mult;
-      sc = sqrt(rho1);  // Ceres corrector for rho'' <= 0: scale residual and Jacobian by sqrt(rho')
-    } else {
-      cost = 0.5 * s;
-    }
-    a.r0[i] = r0 * sc;
-    a.r1[i] = r1 * sc;
-    if (JAC) {
-      const int64_t n = a.n;
+  if (i >= a.n) return;
+  const double* state = a.state[pick(a.ctl, 0)];
+  V3 pk;
+  double R[9], dzp[6], dzi[2 * K], r0, r1;
+  reproj_residual<MODEL>(state + 7 * static_cast<int64_t>(a.frame[i]), state + a.cam_off, a.pw + 3 * i, a.pc + 2 * i, &r0, &r1, &pk, R,
+                         JAC ? dzp : nullptr, JAC ? dzi : nullptr);
+  a.r0[i] = r0;
+  a.r1[i] = r1;
+  if (JAC) {
+    const int64_t n = a.n;
 #pragma unroll
-      for (int row = 0; row < 2; ++row) {
-        const double* d = dzp + 3 * row;
-        const double m0 = d[0] * R[0] + d[1] * R[3] + d[2] * R[6];
-        const double m1 = d[0] * R[1] + d[1] * R[4] + d[2] * R[7];
-        const double m2 = d[0] * R[2] + d[1] * R[5] + d[2] * R[8];
-        const double w0 = m1 * pk.z - m2 * pk.y;
-        const double w1 = m2 * pk.x - m0 * pk.z;
-        const double w2 = m0 * pk.y - m1 * pk.x;
-        double* Jc = a.J + static_cast<int64_t>(row * NT) * n + i;
-        Jc[0 * n] = -m0 * sc;
-        Jc[1 * n] = -m1 * sc;
-        Jc[2 * n] = -m2 * sc;
-        Jc[3 * n] = w0 * sc;
-        Jc[4 * n] = w1 * sc;
-        Jc[5 * n] = w2 * sc;
-        Jc[6 * n] = -w0 * sc * a.mask[0];
-        Jc[7 * n] = -w1 * sc * a.mask[1];
-        Jc[8 * n] = -w2 * sc * a.mask[2];
-        Jc[9 * n] = d[0] * sc * a.mask[3];
-        Jc[10 * n] = d[1] * sc * a.mask[4];
-        Jc[11 * n] = d[2] * sc * a.mask[5];
+    for (int row = 0; row < 2; ++row) {
+      const double* d = dzp + 3 * row;
+      const double m0 = d[0] * R[0] + d[1] * R[3] + d[2] * R[6];
+      const double m1 = d[0] * R[1] + d[1] * R[4] + d[2] * R[7];
+      const double m2 = d[0] * R[2] + d[1] * R[5] + d[2] * R[8];
+      const double w0 = m1 * pk.z - m2 * pk.y;
+      const double w1 = m2 * pk.x - m0 * pk.z;
+      const double w2 = m0 * pk.y - m1 * pk.x;
+      double* Jc = a.J + static_cast<int64_t>(row * NT) * n + i;
+      Jc[0 * n] = -m0;
+      Jc[1 * n] = -m1;
+      Jc[2 * n] = -m2;
+      Jc[3 * n] = w0;
+      Jc[4 * n] = w1;
+      Jc[5 * n] = w2;
+      Jc[6 * n] = -w0 * a.mask[0];
+      Jc[7 * n] = -w1 * a.mask[1];
+      Jc[8 * n] = -w2 * a.mask[2];
+      Jc[9 * n] = d[0] * a.mask[3];
+      Jc[10 * n] = d[1] * a.mask[4];
+      Jc[11 * n] = d[2] * a.mask[5];
 #pragma unroll
-        for (int k = 0; k < K; ++k) Jc[(12 + k) * n] = dzi[row * K + k] * sc * a.mask[6 + k];
-      }
+      for (int k = 0; k < K; ++k) Jc[(12 + k) * n] = dzi[row * K + k] * a.mask[6 + k];
     }
   }
-  __shared__ double wsum[8];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) cost += __shfl_down_sync(0xffffffffu, cost, o);
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = cost;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double s = 0.0;
-    for (int w = 0; w < (blockDim.x >> 5); ++w) s += wsum[w];
-    a.cost_part[blockIdx.x] = s;
-  }
-}
-
-// ---------------------------------------------------------------- per-frame block build (two-pass path)
-struct BuildArgs {
-  DevProblem dp;
-  const Ctl* ctl;
-  int which;
-  const int32_t *grp_start, *grp_count, *group_of;
-  const double* r;   // [2][n_obs]
-  const double* J;
-  int64_t n_obs;
-  Blocks out[2];
-  double* Cg;
-};
-
-constexpr int kBuildThreads = 128;
-constexpr int kBuildChunk = 128;  // observations staged per pass
-
-template <int FD>
-__global__ void __launch_bounds__(kBuildThreads) build_frames_kernel(BuildArgs a) {
-  extern __shared__ double smem[];
-  double* tile = smem;                              // [2*kBuildChunk][W]
-  double* smB = smem + 2 * kBuildChunk * kMaxW;     // [FD*FD]
-  double* smg = smB + FD * FD;                      // [FD]
-  const Blocks& out = a.out[pick(a.ctl, a.which)];
-  const int f = blockIdx.x, tid = threadIdx.x;
-  const int G = a.dp.G, nf = a.dp.n_frames;
-  for (int k = tid; k < FD * FD + FD; k += kBuildThreads) smB[k] = 0.0;
-  double* Ef = out.E + static_cast<int64_t>(f) * FD * G;
-  for (int k = tid; k < FD * G; k += kBuildThreads) Ef[k] = 0.0;
-  int ei[2], ej[2];
-#pragma unroll
-  for (int s = 0; s < 2; ++s) {
-    const int e = tid + s * kBuildThreads;
-    int i = static_cast<int>((sqrt(8.0 * e + 1.0) - 1.0) * 0.5);
-    while ((i + 1) * (i + 2) / 2 <= e) ++i;
-    while (i * (i + 1) / 2 > e) --i;
-    ei[s] = i;
-    ej[s] = e - i * (i + 1) / 2;
-  }
-  __syncthreads();
-  for (int c = 0; c < a.dp.n_cams; ++c) {
-    const int g = a.group_of[c * nf + f];
-    if (g < 0) continue;
-    const CamInfo& ci = a.dp.cams[c];
-    const int NT = 12 + ci.K, W = NT + 1, ntri = W * (W + 1) / 2;
-    const int start = a.grp_start[g], cnt = a.grp_count[g];
-    const int64_t nc = ci.n_obs;
-    const double* Jc = a.J + ci.joff + (start - ci.obs_start);
-    double acc[2] = {0.0, 0.0};
-    for (int ch = 0; ch < cnt; ch += kBuildChunk) {
-      const int m = min(kBuildChunk, cnt - ch);
-      for (int col = 0; col < 2 * NT; ++col) {
-        const int row = col / NT, k = col - row * NT;
-        const double* src = Jc + col * nc + ch;
-        for (int li = tid; li < m; li += kBuildThreads) tile[(2 * li + row) * W + k] = src[li];
-      }
-      for (int li = tid; li < m; li += kBuildThreads) {
-        tile[(2 * li) * W + NT] = a.r[start + ch + li];
-        tile[(2 * li + 1) * W + NT] = a.r[a.n_obs + start + ch + li];
-      }
-      __syncthreads();
-#pragma unroll
-      for (int s = 0; s < 2; ++s) {
-        if (tid + s * kBuildThreads < ntri) {
-          const int i = ei[s], j = ej[s];
-          double sum = 0.0;
-          for (int row = 0; row < 2 * m; ++row) sum += tile[row * W + i] * tile[row * W + j];
-          acc[s] += sum;
-        }
-      }
-      __syncthreads();
-    }
-    double* Cgg = a.Cg + static_cast<int64_t>(g) * kCgStride;
-#pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      if (tid + s * kBuildThreads >= ntri) continue;
-      const int i = ei[s], j = ej[s];
-      const double v = acc[s] * a.dp.visual_mult;
-      if (i < 6) {
-        smB[i * FD + j] += v;
-        if (i != j) smB[j * FD + i] += v;
-      } else if (i < W - 1) {
-        if (j < 6) Ef[j * G + ci.goff + (i - 6)] = v;
-        else Cgg[(i - 6) * (i - 5) / 2 + (j - 6)] = v;
-      } else {
-        if (j < 6) smg[j] += v;
-        else if (j < W - 1) Cgg[105 + (j - 6)] = v;
-      }
-    }
-  }
-  __syncthreads();
-  double* Bf = out.B + static_cast<int64_t>(f) * FD * FD;
-  for (int k = tid; k < FD * FD; k += kBuildThreads) Bf[k] = smB[k];
-  for (int k = tid; k < FD; k += kBuildThreads) out.gf[static_cast<int64_t>(f) * FD + k] = smg[k];
 }
 
 // ---------------------------------------------------------------- accept / reject on the device

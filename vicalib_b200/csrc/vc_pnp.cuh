@@ -22,24 +22,6 @@ constexpr int kLmIters = 12;
 constexpr int kNewtonIters = 8;
 constexpr int kWarps = 4;
 
-struct Args {
-  int n_views;
-  const int32_t* cam;      // [n_views]
-  const int64_t* start;    // [n_views] first correspondence of the view
-  const int32_t* count;    // [n_views]
-  const double* pix;       // [N][2] detected centres (pixels)
-  const double* pw;        // [N][3] target points (z = 0 plane)
-  const int32_t* model;    // [n_cams]
-  const double* intr;      // [n_cams][10]
-  int robust_its;
-  double robust_tol;       // normalised coordinates
-  double* xy;              // [N][2] scratch: unprojected points
-  unsigned char* use;      // [N] scratch: inlier mask
-  double* T_cw;            // [n_views][7]
-  double* rmse;            // [n_views]
-  int32_t* n_used;         // [n_views] 0: fewer than 4 usable points, no pose
-};
-
 __device__ inline void unproject(int model, const double* p, double u, double v, double* x, double* y) {
   const double xd = (u - p[2]) / p[0], yd = (v - p[3]) / p[1];
   const double rd = sqrt(xd * xd + yd * yd);
@@ -448,21 +430,9 @@ __device__ __forceinline__ void pose_pnp_view(int seed, int cnt, const double* p
   }
 }
 
-// vcgpu_pose_pnp_ransac: one warp per view of one handle, seeded by the view's index
-__global__ void __launch_bounds__(32 * kWarps) pose_pnp_kernel(Args a) {
-  __shared__ WarpMem wm[kWarps];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int v = blockIdx.x * kWarps + warp;
-  if (v >= a.n_views) return;
-  const int64_t s0 = a.start[v];
-  const int cam = a.cam[v];
-  pose_pnp_view(v, a.count[v], a.pix + 2 * s0, a.pw + 3 * s0, a.model[cam], a.intr + 10 * cam, a.robust_its, a.robust_tol,
-                a.xy + 2 * s0, a.use + s0, &wm[warp], lane, a.T_cw + 7 * static_cast<int64_t>(v), a.rmse + v, a.n_used + v);
-}
-
-// vcgpu_pose_pnp_ransac_batch: one warp per view of every rig of the batch, the views of a rig one after the other and
-// each view's correspondences packed behind the previous view's.  A view reads its camera from its rig's table and
-// seeds its RANSAC draws with its index within its rig, so a rig's poses are the bits its vcgpu_pose_pnp_ransac gives.
+// vcgpu_pose_pnp_ransac and its batch: one warp per view of every rig, the views of a rig one after the other and each
+// view's correspondences packed behind the previous view's.  A view reads its camera from its rig's table and seeds its
+// RANSAC draws with its index within its rig, so a rig's poses do not depend on the rest of the batch.
 struct BatchRig {
   int32_t model[kMaxCams];
   double intr[kMaxCams][10];

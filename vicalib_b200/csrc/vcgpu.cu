@@ -104,6 +104,7 @@ static int imu_mega_prepare(vcgpu_handle* h);
 
 extern "C" int vcgpu_set_profiling(vcgpu_handle* h, int profile, int flush_l2) {
   if (!h) return VCGPU_ERR_INVALID;
+  if (profile & ~(1 | 4 | 8)) return fail(h, VCGPU_ERR_INVALID, "set_profiling: unknown bit in " + std::to_string(profile) + " (bits: 1, 4, 8)");
   CUDA_TRY(h, cudaSetDevice(h->device));
   if ((profile || flush_l2) && !h->it_ev[0]) {
     for (int s = 0; s < VCGPU_STAGE_COUNT; ++s)
@@ -113,7 +114,6 @@ extern "C" int vcgpu_set_profiling(vcgpu_handle* h, int profile, int flush_l2) {
   }
   if (flush_l2 && !h->d_flush) CUDA_TRY(h, cudaMalloc(&h->d_flush, 256u << 20));
   h->profiling = (profile & 1) != 0;
-  h->materialize = (profile & 2) != 0;  // bit 1: use the two-pass path that materialises J in HBM
   h->multi_launch = (profile & 4) != 0; // bit 2: multi-launch engine even where the persistent kernel applies
   h->phase_clocks = (profile & 8) != 0; // bit 3: persistent kernel records per-phase device clocks
   h->flush_l2 = flush_l2 != 0;
@@ -432,7 +432,7 @@ static void write_mirrors(vcgpu_handle* h) {
 
 static inline int64_t perm_at(const vcgpu_handle* h, int64_t k) { return h->perm_identity ? k : h->perm[k]; }
 
-// residual / Jacobian buffers of the two-pass (materialising) path and the inspection hooks
+// residual / Jacobian buffers of vcgpu_eval_reproj
 static int ensure_rJ(vcgpu_handle* h) {
   VC_TRY(dev_alloc(h, &h->d_r, 2 * static_cast<size_t>(std::max<int64_t>(h->n_obs, 1))));
   VC_TRY(dev_alloc(h, &h->d_J, static_cast<size_t>(std::max<int64_t>(h->j_doubles, 1))));
@@ -677,10 +677,8 @@ static int prepare(vcgpu_handle* h) {
     VC_TRY(dev_alloc(h, &h->d_state[0], dp.state_size));
     VC_TRY(dev_alloc(h, &h->d_state[1], dp.state_size));
     VC_TRY(dev_alloc(h, &h->d_mask, G));
-    h->j_doubles = joff;  // residual / Jacobian buffers of the two-pass path are allocated on first use (ensure_rJ)
-    h->n_cost_part = 0;
-    for (int c = 0; c < nc; ++c) h->n_cost_part += (dp.cams[c].n_obs + 255) / 256;
-    VC_TRY(dev_alloc(h, &h->d_cost_part, std::max(h->n_cost_part, nf)));
+    h->j_doubles = joff;  // the residual / Jacobian buffers of vcgpu_eval_reproj are allocated on first use (ensure_rJ)
+    VC_TRY(dev_alloc(h, &h->d_cost_part, nf));
     VC_TRY(dev_alloc(h, &h->d_Cg, static_cast<size_t>(h->n_groups) * kCgStride));
     CUDA_TRY(h, cudaMemsetAsync(h->d_Cg, 0, std::max<size_t>(1, static_cast<size_t>(h->n_groups) * kCgStride) * sizeof(double), h->stream));
     const size_t NS = static_cast<size_t>(G) * G + G;
@@ -797,68 +795,60 @@ extern "C" int vcgpu_cost(vcgpu_handle* h, double* cost) {
   return VCGPU_OK;
 }
 
+// Problem::Evaluate of one camera's or every camera's residual blocks, without the loss (vicalibrator.h:873-887, 958-966):
+// run_evaluate_batch of this handle alone, then the asked camera's share of its per-camera results.  Frame shards
+// evaluate their own observations.
 extern "C" int vcgpu_evaluate(vcgpu_handle* h, int cam, double* cost, double* residuals, int64_t* n_blocks) {
   if (!h) return VCGPU_ERR_INVALID;
-  VC_TRY(prepare(h));
-  const DevProblem& dp = h->dp;
-  if (cam >= dp.n_cams) return fail(h, VCGPU_ERR_INVALID, "evaluate: camera index out of range");
-  VC_TRY(ctl_reset(h, 0, 0));
-  VC_TRY(eval_reproj(h, 0, false, false, h->d_mask));
-  const int64_t n = h->n_obs;
-  std::vector<double> r(2 * std::max<int64_t>(n, 1));
-  CUDA_TRY(h, cudaMemcpyAsync(r.data(), h->d_r, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  h->blocks_valid = false;
-  // caller order: gather the sorted residuals back through perm
-  const int c0 = cam < 0 ? 0 : cam, c1 = cam < 0 ? dp.n_cams : cam + 1;
-  std::vector<std::pair<int64_t, int64_t>> idx;  // (caller index, sorted index)
-  for (int c = c0; c < c1; ++c)
-    for (int64_t k = dp.cams[c].obs_start; k < dp.cams[c].obs_start + dp.cams[c].n_obs; ++k) idx.emplace_back(perm_at(h, k), k);
-  std::sort(idx.begin(), idx.end());
+  if (cam >= h->n_cams) return fail(h, VCGPU_ERR_INVALID, "evaluate: camera index out of range");
+  double cam_cost[kMaxCams];
+  int64_t cam_blocks[kMaxCams];
+  std::vector<double> all;  // one camera's residuals are picked from every camera's
+  double* res = residuals;
+  if (residuals && cam >= 0) {
+    all.resize(2 * static_cast<size_t>(h->n_obs_all));
+    res = all.data();
+  }
+  double* cp = cam_cost;
+  int64_t* bp = cam_blocks;
+  VC_TRY(run_evaluate_batch(&h, 1, EvalBatchOut{&cp, &bp, &res, nullptr, 0.0, nullptr}, "vcgpu_evaluate",
+                            [](const vcgpu_handle*, int) -> const char* { return nullptr; }));
+  const int c0 = cam < 0 ? 0 : cam, c1 = cam < 0 ? h->dp.n_cams : cam + 1;
   double s = 0;
   int64_t o = 0;
-  for (const auto& pr : idx) {
-    const double a = r[pr.second], b = r[n + pr.second];
-    s += a * a + b * b;
-    if (residuals) { residuals[2 * o] = a; residuals[2 * o + 1] = b; }
-    ++o;
-  }
-  if (cost) *cost = 0.5 * s;
+  for (int c = c0; c < c1; ++c) { s += cam_cost[c]; o += cam_blocks[c]; }
+  if (residuals && cam >= 0)  // the camera's active observations in caller order
+    for (int64_t k = 0, a = 0, m = 0; k < h->n_obs_all; ++k) {
+      if (!h->h_active[k]) continue;
+      if (h->h_obs_cam[k] == cam) { residuals[2 * m] = all[2 * a]; residuals[2 * m + 1] = all[2 * a + 1]; ++m; }
+      ++a;
+    }
+  if (cost) *cost = s;
   if (n_blocks) *n_blocks = o;
   return VCGPU_OK;
 }
 
+// RemoveOutliers (vicalibrator.h:859-916): run_evaluate_batch of this handle alone
 extern "C" int vcgpu_remove_outliers(vcgpu_handle* h, const double* rmse, double threshold, int64_t* n_removed) {
   if (!h || !rmse) return VCGPU_ERR_INVALID;
-  VC_TRY(prepare(h));
-  const DevProblem& dp = h->dp;
-  VC_TRY(ctl_reset(h, 0, 0));
-  VC_TRY(eval_reproj(h, 0, false, false, h->d_mask));
-  const int64_t n = h->n_obs;
-  std::vector<double> r(2 * std::max<int64_t>(n, 1));
-  CUDA_TRY(h, cudaMemcpyAsync(r.data(), h->d_r, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  int64_t removed = 0;
-  for (int c = 0; c < dp.n_cams; ++c)
-    for (int64_t k = dp.cams[c].obs_start; k < dp.cams[c].obs_start + dp.cams[c].n_obs; ++k) {
-      const double err = std::sqrt(r[k] * r[k] + r[n + k] * r[n + k]);
-      if (err > threshold * rmse[c]) { h->h_active[perm_at(h, k)] = 0; ++removed; }  // vicalibrator.h:890-893
-    }
-  if (removed) h->dirty = true;
-  if (n_removed) *n_removed = removed;
-  return VCGPU_OK;
+  return run_evaluate_batch(&h, 1, EvalBatchOut{nullptr, nullptr, nullptr, &rmse, threshold, n_removed}, "vcgpu_remove_outliers",
+                            [](const vcgpu_handle*, int) -> const char* { return nullptr; });
 }
+// the batch calls refuse frame shards
+static const char* eval_batch_refusal(const vcgpu_handle* h) { return h->nranks > 1 ? "frame shards (use the per-handle call)" : nullptr; }
 extern "C" int vcgpu_evaluate_batch(vcgpu_handle* const* handles, int n, double* const* cam_cost, int64_t* const* cam_blocks,
                                     double* const* residuals_or_null) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!cam_cost) return batch_refuse(handles, n, 0, "null cam_cost array", "vcgpu_evaluate_batch");
-  return run_evaluate_batch(handles, n, EvalBatchOut{cam_cost, cam_blocks, residuals_or_null, nullptr, 0.0, nullptr});
+  return run_evaluate_batch(handles, n, EvalBatchOut{cam_cost, cam_blocks, residuals_or_null, nullptr, 0.0, nullptr}, "vcgpu_evaluate_batch",
+                            [&](const vcgpu_handle* h, int i) { return cam_cost[i] ? eval_batch_refusal(h) : "null cam_cost pointer"; });
 }
 extern "C" int vcgpu_remove_outliers_batch(vcgpu_handle* const* handles, int n, const double* const* rmse, double threshold,
                                            int64_t* n_removed) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!rmse) return batch_refuse(handles, n, 0, "null rmse array", "vcgpu_remove_outliers_batch");
-  return run_evaluate_batch(handles, n, EvalBatchOut{nullptr, nullptr, nullptr, rmse, threshold, n_removed});
+  return run_evaluate_batch(handles, n, EvalBatchOut{nullptr, nullptr, nullptr, rmse, threshold, n_removed}, "vcgpu_remove_outliers_batch",
+                            [&](const vcgpu_handle* h, int i) { return rmse[i] ? eval_batch_refusal(h) : "null rmse pointer"; });
 }
 extern "C" int vcgpu_get_obs_active(vcgpu_handle* h, uint8_t* active) {
   if (!h || !active) return VCGPU_ERR_INVALID;
@@ -911,7 +901,7 @@ extern "C" int vcgpu_eval_reproj(vcgpu_handle* h, double* r_out, double* J_out) 
   std::vector<double> hones(dp.G, 1.0);
   CUDA_TRY(h, cudaMemcpy(ones, hones.data(), dp.G * sizeof(double), cudaMemcpyHostToDevice));
   VC_TRY(ctl_reset(h, 0, 0));
-  VC_TRY(eval_reproj(h, 0, J_out != nullptr, false, ones));
+  VC_TRY(eval_reproj(h, J_out != nullptr, ones));
   std::vector<double> r(2 * std::max<int64_t>(n, 1));
   CUDA_TRY(h, cudaMemcpyAsync(r.data(), h->d_r, 2 * n * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->stream));
@@ -968,7 +958,7 @@ extern "C" int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const dou
   CUDA_TRY(h, cudaMemcpyAsync(h->d_scale, scale, np * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemcpyAsync(h->d_scale + np, D2, np * sizeof(double), cudaMemcpyHostToDevice, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
-  VC_TRY(solve_and_update(h, h->d_scale + np, false));
+  VC_TRY(solve_and_update(h, h->d_scale + np));
   VC_TRY(read_scalars(h));
   if (h->h_scalars[kScNotPD] > 0) return fail(h, VCGPU_ERR_NUMERIC, "arrow system is not positive definite");
   CUDA_TRY(h, cudaMemcpy(x, h->d_delta, np * sizeof(double), cudaMemcpyDeviceToHost));
@@ -1007,7 +997,7 @@ extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
     col[j] = -1.0;  // the solver forms the right-hand side -g_c * scale and returns the scaled solution
     CUDA_TRY(h, cudaMemcpyAsync(b.gc, col.data(), G * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
-    rc = solve_and_update(h, h->d_scale + np, false);
+    rc = solve_and_update(h, h->d_scale + np);
     if (rc != VCGPU_OK) break;
     CUDA_TRY(h, cudaMemcpyAsync(x.data(), h->d_delta, np * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     rc = read_scalars(h);
@@ -1098,73 +1088,21 @@ extern "C" int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, in
 }
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp
-// per view (vc_pnp.cuh).  Cameras (model, intrinsics) are the ones given to vcgpu_set_cameras.
+// per view (vc_pnp.cuh): run_pnp_batch of this handle alone.  Cameras (model, intrinsics) are the ones given to
+// vcgpu_set_cameras.
 extern "C" int vcgpu_pose_pnp_ransac(vcgpu_handle* h, int n_views, const int32_t* cam_id, const int64_t* start, const int32_t* count,
                                      const double* pix, const double* pw, int robust_its, double robust_tol, double* T_cw,
                                      double* rmse, int32_t* n_used) {
-  if (!h || n_views < 0 || (n_views > 0 && (!cam_id || !start || !count || !pix || !pw || !T_cw)))
-    return h ? fail(h, VCGPU_ERR_INVALID, "pose_pnp_ransac: bad arguments") : VCGPU_ERR_INVALID;
-  if (h->n_cams <= 0) return fail(h, VCGPU_ERR_INVALID, "pose_pnp_ransac: cameras must be set first");
-  if (n_views == 0) return VCGPU_OK;
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  int64_t N = 0;
-  for (int v = 0; v < n_views; ++v) {
-    if (cam_id[v] < 0 || cam_id[v] >= h->n_cams || start[v] < 0 || count[v] < 0)
-      return fail(h, VCGPU_ERR_INVALID, "pose_pnp_ransac: bad view description");
-    N = std::max<int64_t>(N, start[v] + count[v]);
-  }
-  int32_t *d_cam = nullptr, *d_count = nullptr, *d_model = nullptr, *d_used = nullptr;
-  int64_t* d_start = nullptr;
-  double *d_pix = nullptr, *d_pw = nullptr, *d_intr = nullptr, *d_xy = nullptr, *d_T = nullptr, *d_rmse = nullptr;
-  unsigned char* d_use = nullptr;
-  auto release = [&] {
-    cudaFree(d_cam); cudaFree(d_count); cudaFree(d_model); cudaFree(d_used); cudaFree(d_start); cudaFree(d_pix); cudaFree(d_pw);
-    cudaFree(d_intr); cudaFree(d_xy); cudaFree(d_T); cudaFree(d_rmse); cudaFree(d_use);
-  };
-  const size_t nv = static_cast<size_t>(n_views), np_ = static_cast<size_t>(std::max<int64_t>(N, 1));
-  cudaError_t e = cudaSuccess;
-  auto up = [&](void** d, const void* src, size_t bytes) {
-    if (e != cudaSuccess) return;
-    e = cudaMalloc(d, std::max<size_t>(bytes, 8));
-    if (e == cudaSuccess && src) e = cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, h->stream);
-  };
-  up(reinterpret_cast<void**>(&d_cam), cam_id, nv * sizeof(int32_t));
-  up(reinterpret_cast<void**>(&d_start), start, nv * sizeof(int64_t));
-  up(reinterpret_cast<void**>(&d_count), count, nv * sizeof(int32_t));
-  up(reinterpret_cast<void**>(&d_pix), pix, 2 * np_ * sizeof(double));
-  up(reinterpret_cast<void**>(&d_pw), pw, 3 * np_ * sizeof(double));
-  up(reinterpret_cast<void**>(&d_model), h->h_model.data(), h->n_cams * sizeof(int32_t));
-  up(reinterpret_cast<void**>(&d_intr), h->h_intr.data(), 10 * h->n_cams * sizeof(double));
-  up(reinterpret_cast<void**>(&d_xy), nullptr, 2 * np_ * sizeof(double));
-  up(reinterpret_cast<void**>(&d_use), nullptr, np_);
-  up(reinterpret_cast<void**>(&d_T), nullptr, 7 * nv * sizeof(double));
-  up(reinterpret_cast<void**>(&d_rmse), nullptr, nv * sizeof(double));
-  up(reinterpret_cast<void**>(&d_used), nullptr, nv * sizeof(int32_t));
-  if (e != cudaSuccess) { release(); h->err = std::string("pose_pnp_ransac: ") + cudaGetErrorString(e); return VCGPU_ERR_CUDA; }
-  vc::pnp::Args a;
-  a.n_views = n_views; a.cam = d_cam; a.start = d_start; a.count = d_count; a.pix = d_pix; a.pw = d_pw; a.model = d_model; a.intr = d_intr;
-  a.robust_its = robust_its; a.robust_tol = robust_tol; a.xy = d_xy; a.use = d_use; a.T_cw = d_T; a.rmse = d_rmse; a.n_used = d_used;
-  vc::pnp::pose_pnp_kernel<<<(n_views + vc::pnp::kWarps - 1) / vc::pnp::kWarps, 32 * vc::pnp::kWarps, 0, h->stream>>>(a);
-  ++h->launches;
-  std::vector<double> hr(nv);
-  std::vector<int32_t> hu(nv);
-  e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(T_cw, d_T, 7 * nv * sizeof(double), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(hr.data(), d_rmse, nv * sizeof(double), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaMemcpyAsync(hu.data(), d_used, nv * sizeof(int32_t), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-  release();
-  if (e != cudaSuccess) { h->err = std::string("pose_pnp_ransac: ") + cudaGetErrorString(e); return VCGPU_ERR_CUDA; }
-  if (rmse) std::copy(hr.begin(), hr.end(), rmse);
-  if (n_used) std::copy(hu.begin(), hu.end(), n_used);
-  return VCGPU_OK;
+  if (!h) return VCGPU_ERR_INVALID;
+  const vcgpu_pnp_views views{n_views, cam_id, start, count, pix, pw, T_cw, rmse, n_used};
+  return run_pnp_batch(&h, 1, &views, robust_its, robust_tol, "vcgpu_pose_pnp_ransac");
 }
 
 extern "C" int vcgpu_pose_pnp_ransac_batch(vcgpu_handle* const* handles, int n, const vcgpu_pnp_views* views, int robust_its,
                                            double robust_tol) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!views) return batch_refuse(handles, n, 0, "null views array", "vcgpu_pose_pnp_ransac_batch");
-  return run_pnp_batch(handles, n, views, robust_its, robust_tol);
+  return run_pnp_batch(handles, n, views, robust_its, robust_tol, "vcgpu_pose_pnp_ransac_batch");
 }
 
 extern "C" int vcgpu_eval_imu(vcgpu_handle* h, double* r, double* J) {
