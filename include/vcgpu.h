@@ -280,9 +280,17 @@ int vcgpu_pose_pnp_ransac_batch(vcgpu_handle* const* handles, int n, const vcgpu
 
 /* GetSolutionCovariance (vicalibrator.h:802-857; compiled out upstream behind COMPUTE_VICALIB_COVARIANCE): the
  * [globals, globals] block of (J^T J)^-1 at the current state, tangent space, G x G row-major with G = vcgpu_num_globals:
- * per camera (w_ck 3 | p_ck 3 | intrinsics K), then with inertial terms (g 2 | b 6 | sf 6 | ts 1).  Rows / columns of
- * constant or unused parameter blocks (the blocks of a camera no active observation sees) are zero (ceres::Covariance
- * convention). */
+ * per camera (w_ck 3 | p_ck 3 | intrinsics K), then with inertial terms (g 2 | b 6 | sf 6 | ts 1).  Computed on the
+ * Jacobi-scaled undamped system (constant globals on a unit diagonal) by one elimination of the frames, as the solve
+ * runs it, and one dense inversion of the system that elimination leaves: [globals] (vision) or [globals | top nodes]
+ * (inertial), whose globals' block this is; unscaled on the host.  The matrix is exactly symmetric (one triangle is
+ * computed and mirrored).  Rows / columns of constant or unused parameter blocks (the blocks of a camera no active
+ * observation sees) are exactly 0.0 (ceres::Covariance convention).  Options play no part.  Nothing on the handle
+ * changes: state, IMU weights and what a later vcgpu_solve or batch solve computes stay as they were.  Frame shards are
+ * accepted: every rank calls with its shard, and each gets the same matrix.
+ * VCGPU_ERR_NUMERIC: J^T J is not positive definite at the current state; cov is not written.
+ * Device memory, kept on the handle and shared with vcgpu_get_frame_covariance: vision G^2 doubles; inertial N^2,
+ * N = G + 9 t, t the nodes of the chain's top level (at most 4; on frame shards, the number of ranks). */
 int vcgpu_get_covariance(vcgpu_handle* h, double* cov);
 /* vcgpu_get_covariance of n handles in one call; vision and inertial rigs may be mixed.  cov[i] (G_i x G_i row-major,
  * G_i = vcgpu_num_globals) gets what vcgpu_get_covariance(handles[i]) returns at the handle's current state, equal to

@@ -1,7 +1,8 @@
 """Worker for the multi-GPU parity test: run under torchrun with N ranks (one GPU each).
 
 Every rank solves its frame shard of the same seeded problem jointly (NCCL all-reduce inside
-libvcgpu); rank 0 additionally solves the whole problem on its own GPU and compares.
+libvcgpu), then reads the covariance of the globals on its shard; rank 0 additionally solves the whole problem on its
+own GPU and compares both.
 """
 import os
 import sys
@@ -13,6 +14,7 @@ sys.path.insert(0, ROOT)
 
 import torch.distributed as dist  # noqa: E402
 
+from test_gpu_covariance_batch import BAR, _corr_err  # noqa: E402
 from vicalib_b200 import synth  # noqa: E402
 from vicalib_b200.capi import Calibrator  # noqa: E402
 
@@ -37,11 +39,13 @@ def run_case(rank, world, local, inertial, strategy=0):
     g.set_options(function_tol=1e-14, max_iters=iters, strategy=strategy)
     s = g.solve()
     st = g.state()
+    cov = g.covariance()  # every rank, on its shard
     n_own = synth.shard_frames(p.n_frames, rank, world)
     n_own = n_own[1] - n_own[0]
     out = [None] * world
     dist.all_gather_object(out, dict(cost=s["final_cost"], iters=s["iterations"], intr=st["intr"], p_ck=st["p_ck"],
-                                     q_ck=st["q_ck"], T=st["T_wp"][:n_own], v=st["v_w"][:n_own], b=st["b"], ts=st["ts"]))
+                                     q_ck=st["q_ck"], T=st["T_wp"][:n_own], v=st["v_w"][:n_own], b=st["b"], ts=st["ts"],
+                                     cov=cov))
     ok = True
     if rank == 0:
         ref = Calibrator(device=local)
@@ -58,6 +62,8 @@ def run_case(rank, world, local, inertial, strategy=0):
             "intr": np.abs(out[0]["intr"] - sref["intr"]).max() <= 1e-6 * np.abs(sref["intr"]).max(),
             "p_ck": np.abs(out[0]["p_ck"] - sref["p_ck"]).max() <= 1e-8,
             "poses": np.abs(T - sref["T_wp"]).max() <= 1e-8,
+            "cov": _corr_err(out[0]["cov"], ref.covariance()) <= BAR[inertial],
+            "cov_ranks_agree": all(np.array_equal(o["cov"], out[0]["cov"]) for o in out),
         }
         if inertial:
             V = np.concatenate([o["v"] for o in out])

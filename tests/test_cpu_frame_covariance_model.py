@@ -99,7 +99,7 @@ def chain_frame_cov(B, U, E, C, sizes):
                 nxt["U"][j + 1] = -Sch[:fd, fd:2 * fd]
             S -= Sch[2 * fd:, 2 * fd:]
         levels.append(nxt)
-    # ---- the dense phase: the inverse of [globals | top nodes] (dense_solve_kernel, mode 3)
+    # ---- the dense phase: the inverse of [globals | top nodes] (dense_solve_kernel's inversion)
     top, nt = levels[-1], sizes[-1]
     N = G + nt * fd
     D = np.zeros((N, N))

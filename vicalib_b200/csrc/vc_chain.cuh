@@ -62,7 +62,7 @@ __host__ inline size_t chain_eliminate_smem_bytes(int G, int c) {
   const size_t g = static_cast<size_t>(G), w = 2 * FD + g + 1;
   return (g * g + g + 3 * FD * FD + FD * g + FD + static_cast<size_t>(c - 1) * FD * (FD + w)) * sizeof(double);
 }
-// dynamic shared memory of dense_solve_kernel when it factors (modes 0 and 2): S [N^2] | rhs [N]
+// dynamic shared memory of dense_solve_kernel when it factors (src 0 and 2): S [N^2] | rhs [N]
 __host__ inline size_t chain_dense_smem_bytes(int N) { return (static_cast<size_t>(N) * N + N) * sizeof(double); }
 
 struct ElimArgs {
@@ -343,16 +343,17 @@ struct DenseArgs {
   int n_slots;         // frame blocks in the dense system (single GPU: top.n; sharded: one per rank)
   int slot_of[4];      // dense slot of each local top node
   int add_globals;     // 1: this rank contributes C + D and -g_c (exactly one rank does)
-  int mode;            // 0: assemble + solve; 1: assemble the local partial into buf only; 2: solve the (summed) buf;
-                       // 3: assemble + invert: the whole inverse into buf [N*N], the top nodes' blocks of it into sig
+  int src;             // the system: 0 assembled here; 1 this rank's partial assembled into buf, and nothing else done;
+                       // 2 loaded from buf (the ranks' partials summed)
   double* buf;         // [N*N + N], N = G + n_slots*FD
-  SigmaLevel sig;      // mode 3
+  double* inv;         // null: solve into delta; else invert: the whole inverse into inv [N*N] ...
+  SigmaLevel sig;      // ... and, where sig.kk is set, the top nodes' blocks of it into sig
 };
 template <int FD>
 __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
   extern __shared__ double sm[];
   const int G = a.dp.G, nt = a.top.n, N = G + a.n_slots * FD, tid = threadIdx.x;
-  double* S = a.mode == 1 ? a.buf : sm;              // [N*N]
+  double* S = a.src == 1 ? a.buf : sm;               // [N*N]
   double* rhs = S + N * N;
   __shared__ int bad;
   if (a.ctl->done) return;
@@ -361,7 +362,7 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
   if (tid == 0) bad = 0;
   const int64_t nfp = static_cast<int64_t>(a.dp.n_frames) * a.dp.fd;
   const double* sc = a.scale + nfp;
-  if (a.mode == 2) {
+  if (a.src == 2) {
     for (int e = tid; e < N * N + N; e += 256) S[e] = a.buf[e];
   } else {
     for (int e = tid; e < N * N + N; e += 256) S[e] = 0.0;
@@ -403,7 +404,7 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
         rhs[o + e] = -(a.top.g[static_cast<int64_t>(t) * FD + e] + (add ? a.top.addg[static_cast<int64_t>(t) * FD + e] : 0.0));
     }
   }
-  if (a.mode == 1) return;
+  if (a.src == 1) return;
   __syncthreads();
   for (int j = 0; j < N; ++j) {
     if (tid == 0) {
@@ -422,9 +423,9 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
     }
     __syncthreads();
   }
-  if (a.mode == 3) {
+  if (a.inv) {
     // N unit right-hand sides through the factor, one column per thread: L y = e_j (y is zero above row j), L^T x = y
-    double* X = a.buf;
+    double* X = a.inv;
     for (int j = tid; j < N; j += 256) {
       for (int i = j; i < N; ++i) {
         double t = i == j ? 1.0 : 0.0;
@@ -439,6 +440,7 @@ __global__ void __launch_bounds__(256) dense_solve_kernel(DenseArgs a) {
     }
     __syncthreads();
     if (bad && tid == 0) a.scalars[kScNotPD] = 1.0;
+    if (!a.sig.kk) return;
     for (int e = tid; e < nt * FD * FD; e += 256) {
       const int t = e / (FD * FD), r = (e / FD) % FD, q = e % FD, o = G + a.slot_of[t] * FD;
       a.sig.kk[e] = X[static_cast<int64_t>(o + r) * N + o + q];

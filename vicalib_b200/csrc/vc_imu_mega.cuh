@@ -1423,7 +1423,7 @@ __host__ __device__ inline size_t chain_frame_cov_smem_bytes(int G) {
 }
 // A batch of inertial rigs, one thread-block cluster each: cluster k writes the frame covariance of args[k].  The
 // elimination and the dense factorisation of chain_solve; CTA 0's warps solve the N unit right-hand sides (the whole
-// inverse of [globals | top nodes], as dense_solve_kernel's mode 3 gives it) and leave the top nodes' blocks; then the
+// inverse of [globals | top nodes], as dense_solve_kernel's inversion gives it) and leave the top nodes' blocks; then the
 // levels top-down, a cluster barrier between two, their chunks spread over the CTAs (chain_selinv_chunk); then level 0
 // unscaled.
 __global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {

@@ -965,81 +965,41 @@ extern "C" int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const dou
   return VCGPU_OK;
 }
 
-// Solution covariance of the global parameters (GetSolutionCovariance, vicalibrator.h:802-857, compiled out upstream
-// behind COMPUTE_VICALIB_COVARIANCE because ceres::Covariance on the full problem "can run out of memory"): the
-// [globals, globals] block of (J^T J)^-1 at the current state, i.e. the inverse of the Schur complement of the frames —
-// one solve of the (undamped, unscaled) arrow system per global column on the device, through the same frame
-// elimination the trust-region step uses.  Tangent space: per camera (w_ck 3 | p_ck 3 | intrinsics K), then with
-// inertial terms (g 2 | b 6 | sf 6 | ts 1); rows / columns of constant or unused parameters (fill_mask) are zero like
-// ceres::Covariance's.
-extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
-  if (!h || !cov) return VCGPU_ERR_INVALID;
-  VC_TRY(prepare(h));
-  std::vector<double> mask, D2;
-  VC_TRY(cov_prelude(h, false, &D2));
-  fill_mask(h, &mask);
-  const DevProblem& dp = h->dp;
-  const int G = dp.G;
-  const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + G;
-  const Blocks& b = h->blk[h->cur];
-  // the gradient, which the unit right-hand sides replace, is put back after the solves
-  std::vector<double> gf0(nfp), gc0(G), sc(G), col(G, 0.0), x(np);
-  CUDA_TRY(h, cudaMemcpyAsync(gf0.data(), b.gf, nfp * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(gc0.data(), b.gc, G * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(sc.data(), h->d_scale + nfp, G * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(b.gf, 0, nfp * sizeof(double), h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  std::fill(cov, cov + static_cast<size_t>(G) * G, 0.0);
-  int rc = VCGPU_OK;
-  for (int j = 0; j < G && rc == VCGPU_OK; ++j) {
-    if (mask[j] == 0.0) continue;
-    std::fill(col.begin(), col.end(), 0.0);
-    col[j] = -1.0;  // the solver forms the right-hand side -g_c * scale and returns the scaled solution
-    CUDA_TRY(h, cudaMemcpyAsync(b.gc, col.data(), G * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
-    rc = solve_and_update(h, h->d_scale + np);
-    if (rc != VCGPU_OK) break;
-    CUDA_TRY(h, cudaMemcpyAsync(x.data(), h->d_delta, np * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    rc = read_scalars(h);
-    if (rc == VCGPU_OK && h->h_scalars[kScNotPD] > 0) rc = fail(h, VCGPU_ERR_NUMERIC, "covariance: J^T J is singular at the current state");
-    for (int i = 0; i < G; ++i) cov[static_cast<size_t>(i) * G + j] = mask[i] != 0.0 ? sc[i] * x[nfp + i] : 0.0;
-  }
-  // put the gradient back; the Jacobi scale is recomputed by the next solve
-  CUDA_TRY(h, cudaMemcpyAsync(b.gf, gf0.data(), nfp * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaMemcpyAsync(b.gc, gc0.data(), G * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  h->blocks_valid = false;
-  return rc;
-}
-
-// The frames' blocks of vcgpu_get_frame_covariance (vc_frame_cov.cuh) into w.out [nf][fd*fd] on the device.
-// Vision: the solve's frame elimination and Schur sum, the inverse of the reduced system, then one warp per frame.
-static int frame_cov_vision(vcgpu_handle* h, const double* D2x, const FrameCovSpace& w) {
+// The frames' elimination and the inverse of the system it leaves into w.inv [N*N]: vision: the solve's frame
+// elimination and Schur sum (summed over frame shards), then the inverse of the reduced system [globals].  frames: then
+// the blocks (vc_frame_cov.cuh) into w.out [nf][fd*fd], one warp per frame.
+static int cov_vision(vcgpu_handle* h, const double* D2x, bool frames, const CovSpace& w) {
   const DevProblem& dp = h->dp;
   const int G = dp.G;
   VC_TRY(vision_frame_solve(h, D2x));
+  VC_TRY(all_reduce(h, h->d_Ssum, static_cast<size_t>(G) * G + G));
   DenseArgs da{};
   da.dp = dp; da.bs[0] = h->blk[0]; da.bs[1] = h->blk[1]; da.ctl = h->d_ctl; da.scale = h->d_scale; da.D2x = D2x;
-  da.Ssum = h->d_Ssum; da.delta = h->d_delta; da.scalars = h->d_scalars; da.add_globals = 1; da.mode = 3; da.buf = w.inv;
+  da.Ssum = h->d_Ssum; da.delta = h->d_delta; da.scalars = h->d_scalars; da.add_globals = 1; da.src = 0; da.inv = w.inv;
   VC_TRY(kernel_smem_optin(h));
   dense_solve_kernel<6><<<1, 256, vc::chain_dense_smem_bytes(G), h->stream>>>(da);
-  vc::FrameCovArgs fa;
-  fa.dp = dp; fa.b[0] = h->blk[0]; fa.b[1] = h->blk[1]; fa.ctl = h->d_ctl; fa.scale = h->d_scale; fa.D2x = D2x; fa.X = h->d_X;
-  fa.Sgg = w.inv; fa.frame_used = h->d_frame_used; fa.out = w.out;
-  vc::frame_cov_vision_kernel<6><<<(dp.n_frames + vc::kFrameCovWarps - 1) / vc::kFrameCovWarps, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
-  h->launches += 2;
+  ++h->launches;
+  if (frames) {
+    vc::FrameCovArgs fa;
+    fa.dp = dp; fa.b[0] = h->blk[0]; fa.b[1] = h->blk[1]; fa.ctl = h->d_ctl; fa.scale = h->d_scale; fa.D2x = D2x; fa.X = h->d_X;
+    fa.Sgg = w.inv; fa.frame_used = h->d_frame_used; fa.out = w.out;
+    vc::frame_cov_vision_kernel<6><<<(dp.n_frames + vc::kFrameCovWarps - 1) / vc::kFrameCovWarps, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
+    ++h->launches;
+  }
   CUDA_TRY(h, cudaGetLastError());
   return VCGPU_OK;
 }
-// Inertial: the chain elimination, the inverse of [globals | top nodes], then the levels top-down (chain_selinv_kernel);
-// rows and columns from `live` on are 0.
-static int frame_cov_inertial(vcgpu_handle* h, const double* D2x, int live, const FrameCovSpace& w) {
+// Inertial: the chain elimination, the inverse of [globals | top nodes] (on frame shards: of the ranks' summed
+// partials).  frames: with the top nodes' blocks, then the levels top-down (chain_selinv_kernel); rows and columns
+// from `live` on are 0.
+static int cov_inertial(vcgpu_handle* h, const double* D2x, bool frames, int live, const CovSpace& w) {
   constexpr int FD = 9;
   vc::ImuDev* d = imu_dev(h);
   const DevProblem& dp = h->dp;
   const int G = dp.G, nl = static_cast<int>(d->levels.size());
   VC_TRY(imu_chain_eliminate(h, D2x));
-  VC_TRY(imu_chain_dense(h, D2x, w.inv, &w.sig.back()));
+  VC_TRY(imu_chain_dense(h, D2x, w.inv, frames ? &w.sig.back() : nullptr));
+  if (!frames) return VCGPU_OK;
   const size_t sm = vc::chain_selinv_smem_bytes<FD>(G, kChainC);
   if (nl > 1 && sm > h->selinv_smem_max)
     return fail(h, VCGPU_ERR_INVALID, "frame covariance: G = " + std::to_string(G) + " needs " + std::to_string(sm) +
@@ -1058,28 +1018,64 @@ static int frame_cov_inertial(vcgpu_handle* h, const double* D2x, int live, cons
   return VCGPU_OK;
 }
 
+// vcgpu_get_covariance (frames false) and vcgpu_get_frame_covariance (frames true) of one handle, the per-handle
+// counterpart of run_cov_batch: cov_prelude, the frames' elimination and one inversion of the system it leaves; the
+// globals' block of that inverse (frames false) or the frames' blocks from it (frames true).  Writes no state buffer.
+static int run_cov(vcgpu_handle* h, double* cov, bool frames) {
+  VC_TRY(prepare(h));
+  std::vector<double> D2;
+  int live = 0;
+  VC_TRY(cov_prelude(h, frames, &D2, &live));
+  const DevProblem& dp = h->dp;
+  const size_t G = dp.G, nfp = static_cast<size_t>(dp.n_frames) * dp.fd;
+  const double* D2x = h->d_scale + nfp + G;
+  CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
+  CovSpace w;
+  int rc = cov_space(h, frames, &w);
+  if (rc == VCGPU_OK) rc = dp.inertial ? cov_inertial(h, D2x, frames, live, w) : cov_vision(h, D2x, frames, w);
+  h->blocks_valid = false;  // the Jacobi scale is the next solve's to set
+  if (rc != VCGPU_OK) return rc;
+  std::vector<double> inv(frames ? 0 : G * G), sc(frames ? 0 : G);
+  if (!frames) {  // Σ_gg: the globals' block of the inverse, row stride N, and the globals' Jacobi scale
+    CUDA_TRY(h, cudaMemcpy2DAsync(inv.data(), G * sizeof(double), w.inv, w.N * sizeof(double), G * sizeof(double), G,
+                                  cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(sc.data(), h->d_scale + nfp, G * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+  }
+  VC_TRY(read_scalars(h));
+  if (h->h_scalars[kScNotPD] > 0)
+    return fail(h, VCGPU_ERR_NUMERIC, std::string(frames ? "frame covariance" : "covariance") + ": J^T J is singular at the current state");
+  if (frames) {
+    CUDA_TRY(h, cudaMemcpy(cov, w.out, nfp * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
+    return VCGPU_OK;
+  }
+  // as cov_store_column: the lower triangle unscaled by s_i s_j and mirrored; constant or unused globals exactly 0
+  std::vector<double> mask;
+  fill_mask(h, &mask);
+  for (size_t j = 0; j < G; ++j)
+    for (size_t i = j; i < G; ++i)
+      cov[i * G + j] = cov[j * G + i] = mask[j] != 0.0 && mask[i] != 0.0 ? sc[i] * sc[j] * inv[i * G + j] : 0.0;
+  return VCGPU_OK;
+}
+
+// Solution covariance of the global parameters (GetSolutionCovariance, vicalibrator.h:802-857, compiled out upstream
+// behind COMPUTE_VICALIB_COVARIANCE because ceres::Covariance on the full problem "can run out of memory"): the
+// [globals, globals] block of (J^T J)^-1 at the current state, i.e. the inverse of the Schur complement of the frames.
+// run_cov eliminates the frames once, as the trust-region step does, and inverts the system left, [globals] (vision)
+// or [globals | top nodes] (inertial), whose globals' block this is.  Tangent space: per camera (w_ck 3 | p_ck 3 |
+// intrinsics K), then with inertial terms (g 2 | b 6 | sf 6 | ts 1); rows / columns of constant or unused parameters
+// (fill_mask) are zero like ceres::Covariance's.
+extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
+  if (!h || !cov) return VCGPU_ERR_INVALID;
+  return run_cov(h, cov, false);
+}
+
 // Marginal covariance of every frame's tangent (GetCovarianceBlock(t_wp, t_wp) and (v_w, v_w) of ceres::Covariance):
 // the [f, f] blocks of (J^T J)^-1 on the system vcgpu_get_covariance inverts, by a selected inversion of the frame
 // elimination (vc_frame_cov.cuh); no step forms more than a chunk-sized or [globals | top nodes]-sized matrix.
 extern "C" int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   if (h->nranks > 1) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_frame_covariance is one-GPU only: frame shards are not supported");
-  VC_TRY(prepare(h));
-  std::vector<double> D2;
-  int live = 0;
-  VC_TRY(cov_prelude(h, true, &D2, &live));
-  const DevProblem& dp = h->dp;
-  const int64_t nfp = static_cast<int64_t>(dp.n_frames) * dp.fd, np = nfp + dp.G;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
-  FrameCovSpace w;
-  int rc = frame_cov_space(h, &w);
-  if (rc == VCGPU_OK) rc = dp.inertial ? frame_cov_inertial(h, h->d_scale + np, live, w) : frame_cov_vision(h, h->d_scale + np, w);
-  h->blocks_valid = false;  // as vcgpu_get_covariance: the Jacobi scale is the next solve's to set
-  if (rc != VCGPU_OK) return rc;
-  VC_TRY(read_scalars(h));
-  if (h->h_scalars[kScNotPD] > 0) return fail(h, VCGPU_ERR_NUMERIC, "frame covariance: J^T J is singular at the current state");
-  CUDA_TRY(h, cudaMemcpy(cov, w.out, static_cast<size_t>(nfp) * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
-  return VCGPU_OK;
+  return run_cov(h, cov, true);
 }
 extern "C" int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
