@@ -261,11 +261,6 @@ def persistent_fits(G, n_frames, smem_optin=H100_SMEM_OPTIN):
 
 
 # ------------------------------------------------------------------------------------------------ multi-launch engine
-def chain_eliminate_smem_bytes(G, c=CHUNK):
-    """chain_eliminate_kernel: Sacc [G^2 + G] | Al Ap Uc [3 x 81] | El [9 G] | gl [9] | V [(c - 1) 9 (G + 28)]."""
-    return (G * G + G + 3 * FD * FD + FD * G + FD + (c - 1) * FD * (FD + 2 * FD + G + 1)) * 8
-
-
 def chain_dense_smem_bytes(N):
     """dense_solve_kernel: S [N^2] | rhs [N]."""
     return (N * N + N) * 8
@@ -276,7 +271,7 @@ def multi_launch_requests(G, inertial=True, top=TOP):
     NS = G * G + G
     out = {"reduce_finalize_kernel": NS * 8}
     if inertial:
-        out["chain_eliminate_kernel"] = chain_eliminate_smem_bytes(G)
+        out["chain_eliminate_kernel"] = chain_group_doubles(G) * 8  # one group's workspace of chain_solve_kernel
         out["dense_solve_kernel"] = chain_dense_smem_bytes(G + FD * top)
     else:
         out["frame_solve_kernel"] = (NS + (K["kSolveThreads"] // 32) * 2 * 6 * (G + 1)) * 8

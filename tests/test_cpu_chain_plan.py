@@ -127,7 +127,7 @@ def _rig_globals_accepted():
 @pytest.mark.parametrize("inertial", [False, True])
 def test_multi_launch_requests_fit_every_rig(inertial):
     """Every multi-launch kernel's dynamic shared memory, for every accepted rig and 1..4 top nodes, is at most what the
-    engine opts in to.  The largest rig (8 x kb4 + IMU, G = 127) asks 219 328 B for the chain elimination and 213 856 B
+    engine opts in to.  The largest rig (8 x kb4 + IMU, G = 127) asks 227 752 B for the chain elimination and 213 856 B
     for the dense solve with 4 top nodes: more than a fixed 200 KB, less than the H100's 227 KB."""
     limit = cp.engine_smem_optin(cp.H100_SMEM_OPTIN)
     worst = {}
@@ -140,5 +140,5 @@ def test_multi_launch_requests_fit_every_rig(inertial):
     over = {k: v for k, v in worst.items() if v[0] > limit}
     assert not over, f"requests (bytes, G) above the {limit} B opt-in: {over}"
     if inertial:
-        assert worst["chain_eliminate_kernel"] == (219328, 127)
+        assert worst["chain_eliminate_kernel"] == (227752, 127)
         assert worst["dense_solve_kernel"] == (213856, 127)

@@ -121,6 +121,13 @@ struct SelinvArgs {
   const double* Sgg;       // Σ_gg, leading dimension ldg
   int ldg;
   double* scalars;
+  // chain_selinv_kernel's NodeSrc of level l = lev[l] (level 0: the normal equations, with the damping in D2x)
+  const ChainLevel* lev;
+  int l, nf;
+  Blocks b[2];
+  const Ctl* ctl;
+  const double* scale;
+  const double* D2x;
 };
 
 // shared memory of one chunk of c nodes (chain_selinv_chunk): T [(c-1) FD]^2 | K [(c-1) FD]^2 | P [(c-1) FD][2 FD + G]
@@ -147,8 +154,8 @@ __device__ __forceinline__ double selinv_boundary(const SelinvArgs& a, int j, bo
 
 // Chunk j of level l (separator s = j c, interior nodes s+1 .. s+m) by NT threads: this thread is `tid` of them, sync()
 // is their barrier, sm their workspace (chain_selinv_smem_bytes), *bad their pivot flag.  node_A(p, e) and node_U(p, e)
-// give entry e of H[p, p] and of H[p-1, p] at level l as the elimination saw them (A + addA and U, or at level 0 of a
-// cluster, which never stores them, the scaled and damped normal equations).  The caller separates two chunks that
+// give entry e of H[p, p] and of H[p-1, p] at level l as the elimination saw them (A + addA and U, or at level 0,
+// which the elimination reads on the fly, the scaled and damped normal equations: src_A, src_U).  The caller separates two chunks that
 // share a workspace with sync().
 template <int FD, int NT, class Sync, class NodeA, class NodeU>
 __device__ __forceinline__ void chain_selinv_chunk(const SelinvArgs& a, int j, double* sm, int tid, int* bad, Sync sync, NodeA node_A,
@@ -245,16 +252,19 @@ __device__ __forceinline__ void chain_selinv_chunk(const SelinvArgs& a, int j, d
     a.sig.kg[static_cast<int64_t>(s) * FD * G + e] = __ldcg(a.up.kg + static_cast<int64_t>(j) * FD * G + e);
 }
 
-// One CTA per chunk of level l (vcgpu_get_frame_covariance: the multi-launch chain kernels stored every level's blocks)
+// One CTA per chunk of level l (vcgpu_get_frame_covariance), its nodes read as chain_frame_cov_batch_kernel's walk reads
+// them: the call refuses frame shards, so level 0 has neither a ghost nor a separator's summed diagonal
 template <int FD>
 __global__ void __launch_bounds__(kChainThreads) chain_selinv_kernel(SelinvArgs a) {
   extern __shared__ double sm[];
   __shared__ int bad;
-  const ChainLevel& L = a.cur;
+  NodeSrc src;
+  src.L = a.l > 0 ? a.lev + a.l : nullptr;
+  src.b = a.b[a.ctl->cur]; src.scale = a.scale; src.D2x = a.D2x; src.rinv = 0.0; src.G = a.G; src.nf = a.nf;
+  src.sepdiag = nullptr; src.rank = 0; src.ghost = 0;
   chain_selinv_chunk<FD, kChainThreads>(
-      a, blockIdx.x, sm, threadIdx.x, &bad, [] { __syncthreads(); },
-      [&](int64_t p, int e) { return L.A[p * FD * FD + e] + (L.addA ? L.addA[p * FD * FD + e] : 0.0); },
-      [&](int64_t p, int e) { return L.U[p * FD * FD + e]; });
+      a, blockIdx.x, sm, threadIdx.x, &bad, [] { __syncthreads(); }, [&](int64_t p, int e) { return src_A<FD>(src, p, e); },
+      [&](int64_t p, int e) { return src_U<FD>(src, p, e); });
 }
 
 // Level 0's Σ_ff unscaled, s_f Σ_ff s_f, and exactly symmetric: both halves are written from the lower triangle.  Rows

@@ -1,6 +1,6 @@
 // Persistent (cooperative) kernels of the inertial trust-region iteration — one GPU.
 //
-// An inertial LM iteration used to be ~21 launches (chain_init, one chain_eliminate per level, sum_partials,
+// An inertial LM iteration on the multi-launch engine is ~20 launches (one chain_eliminate per level, sum_partials,
 // dense_solve, one chain_backsub per level, backsub_update, fused_build, imu_eval, imu_accumulate, reduce_finalize,
 // imu_weights).  Here it is TWO cooperative launches of one CTA per SM, with grid barriers where a launch boundary
 // used to be:
@@ -16,8 +16,9 @@
 //                        reduction, accept/reject, UpdateImuWeights
 //
 // Replaces what ceres::Solve does per iteration for the inertial stages (vicalibrator.h:956; SPARSE_NORMAL_CHOLESKY
-// on the block-tridiagonal + arrow J^T J, SURVEY §8 a12).  Same arithmetic as vc_chain.cuh's kernels (which remain
-// the engine of frame-sharded runs, where an NCCL all-reduce sits between assembling and factoring the dense system).
+// on the block-tridiagonal + arrow J^T J, SURVEY §8 a12).  The multi-launch engine (vc_imu_host.inl; the solves that do
+// not fit here, frame shards without mapped exchange buffers, the per-handle covariance calls) runs the same chunk and
+// node routines, one level per launch (chain_eliminate_kernel, chain_backsub_kernel below).
 #pragma once
 #include <cooperative_groups.h>
 
@@ -129,54 +130,6 @@ __device__ __forceinline__ void adv2(int& r, int& q, int W, int step) {
   while (q >= W) { q -= W; ++r; }
 }
 
-// where a level's node blocks come from: level 0 reads the block normal equations and applies the Jacobi scaling and
-// the LM damping on the fly (no separate pass, no copy); deeper levels read what the level above left
-struct NodeSrc {
-  const ChainLevel* L;   // level >= 1 (null at level 0)
-  Blocks b;              // level 0
-  const double* scale;
-  const double* D2x;
-  double rinv;
-  int G, nf;
-  const double* sepdiag;  // sharded: summed diagonal of the ranks' first frames (damping of frame 0; the ghost is damped by its owner)
-  int rank, ghost;
-};
-template <int FD>
-__device__ __forceinline__ double src_A(const NodeSrc& s, int64_t p, int e) {
-  if (s.L) return s.L->A[p * FD * FD + e] + (s.L->addA ? s.L->addA[p * FD * FD + e] : 0.0);
-  const int r = e / FD, c = e - r * FD;
-  const double* sf = s.scale + p * FD;
-  const double bij = s.b.B[p * FD * FD + e];
-  double v = bij * sf[r] * sf[c];
-  // frame_damp's rule, written out: through frame_damp the compiler fuses this add differently and the solve's bits change
-  if (r == c) {
-    const bool is_ghost = s.ghost && p == s.nf - 1;
-    if (is_ghost) ;  // damped once, by the rank that owns the frame
-    else if (s.D2x) v += s.D2x[p * FD + r];
-    else if (s.sepdiag && p == 0) v += lm_damp(s.sepdiag[s.rank * FD + r], sf[r], s.rinv);
-    else v += lm_damp(bij, sf[r], s.rinv);
-  }
-  return v;
-}
-template <int FD>
-__device__ __forceinline__ double src_U(const NodeSrc& s, int64_t p, int e) {  // H[p-1, p]
-  if (s.L) return s.L->U[p * FD * FD + e];
-  if (p == 0) return 0.0;
-  const int r = e / FD, c = e - r * FD;
-  return s.b.U[p * FD * FD + e] * s.scale[(p - 1) * FD + r] * s.scale[p * FD + c];
-}
-template <int FD>
-__device__ __forceinline__ double src_E(const NodeSrc& s, int64_t p, int r, int c) {
-  const int e = r * s.G + c;
-  if (s.L) return s.L->E[p * FD * s.G + e] + (s.L->addE ? s.L->addE[p * FD * s.G + e] : 0.0);
-  return s.b.E[p * FD * s.G + e] * s.scale[p * FD + r] * s.scale[static_cast<int64_t>(s.nf) * FD + c];
-}
-template <int FD>
-__device__ __forceinline__ double src_g(const NodeSrc& s, int64_t p, int e) {
-  if (s.L) return s.L->g[p * FD + e] + (s.L->addg ? s.L->addg[p * FD + e] : 0.0);
-  return s.b.gf[p * FD + e] * s.scale[p * FD + e];
-}
-
 // 8-byte copy global -> shared that does not pass through a register, and the wait for all of this thread's copies
 __device__ __forceinline__ void cp_async8(double* dst, const double* src) {
   const unsigned d = static_cast<unsigned>(__cvta_generic_to_shared(dst));
@@ -201,13 +154,13 @@ __device__ __forceinline__ void add_in_place(const double* add, int n, int tid, 
   }
 }
 
-// Forward + backward sweep of one chunk (separator s = j*c, interior nodes s+1..s+m) by one group of 128 threads.
-// Same algorithm as chain_eliminate_kernel (vc_chain.cuh); here the chunk's blocks arrive by asynchronous copies
-// straight into their places in shared memory, all in flight before the first one is used (no register staging: nothing
-// grows with the chunk length), the 9 x 9 pivots are factored right-looking with rsqrt, and the group's Schur
-// accumulator Sacc lives on across chunks and levels.
+// Forward + backward sweep of one chunk (separator s = j*c, interior nodes s+1..s+m) by one group of 128 threads, in
+// chain_solve and, one chunk per CTA, in the multi-launch engine's chain_eliminate_kernel.  The chunk's blocks arrive by
+// asynchronous copies straight into their places in shared memory, all in flight before the first one is used (no
+// register staging: nothing grows with the chunk length), the 9 x 9 pivots are factored right-looking with rsqrt, and
+// the group's Schur accumulator Sacc lives on across chunks and levels.
 // NT: threads working on the chunk — a group of 128 (two chunks per CTA in flight: the wide levels) or the whole CTA of
-// 256 (levels with fewer chunks than CTAs, where the other group would idle)
+// 256 (levels with fewer chunks than CTAs, where the other group would idle); either covers a V row, one column each
 template <int NT>
 __device__ __forceinline__ void gsync(int grp) {
   if (NT == kCsThreads) __syncthreads();
@@ -568,6 +521,59 @@ template <int FD>
 __device__ __forceinline__ void chain_backsub_level(const ChainLevel cur, int l, double* delta, int64_t nfp, int G, int gw, int nw, int lane) {
   const int n_slots = chain_backsub_slots(cur);
   for (int t = gw; t < n_slots; t += nw) chain_backsub_node<FD>(cur, l, delta, nfp, G, t, lane);
+}
+
+// ------------------------------------------------------------------ the multi-launch engine (vc_imu_host.inl)
+// One level of the elimination per launch, one CTA per separator-led chunk, chain_solve's chunk routine on the CTA's
+// own Schur accumulator.  The CTA's partial is written unpacked, [G*G + G]: both triangles from the packed lower one,
+// then the right-hand side, the layout sum_partials_kernel, dense_solve_kernel and the sharded all-reduce take.
+// NT: kCsGroup threads where they cover a V row (3 FD + G + 1 columns, one pivot solve each), else kCsThreads.
+struct ElimArgs {
+  DevProblem dp;
+  Blocks b[2];
+  const Ctl* ctl;
+  const double* scale;
+  const double* D2x;
+  const double* sepdiag;
+  const ChainLevel* lev;  // the level table (device memory)
+  int l;                  // the level eliminated: lev[l] -> lev[l + 1]
+  double* Spart;          // [gridDim][G*G+G]
+  double* scalars;
+};
+template <int NT>
+__global__ void __launch_bounds__(NT) chain_eliminate_kernel(ElimArgs a) {
+  extern __shared__ double sm[];  // chain_group_doubles(G)
+  __shared__ int bad;
+  if (a.ctl->done) return;
+  constexpr int FD = 9;
+  const int G = a.dp.G, GT = G * (G + 1) / 2, tid = threadIdx.x;
+  const NodeSrc src = chain_src(a.l > 0 ? a.lev + a.l : nullptr, a.dp, a.b, a.ctl, a.scale, a.D2x, a.sepdiag);
+  if (tid == 0) bad = 0;
+  for (int e = tid; e < chain_sacc_doubles(G); e += NT) sm[e] = 0.0;
+  chain_eliminate_chunk<FD, NT>(src, a.lev[a.l], a.lev[a.l + 1], G, blockIdx.x, sm, tid, 0, &bad);
+  __syncthreads();
+  if (tid == 0 && bad) a.scalars[kScNotPD] = 1.0;
+  double* out = a.Spart + static_cast<int64_t>(blockIdx.x) * (G * G + G);
+  for (int e = tid; e < G * G; e += NT) {
+    const int r = e / G, c = e - r * G, hi = max(r, c), lo = min(r, c);
+    out[e] = sm[hi * (hi + 1) / 2 + lo];
+  }
+  for (int r = tid; r < G; r += NT) out[G * G + r] = sm[GT + r];
+}
+
+// One level of the back-substitution per launch, one warp per node slot (chain_backsub_slots)
+struct BacksubArgs {
+  const Ctl* ctl;
+  int G, l;
+  ChainLevel cur;
+  double* delta;
+  int64_t nfp;
+};
+constexpr int kBacksubWarps = 4;
+__global__ void __launch_bounds__(32 * kBacksubWarps) chain_backsub_kernel(BacksubArgs a) {
+  const int slot = blockIdx.x * kBacksubWarps + (threadIdx.x >> 5);
+  if (a.ctl->done || slot >= chain_backsub_slots(a.cur)) return;
+  chain_backsub_node<9>(a.cur, a.l, a.delta, a.nfp, a.G, slot, threadIdx.x & 31);
 }
 
 // The back-substitution of every level on the cooperative grid, by whichever CTA calls it: items of kCsBsItem nodes at

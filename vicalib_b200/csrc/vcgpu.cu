@@ -1008,6 +1008,7 @@ static int cov_inertial(vcgpu_handle* h, const double* D2x, bool frames, int liv
     vc::SelinvArgs sa;
     sa.G = G; sa.c = kChainC; sa.cur = d->levels[l]; sa.sig = w.sig[l]; sa.up = w.sig[l + 1];
     sa.Sgg = w.inv; sa.ldg = w.N; sa.scalars = h->d_scalars;
+    sa.lev = d->d_levels; sa.l = l; sa.nf = dp.n_frames; sa.b[0] = h->blk[0]; sa.b[1] = h->blk[1]; sa.ctl = h->d_ctl; sa.scale = h->d_scale; sa.D2x = D2x;
     vc::chain_selinv_kernel<FD><<<d->levels[l + 1].n, vc::kChainThreads, sm, h->stream>>>(sa);
     ++h->launches;
   }
