@@ -213,6 +213,19 @@ def get_range(t, w, a, ts, t0, t1):
 
 
 def imu_residual(t, w, a, t0, t1, R2, p2, v2, R1, p1, v1, g, b, sf, ts, W, switch):
+    p, R, v = integrate(t, w, a, t0, t1, R1, p1, v1, g, b, sf, ts)
+    Re = R * R2.T
+    te = p - Re * p2
+    raw = se3_log(Re, te) + list(v - v2)
+    r = [sum(raw[i] * W[i, j] for i in range(9)) for j in range(9)]
+    if switch:
+        for j in (0, 1, 2, 6, 7, 8):
+            r[j] = mp.mpf(0)
+    return r
+
+
+def integrate(t, w, a, t0, t1, R1, p1, v1, g, b, sf, ts):
+    """(p, R, v) at t1 from (p1, R1, v1) at t0: RK4 over the measurements of get_range"""
     gv = gravity_vec(g)
     bg, ba = mp.matrix(b[:3]), mp.matrix(b[3:])
     meas = get_range(t, w, a, ts, t0, t1)
@@ -242,14 +255,7 @@ def imu_residual(t, w, a, t0, t1, R2, p2, v2, R1, p1, v1, g, b, sf, ts, W, switc
         k4 = deriv(*y3, z0, z1, dt)
         k = [k1[i] + 2 * k2[i] + 2 * k3[i] + k4[i] for i in range(3)]
         p, R, v = step(p, R, v, k, dt / 6)
-    Re = R * R2.T
-    te = p - Re * p2
-    raw = se3_log(Re, te) + list(v - v2)
-    r = [sum(raw[i] * W[i, j] for i in range(9)) for j in range(9)]
-    if switch:
-        for j in (0, 1, 2, 6, 7, 8):
-            r[j] = mp.mpf(0)
-    return r
+    return p, R, v
 
 
 def imu_kat(rng):
@@ -359,6 +365,75 @@ def imu_edge_kat():
                 ts=np.array(EDGE_TS), W=W, r=np.array(out_r).reshape(1, nf - 1, 9), J=np.array(out_J).reshape(1, nf - 1, 9, 33))
 
 
+# interval k of the vigorous fixture: frame k + 1 = sign * (integrated end state of interval k) * Exp(angle * axis), so
+# that the rotation of log(T_end T_2^-1) is `angle` and its quaternion has w = sign * cos(angle / 2) as the kernels
+# compute it (the integrated end keeps the sign of frame k)
+VIGOROUS_CASES = [
+    (-1, 3e-11),  # converged, frame 2 of the opposite sign: w ~ -1, SO3 log's Taylor branch (|vec| < 1e-10)
+    (-1, 0.9),    # opposite sign, large residual
+    (+1, 2.6),    # large angle: the V^-1 coefficient far from its small-angle limit
+    (-1, 2.95),   # large angle, opposite sign: w ~ -0.1
+    (+1, 0.2),
+    (-1, 2.75),
+    (+1, 3e-11),  # converged, same sign
+]
+VIGOROUS_RATE = 300.0
+VIGOROUS_TS = 0.0031
+
+
+def imu_vigorous_kat():
+    """The IMU residual under vigorous motion and across the quaternion double cover (tests/golden/imu_vigorous_kat.npz,
+    keys of imu_kat.npz with both switch values): a ~300 Hz jittered stream with |w| up to ~9 rad/s (|w| dt up to ~0.03
+    per RK4 step) and |a| up to ~25 m/s^2, 21-36 steps per interval, frame quaternions of both signs (frame 0 has w < 0)
+    and the residual rotations of VIGOROUS_CASES."""
+    from vicalib_b200.synth import mat_to_quat, quat_mul, quat_to_mat, so3_exp as np_exp
+    rng = np.random.default_rng(20261018)
+    nf = len(VIGOROUS_CASES) + 1
+    lengths = rng.uniform(0.07, 0.12, nf - 1)
+    ftime = 0.15 + np.concatenate([[0.0], np.cumsum(lengths)])
+    n = int((ftime[-1] - 0.1) * VIGOROUS_RATE) + 15
+    t = 0.1 + (np.arange(n) + 0.25 * rng.random(n)) / VIGOROUS_RATE
+    f, ph = rng.uniform(1.5, 3.0, (2, 3)), rng.uniform(0, 2 * np.pi, (2, 3))
+    w = np.array([6.0, 5.0, 6.5]) * np.sin(2 * np.pi * f[0] * t[:, None] + ph[0]) + rng.normal(0, 0.05, (n, 3))
+    a = np.array([0.3, 9.7, 0.5]) + np.array([12.0, 10.0, 13.0]) * np.sin(2 * np.pi * f[1] * t[:, None] + ph[1])
+    a += rng.normal(0, 0.05, (n, 3))
+    tt = t + VIGOROUS_TS
+    assert np.all(np.diff(t) > 0) and tt[0] < ftime[0] and tt[-1] > ftime[-1]
+    assert np.abs(tt[:, None] - ftime[None, :]).min() > 1e-5  # no sample near a frame time: no ts kink
+    g = np.array([0.05, -0.03]); b = np.concatenate([rng.normal(0, 1e-2, 3), rng.normal(0, 1e-1, 3)])
+    sf = 1 + 0.02 * rng.normal(size=6)
+    W = 500 * np.eye(9) + 20 * rng.normal(size=(9, 9))
+    q = np.zeros((nf, 4)); p = np.zeros((nf, 3)); v = np.zeros((nf, 3))
+    q[0] = -np_exp(rng.normal(0, 0.5, 3)); p[0] = rng.normal(0, 0.3, 3); v[0] = rng.normal(0, 0.5, 3)
+    assert q[0, 3] < 0
+    tm, wm, am = [mp.mpf(float(x)) for x in t], [V(x) for x in w], [V(x) for x in a]
+    mpl = lambda x: [mp.mpf(float(y)) for y in x]  # noqa: E731
+    for k, (sign, angle) in enumerate(VIGOROUS_CASES):
+        pe, Re, ve = integrate(tm, wm, am, mp.mpf(float(ftime[k])), mp.mpf(float(ftime[k + 1])), quat_R(q[k]), V(p[k]), V(v[k]),
+                               mpl(g), mpl(b), mpl(sf), mp.mpf(VIGOROUS_TS))
+        Rk = quat_to_mat(q[k])
+        Re = np.array(Re.tolist(), dtype=np.float64)
+        dq = mat_to_quat(Rk.T @ Re)  # the interval's rotation (< pi), w >= 0: the end keeps frame k's sign
+        qe = quat_mul(q[k], dq)
+        axis = rng.normal(size=3)
+        axis /= np.linalg.norm(axis)
+        q[k + 1] = sign * quat_mul(qe, np_exp(angle * axis))
+        tiny = angle < 1e-6
+        p[k + 1] = np.array([float(x) for x in pe]) + (1e-9 if tiny else 0.05) * rng.normal(size=3)
+        v[k + 1] = np.array([float(x) for x in ve]) + (1e-8 if tiny else 0.1) * rng.normal(size=3)
+        rel = quat_mul(qe, q[k + 1] * np.array([-1, -1, -1, 1.0]))
+        assert np.sign(rel[3]) == sign and abs(2 * np.arccos(min(1.0, abs(rel[3]))) - angle) < 1e-6 + 1e-3 * angle, (k, rel)
+        steps = np.count_nonzero((tt > ftime[k]) & (tt < ftime[k + 1])) + 1
+        assert 20 <= steps <= 50, steps
+    wdt = np.linalg.norm(w[1:], axis=1) * np.diff(t)
+    print(f"vigorous: max |w| {np.linalg.norm(w, axis=1).max():.2f} rad/s, max |w| dt {wdt.max():.4f}, "
+          f"max |a| {np.linalg.norm(a, axis=1).max():.1f} m/s^2", flush=True)
+    out_r, out_J = imu_rows(t, w, a, ftime, q, p, v, g, b, sf, VIGOROUS_TS, W, (0, 1))
+    return dict(imu_t=t, imu_w=w, imu_a=a, ftime=ftime, T_wp=np.concatenate([q, p], 1), v_w=v, g=g, b=b, sf=sf,
+                ts=np.array(VIGOROUS_TS), W=W, r=np.array(out_r).reshape(2, nf - 1, 9),
+                J=np.array(out_J).reshape(2, nf - 1, 9, 33))
+
+
 def edge_kat():
     """Branch and boundary cases of the camera models (each model's own small-argument branches, the image
     centre, the image border).  Written to reproj_edge_kat.npz with the keys of reproj_kat.npz."""
@@ -390,6 +465,9 @@ if __name__ == "__main__":
         sys.exit(0)
     if "--imu-edge" in sys.argv:  # only the interpolation-buffer edge fixture (the others are unchanged)
         np.savez_compressed(os.path.join(HERE, "imu_edge_kat.npz"), **imu_edge_kat())
+        sys.exit(0)
+    if "--imu-vigorous" in sys.argv:  # only the vigorous-motion fixture (the others are unchanged)
+        np.savez_compressed(os.path.join(HERE, "imu_vigorous_kat.npz"), **imu_vigorous_kat())
         sys.exit(0)
     rng = np.random.default_rng(20260924)
     out = {}

@@ -210,6 +210,33 @@ def _look_at(cam_pos, target, roll):
     return R @ Rz
 
 
+def _vigorous_cam0_pose(t, centre, ph):
+    """Camera 0 of a handheld recording that excites every axis, still looking at the grid: translations at 1.3-2 Hz
+    (up to ~13 m/s^2 along the optical axis, so the specific force departs from g by more than 10 m/s^2), tilts at
+    1.1-1.4 Hz and a roll of -0.5 +- 1.4 rad about the optical axis at 0.7 Hz (up to 6 rad/s), which carries the
+    rig's attitude across pi from the world frame (near a roll of -pi/2)."""
+    t = np.asarray(t, dtype=np.float64)
+    w = 2 * np.pi * np.array([1.3, 1.7, 2.0, 1.1, 1.4, 0.7])
+    pos = np.stack(
+        [
+            centre[0] + 0.10 * np.sin(w[0] * t + ph[0]),
+            centre[1] + 0.08 * np.sin(w[1] * t + ph[1]),
+            -(0.47 + 0.08 * np.sin(w[2] * t + ph[2])),
+        ],
+        -1,
+    )
+    tgt = np.stack(
+        [
+            centre[0] + 0.06 * np.sin(w[3] * t + ph[3]),
+            centre[1] + 0.05 * np.sin(w[4] * t + ph[4]),
+            np.zeros_like(t),
+        ],
+        -1,
+    )
+    roll = -0.5 + 1.4 * np.sin(w[5] * t + ph[5])
+    return _look_at(pos, tgt, roll), pos
+
+
 def make_problem(
     models=("poly3",),
     n_frames=50,
@@ -226,6 +253,7 @@ def make_problem(
     height=480,
     imu_noise=True,
     spacing=None,
+    motion="gentle",  # "gentle" (the default trajectory) or "vigorous" (_vigorous_cam0_pose)
 ) -> Problem:
     rng = np.random.default_rng(seed)
     models = np.array([MODEL_IDS[m] if isinstance(m, str) else int(m) for m in models], dtype=np.int32)
@@ -263,8 +291,12 @@ def make_problem(
     ftime = 1.0 + np.arange(n_frames) / frame_rate
     ph = rng.uniform(0, 2 * np.pi, 8)
     fr = 2 * np.pi * np.array([0.31, 0.23, 0.17, 0.41, 0.29, 0.13, 0.37, 0.19])
+    if motion not in ("gentle", "vigorous"):
+        raise ValueError(motion)
 
     def cam0_pose(t):
+        if motion == "vigorous":
+            return _vigorous_cam0_pose(t, centre, ph)
         t = np.asarray(t, dtype=np.float64)
         pos = np.stack(
             [
