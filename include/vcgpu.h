@@ -182,6 +182,55 @@ int vcgpu_solve_batch_inertial(vcgpu_handle* const* handles, int n, vcgpu_summar
  * size the device holds at once (the smaller count of the solve and the evaluation kernel; further rigs of a batch
  * queue behind them).  Any pointer may be NULL.  VCGPU_ERR_INVALID where the batch would refuse the handle. */
 int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int* resident_clusters);
+/* The staged calibration flow of ViCalibrator::SolveThread (vicalibrator.h:919-1040) for n rigs in one call.  Per rig:
+ * vision only -> inertial, rotation only -> translation, gravity and biases -> scale factors -> outlier removal ->
+ * finished, a stage advancing only when its solve converges (termination other than VCGPU_TERM_NO_CONVERGENCE).  At
+ * every stage entry the handle gets what SetupProblem gives it: its own state uploaded again (vcgpu_set_cameras,
+ * vcgpu_set_frames, vcgpu_set_imu_params), the stage's flags and, with block_duplication, the multiplicities of the
+ * blocks added so far (visual 1, 2, 3, ...; IMU 1, 1, 2, 3, ... from the first inertial stage on); then, on entering
+ * the first stage past rotation-only with gravity not yet initialised, gravity from the mid-frame accelerometer sample.
+ * After each solve: the per-camera RMSE sqrt(cost / n) (vcgpu_evaluate), the stage decision and, at its step,
+ * vcgpu_remove_outliers with the rig's own RMSE.  Each rig starts at the stage its vcgpu_set_flags describe (inertial,
+ * rotation_only, bias_active, scale_active as SetOptimizationFlags sets them; without calibrate_imu every stage is a
+ * vision stage) and runs every solve with its own options, strategy included.
+ * A round solves every rig still working: the rigs at a vision stage as one vcgpu_solve_batch (LM or DOGLEG), those at
+ * an inertial stage as one vcgpu_solve_batch_inertial, which here also takes strategy 1 (DOGLEG inside the inertial
+ * cluster kernels); then one vcgpu_evaluate_batch of them all and one vcgpu_remove_outliers_batch of the rigs at that
+ * step.  A rig's whole trajectory of stages, solves and results does not depend, bit for bit, on what else is in the
+ * batch or in which order.  A rig leaves when it finishes or has had max_solves solves (or has no residual left).
+ * out: n summaries or NULL; cam_rmse: NULL, or n pointers (an entry may be NULL) to n_cams RMSEs of the rig's last solve.
+ * Returns VCGPU_ERR_INVALID before anything is launched, with a message naming the index in vcgpu_last_error of every
+ * non-null handle, for: n <= 0, a null flow, max_solves <= 0, a null or repeated handle, handles on different devices,
+ * and a rig that a batch of a kind of stage it can reach would refuse: vcgpu_solve_batch where it starts at a vision
+ * stage or calibrate_imu is off, vcgpu_solve_batch_inertial (strategy 1 excepted) where calibrate_imu is on.  A refused
+ * call changes no handle's state, flags or options, and a handle solves after it as a fresh one at that state does (a
+ * handle checked with its inertial switch flipped is prepared again by its next call). */
+typedef struct {
+  int calibrate_imu;        /* FLAGS_calibrate_imu: advance through the inertial stages */
+  int remove_outliers;      /* FLAGS_remove_outliers */
+  double outlier_threshold; /* FLAGS_outlier_threshold */
+  int block_duplication;    /* re-add blocks per stage as SetupProblem does (the host mirror's default: on) */
+  int gravity_initialized;  /* is_gravity_initialized_ at the start: nonzero keeps the handles' gravity */
+  int max_solves;           /* solves per rig at most (the reference repeats a stage that does not converge forever) */
+} vcgpu_flow;
+enum {  /* vcgpu_flow_summary::stage */
+  VCGPU_FLOW_VISION = 0,       /* inertial terms off */
+  VCGPU_FLOW_ROTATION = 1,     /* inertial, rotation only */
+  VCGPU_FLOW_TRANSLATION = 2,  /* inertial: translation, gravity and biases */
+  VCGPU_FLOW_SCALE = 3,        /* inertial: also the scale factors (and the solves after the outlier removal) */
+  VCGPU_FLOW_FINISHED = 4      /* the stage machine reached its end */
+};
+typedef struct {
+  int solves, iterations;   /* solves run, and their iterations summed */
+  int finished;             /* the stage machine reached its end */
+  int stage;                /* VCGPU_FLOW_* at return */
+  int64_t outliers_removed; /* observations RemoveOutliers removed */
+  double mse;               /* final_cost / num_residuals of the last solve (vicalibrator.h:975) */
+  vcgpu_summary last;       /* the last solve's summary */
+  vcgpu_flags flags;        /* the handle's flags at return: its last stage's, as SetupProblem set them */
+} vcgpu_flow_summary;
+int vcgpu_calibrate_batch(vcgpu_handle* const* handles, int n, const vcgpu_flow* flow, vcgpu_flow_summary* out /* n, or NULL */,
+                          double* const* cam_rmse /* n pointers to n_cams, or NULL */);
 /* run exactly n trust-region iterations with no convergence test and no host round trip per
  * iteration (benchmark entry: LM iterations / second) */
 int vcgpu_iterate(vcgpu_handle* h, int n_iterations, vcgpu_summary* out);

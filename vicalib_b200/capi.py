@@ -26,7 +26,7 @@ EXPORTS = [
     "vcgpu_eval_imu", "vcgpu_normal_equations", "vcgpu_solve_arrow", "vcgpu_comm_unique_id", "vcgpu_comm_init",
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
     "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch", "vcgpu_evaluate_batch", "vcgpu_remove_outliers_batch",
-    "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch",
+    "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch", "vcgpu_calibrate_batch",
 ]
 
 
@@ -60,6 +60,21 @@ class PnpViews(C.Structure):
     _fields_ = [("n_views", C.c_int), ("cam_id", C.c_void_p), ("start", C.c_void_p), ("count", C.c_void_p),
                 ("pix", C.c_void_p), ("pw", C.c_void_p), ("T_cw", C.c_void_p), ("rmse_or_null", C.c_void_p),
                 ("n_used_or_null", C.c_void_p)]
+
+
+class Flow(C.Structure):
+    """vcgpu_flow: the switches of ViCalibrator::SolveThread's stage machine (vcgpu_calibrate_batch)"""
+    _fields_ = [("calibrate_imu", C.c_int), ("remove_outliers", C.c_int), ("outlier_threshold", C.c_double),
+                ("block_duplication", C.c_int), ("gravity_initialized", C.c_int), ("max_solves", C.c_int)]
+
+
+class FlowSummary(C.Structure):
+    _fields_ = [("solves", C.c_int), ("iterations", C.c_int), ("finished", C.c_int), ("stage", C.c_int),
+                ("outliers_removed", C.c_int64), ("mse", C.c_double), ("last", Summary), ("flags", Flags)]
+
+
+# vcgpu_flow_summary::stage
+FLOW_VISION, FLOW_ROTATION, FLOW_TRANSLATION, FLOW_SCALE, FLOW_FINISHED = range(5)
 
 
 class Config(C.Structure):
@@ -374,6 +389,32 @@ def solve_batch_inertial(calibrators):
     """vcgpu_solve_batch_inertial: solve_batch for rigs with inertial terms on (each rig in its own thread-block cluster
     of the persistent inertial kernels).  Returns one summary dict per calibrator, in order."""
     return _solve_many(lib().vcgpu_solve_batch_inertial, calibrators)
+
+
+def calibrate_batch(calibrators, calibrate_imu=True, remove_outliers=True, outlier_threshold=2.0, block_duplication=True,
+                    gravity_initialized=False, max_solves=100):
+    """vcgpu_calibrate_batch: ViCalibrator::SolveThread's staged flow for every Calibrator of the list in one call,
+    each rig from the stage its flags describe.  Returns one (summary dict, per-camera RMSE array) per calibrator, in
+    order; the dict holds solves, iterations, finished, stage (FLOW_*), outliers_removed, mse, `last` (the last
+    solve's summary dict) and `flags` (a dict of the handle's flags at return, which also become the calibrator's)."""
+    n = len(calibrators)
+    L = lib()
+    flow = Flow(int(calibrate_imu), int(remove_outliers), float(outlier_threshold), int(block_duplication),
+                int(gravity_initialized), int(max_solves))
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    out = (FlowSummary * max(n, 1))()
+    rmse = [np.zeros(max(g.n_cams, 1)) if g is not None else np.zeros(1) for g in calibrators]
+    rp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in rmse])
+    _batch_check(L, L.vcgpu_calibrate_batch(hs, C.c_int(n), C.byref(flow), out, rp), calibrators)
+    res = []
+    for i, g in enumerate(calibrators):
+        s = out[i]
+        d = {f[0]: getattr(s, f[0]) for f in FlowSummary._fields_ if f[0] not in ("last", "flags")}
+        d["last"] = {f[0]: getattr(s.last, f[0]) for f in Summary._fields_}
+        d["flags"] = {f[0]: getattr(s.flags, f[0]) for f in Flags._fields_}
+        C.memmove(C.byref(g.flags), C.byref(s.flags), C.sizeof(Flags))
+        res.append((d, rmse[i][: g.n_cams].copy()))
+    return res
 
 
 def _solve_many(entry, calibrators):

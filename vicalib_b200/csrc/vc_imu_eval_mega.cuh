@@ -117,8 +117,9 @@ __device__ __noinline__ void eval_imu_task(const ImuEvalView a, int task, int la
 }
 
 // The evaluation of the rig `a` by the CTAs of `scope` (vc_mega.cuh): the cooperative grid (eval_mega_kernel) or one
-// thread-block cluster (eval_mega_batch_kernel; never sharded: the exchange is compiled out for it).
-template <class Scope>
+// thread-block cluster (eval_mega_batch_kernel; never sharded: the exchange is compiled out for it).  Str: the strategy
+// whose decision D takes (decide_step<Str>: a DOGLEG step's model change, mu and radius are the solve launch's, in Ctl).
+template <Strategy Str, class Scope>
 __device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
   extern __shared__ double smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -228,7 +229,7 @@ __device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
       if (sharded) {  // this rank's share; the totals are formed below
         for (int q = 0; q < kScNotPD; ++q) xchg_put(a.x, xbufs, eSc + q, t[q]);
       } else {
-        finish_scalars(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
+        finish_scalars<Str>(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
         *a.counter = 0u;  // the task queue of the next launch
         __threadfence();
       }
@@ -293,7 +294,7 @@ __device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
           t[kScGnorm2] += gsh[ww][0];
           t[kScGmax] = fmax(t[kScGmax], gsh[ww][1]);
         }
-        finish_scalars(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
+        finish_scalars<Str>(a.ctl, a.scalars, bt.cost, t, a.step_part != nullptr, a.decide_mode);
         *a.counter = 0u;
         __threadfence();
       }
@@ -315,13 +316,14 @@ __device__ __forceinline__ void eval_mega(const EvalMegaArgs& a, Scope scope) {
 }
 
 // One rig on the whole cooperative grid.
-__global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a) { eval_mega(a, GridScope()); }
+__global__ void __launch_bounds__(kEvThreads, 1) eval_mega_kernel(EvalMegaArgs a) { eval_mega<Strategy::kLM>(a, GridScope()); }
 
 // A batch of rigs, one thread-block cluster each: cluster k evaluates args[k], read where they are (as
-// chain_solve_batch_kernel's)
+// chain_solve_batch_kernel's), and decides as strategy Str
+template <Strategy Str>
 __global__ void __launch_bounds__(kEvThreads, 1) eval_mega_batch_kernel(const EvalMegaArgs* __restrict__ args) {
   ClusterScope scope;
-  eval_mega(args[blockIdx.x / scope.nb()], scope);
+  eval_mega<Str>(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

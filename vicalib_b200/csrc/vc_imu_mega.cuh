@@ -845,6 +845,188 @@ __device__ __forceinline__ void dense_assemble(const ChainSolveArgs& a, const Bl
     S[e] = entry(e);
   }
 }
+// DOGLEG's step (vc_dogleg.cuh) of the rig `a` and its update, by the CTAs of one cluster, once every frame's Gauss-Newton
+// step x = (H + mu D^2)^-1 (-g) is in a.delta (H = S J^T J S, D = sqrt(clamp(diag H)), g~ = g / D, u = g~ / D, gn = D x).
+// The six step scalars of the persistent vision kernel (kDlG2 .. kDlXHx): per CTA, one warp per frame of frames bid * 8
+// + warp, + 8 nb, ... — |g~_f|^2, |gn_f|^2, g~_f.gn_f and the frame rows of u.Hu, u.Hx, x.Hx over the block-tridiagonal +
+// arrow system: B_f, the couplings U to both neighbours, E_f both ways — the warps added in order, CTA 0 adding the
+// globals' rows (C and their own entries); one slot per CTA (a.Spart: the Schur partials are spent by now); a cluster
+// barrier; every CTA adds the slots up in CTA order, takes dogleg_point() and the same (cg, cn).  Then x (+) S step of
+// every frame and of the globals with step = (cg g~ + cn gn) / D (0 when the solve failed), into acc and the globals'
+// step_part slot as the LM update writes them.  The model change -step.g - step.H.step / 2 is expanded over the explicit
+// products, as the vision kernel forms it: -(cg |g~|^2 + cn g~.gn) - (cg^2 u.Hu + 2 cg cn u.Hx + cn^2 x.Hx) / 2.
+// sm: 3 G doubles of free shared memory.
+__device__ __noinline__ void chain_dogleg_update(const ChainSolveArgs& a, ClusterScope scope, double mu, double* sm, double* acc) {
+  constexpr int FD = 9;
+  constexpr int kWarps = kCsThreads / 32;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nb = scope.nb(), bid = scope.bid();
+  const int G = a.dp.G, NS = G * G + G, nf = a.dp.n_frames;
+  const int64_t nfp = static_cast<int64_t>(nf) * FD;
+  const Blocks& b = a.b[a.ctl->cur];
+  const double* s = a.scale;
+  __shared__ double wpart[kWarps][kDlParts];
+  __shared__ double step_s[3];  // cg, cn, ok
+  double* pug = sm;       // [G] s u of the globals
+  double* pxg = pug + G;  // [G] s x
+  double* dg = pxg + G;   // [G] the globals' step
+  for (int k = tid; k < G; k += kCsThreads) {
+    double D, gt;
+    dl_scaled(b.C[k * G + k], b.gc[k], s[nfp + k], &D, &gt);
+    pug[k] = s[nfp + k] * (gt / D);
+    pxg[k] = s[nfp + k] * __ldcg(a.delta + nfp + k);
+  }
+  __syncthreads();
+  double q[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int f = bid * kWarps + warp; f < nf; f += nb * kWarps) {
+    const int64_t o = static_cast<int64_t>(f) * FD;
+    // lane l < 27: entry l % 9 of frame f - 1 + l / 9 (s u, s x); lane r < 9 works row r of frame f
+    double pu = 0.0, px = 0.0, gt = 0.0, D = 1.0, x = 0.0;
+    {
+      const int node = f - 1 + lane / FD, r = lane % FD;
+      if (lane < 3 * FD && node >= 0 && node < nf) {
+        const int64_t i = static_cast<int64_t>(node) * FD + r;
+        dl_scaled(b.B[i * FD + r], b.gf[i], s[i], &D, &gt);
+        x = __ldcg(a.delta + i);
+        pu = s[i] * (gt / D);
+        px = s[i] * x;
+      }
+    }
+    double hu = 0.0, hx = 0.0;
+    const int r = lane < FD ? lane : 0;
+#pragma unroll
+    for (int c = 0; c < FD; ++c) {  // B_f
+      const double bv = b.B[(o + r) * FD + c];
+      hu += bv * __shfl_sync(0xffffffffu, pu, FD + c);
+      hx += bv * __shfl_sync(0xffffffffu, px, FD + c);
+    }
+#pragma unroll
+    for (int c = 0; c < FD; ++c) {  // U[f] = H[f-1, f]: U[f]^T (f - 1);  U[f+1] (f + 1)
+      const double ul = f > 0 ? b.U[o * FD + c * FD + r] : 0.0;
+      const double ur = f + 1 < nf ? b.U[(o + FD) * FD + r * FD + c] : 0.0;
+      hu += ul * __shfl_sync(0xffffffffu, pu, c) + ur * __shfl_sync(0xffffffffu, pu, 2 * FD + c);
+      hx += ul * __shfl_sync(0xffffffffu, px, c) + ur * __shfl_sync(0xffffffffu, px, 2 * FD + c);
+    }
+    double eu = 0.0, ex = 0.0;
+#pragma unroll
+    for (int rr = 0; rr < FD; ++rr) {  // E_f s u_g, E_f s x_g: lanes split the columns
+      double su = 0.0, sx = 0.0;
+      for (int c = lane; c < G; c += 32) {
+        const double e = b.E[(o + rr) * G + c];
+        su += e * pug[c];
+        sx += e * pxg[c];
+      }
+#pragma unroll
+      for (int k = 16; k > 0; k >>= 1) {
+        su += __shfl_xor_sync(0xffffffffu, su, k);
+        sx += __shfl_xor_sync(0xffffffffu, sx, k);
+      }
+      eu = rr == r ? su : eu;
+      ex = rr == r ? sx : ex;
+    }
+    // the own entry of row r sits in lane 9 + r
+    const double pur = __shfl_sync(0xffffffffu, pu, FD + r), pxr = __shfl_sync(0xffffffffu, px, FD + r);
+    const double gtr = __shfl_sync(0xffffffffu, gt, FD + r), Dr = __shfl_sync(0xffffffffu, D, FD + r);
+    const double xr = __shfl_sync(0xffffffffu, x, FD + r);
+    if (lane < FD) {
+      const double gn = xr * Dr;
+      q[kDlG2] += gtr * gtr;
+      q[kDlGn2] += gn * gn;
+      q[kDlB] += gtr * gn;
+      q[kDlUHu] += pur * (hu + 2.0 * eu);
+      q[kDlUHx] += pur * (hx + ex) + pxr * eu;
+      q[kDlXHx] += pxr * (hx + 2.0 * ex);
+    }
+  }
+  if (bid == 0) {  // the globals' rows: C and their own entries
+    for (int k = tid; k < G; k += kCsThreads) {
+      double cu = 0.0, cx = 0.0;
+      for (int c = 0; c < G; ++c) {
+        const double cv = b.C[k * G + c];
+        cu += cv * pug[c];
+        cx += cv * pxg[c];
+      }
+      double D, gt;
+      dl_scaled(b.C[k * G + k], b.gc[k], s[nfp + k], &D, &gt);
+      const double gn = __ldcg(a.delta + nfp + k) * D;
+      q[kDlG2] += gt * gt;
+      q[kDlGn2] += gn * gn;
+      q[kDlB] += gt * gn;
+      q[kDlUHu] += pug[k] * cu;
+      q[kDlUHx] += pug[k] * cx;
+      q[kDlXHx] += pxg[k] * cx;
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < kDlParts; ++j)
+#pragma unroll
+    for (int k = 16; k > 0; k >>= 1) q[j] += __shfl_xor_sync(0xffffffffu, q[j], k);
+  if (lane == 0)
+    for (int j = 0; j < kDlParts; ++j) wpart[warp][j] = q[j];
+  __syncthreads();
+  if (tid == 0) {
+    for (int j = 0; j < kDlParts; ++j) {
+      double t = 0.0;
+      for (int w = 0; w < kWarps; ++w) t += wpart[w][j];
+      a.Spart[static_cast<int64_t>(bid) * NS + j] = t;
+    }
+  }
+  scope.sync();
+  if (tid == 0) {  // every CTA alike: the totals in CTA order, the dogleg point
+    double t[kDlParts] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int c = 0; c < nb; ++c)
+      for (int j = 0; j < kDlParts; ++j) t[j] += __ldcg(a.Spart + static_cast<int64_t>(c) * NS + j);
+    const int ok = __ldcg(a.scalars + kScNotPD) > 0.0 ? 0 : 1;
+    const double alpha = t[kDlG2] / t[kDlUHu];
+    double cg, cn;
+    const double step_norm = dogleg_point(a.ctl->radius, alpha, t[kDlG2], t[kDlGn2], t[kDlB], &cg, &cn);
+    if (!ok) cg = cn = 0.0;
+    step_s[0] = cg; step_s[1] = cn; step_s[2] = ok;
+    if (bid == 0) {
+      Ctl* c = a.ctl;
+      c->dl_g2 = t[kDlG2];
+      c->dl_alpha = alpha;
+      c->dl_gn2 = t[kDlGn2];
+      c->dl_b = t[kDlB];
+      c->dl_ok = ok;
+      c->dl_step_norm = step_norm;
+      c->dl_model_change = -(cg * t[kDlG2] + cn * t[kDlB]) - 0.5 * (cg * cg * t[kDlUHu] + 2.0 * cg * cn * t[kDlUHx] + cn * cn * t[kDlXHx]);
+    }
+  }
+  __syncthreads();
+  const double cg = step_s[0], cn = step_s[1];
+  const bool ok = step_s[2] != 0.0;
+  const double* x_cur = a.state[a.ctl->cur];
+  double* x_new = a.state[1 - a.ctl->cur];
+  for (int f = bid * kCsThreads + tid; f < nf; f += nb * kCsThreads) {  // every frame, the top nodes' too
+    double d[FD];
+#pragma unroll
+    for (int r = 0; r < FD; ++r) {
+      const int64_t i = static_cast<int64_t>(f) * FD + r;
+      double D, gt;
+      dl_scaled(b.B[i * FD + r], b.gf[i], s[i], &D, &gt);
+      d[r] = ok ? (cg * gt + cn * (__ldcg(a.delta + i) * D)) / D : 0.0;
+    }
+    frame_plus<FD>(a.dp, b, s, mu, a.D2x, a.sepdiag, f, d, true, x_cur, x_new, acc);
+  }
+  if (bid == 0) {
+    for (int k = tid; k < G; k += kCsThreads) {
+      double D, gt;
+      dl_scaled(b.C[k * G + k], b.gc[k], s[nfp + k], &D, &gt);
+      dg[k] = ok ? (cg * gt + cn * (__ldcg(a.delta + nfp + k) * D)) / D : 0.0;
+    }
+    __syncthreads();
+    if (tid == kCsThreads - 1) {
+      double g4[4] = {0.0, 0.0, 0.0, 0.0};
+      for (int k = 0; k < G; ++k) {
+        g4[0] += dg[k] * b.gc[k] * s[nfp + k];
+        g4[1] += dg[k] * dg[k] * global_damp(k, b.C[k * G + k], s[nfp + k], mu, a.D2x, nfp);
+      }
+      globals_plus(a.dp, x_cur, x_new, dg, s + nfp, g4 + 2);
+      for (int k = 0; k < 4; ++k) a.step_part[4 * static_cast<int64_t>(nb) + k] = g4[k];
+    }
+  }
+}
+
 // One damped solve of the frame-chain + globals system and (optionally) the state update of the rig `a`, by the CTAs
 // of `scope` (vc_mega.cuh): the cooperative grid (chain_solve_kernel) or one thread-block cluster (chain_solve_batch_kernel).
 // The barriers count arrivals on the rig's own counters (a.sync) either way; the CTAs of a cluster are co-scheduled, as
@@ -855,8 +1037,12 @@ __device__ __forceinline__ void dense_assemble(const ChainSolveArgs& a, const Bl
 // the [globals | top nodes] inverse, unscaled into cov (G x G; mask: 0 on constant globals).  No step, no state update.
 // kFrame (with kCov; chain_frame_cov_batch_kernel): no right-hand side at all; the factorisation stays in CTA 0's shared
 // memory for the caller (the L D L^T factor S [RT][LD], then 1 / d at S + RT LD).
-template <class Scope, bool kCov = false, bool kFrame = false>
+// Str = kDogleg (clusters only, with a.do_update): the Gauss-Newton step with the damping mu D^2 (mu = Ctl::dl_mu in
+// place of LM's 1 / radius in the same damping rule), then chain_dogleg_update in place of the LM update.
+template <class Scope, bool kCov = false, bool kFrame = false, Strategy Str = Strategy::kLM>
 __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope, const double* mask = nullptr, double* cov = nullptr) {
+  constexpr bool kDl = Str == Strategy::kDogleg;
+  static_assert(!kDl || (std::is_same<Scope, ClusterScope>::value && !kCov), "DOGLEG runs in the cluster solve");
   extern __shared__ double smem[];
   constexpr int FD = 9;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -875,7 +1061,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
     for (int k = 0; k < kCsSyncWords; ++k) a.sync_next[k] = 0ull;
   if (a.ctl->done) return;  // uniform over the grid: written before this launch
   const Blocks& b = a.b[a.ctl->cur];
-  const double rinv = 1.0 / a.ctl->radius;
+  const double rinv = kDl ? a.ctl->dl_mu : 1.0 / a.ctl->radius;  // the damping's multiplier of clamp(diag H)
   unsigned long long t_prev = 0;
   const bool prof = a.prof != nullptr && bid == 0 && tid == 0;
   if (prof) t_prev = global_ns();
@@ -1234,7 +1420,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
         a.delta[static_cast<int64_t>(a.n_levels > 1 ? top.orig[t] : t) * FD + r] = bd ? 0.0 : rhs[G + (slot0 + t) * FD + r];
       }
       if (tid == 0 && bd) a.scalars[kScNotPD] = 1.0;
-      if (a.do_update && tid < nt) {  // the top nodes' frames
+      if (!kDl && a.do_update && tid < nt) {  // the top nodes' frames
         double d[FD];
         for (int r = 0; r < FD; ++r) d[r] = bd ? 0.0 : rhs[G + (slot0 + tid) * FD + r];
         frame_plus<FD>(a.dp, b, a.scale, rinv, a.D2x, a.sepdiag, a.n_levels > 1 ? top.orig[tid] : tid, d, true, a.state[a.ctl->cur],
@@ -1242,7 +1428,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
       }
       // globals: cameras + IMU parameters (one thread; the step.g / step.D2.step sums over the globals by its warp)
       double gs0 = 0.0, gs1 = 0.0;
-      if (a.do_update && warp == kCsThreads / 32 - 1) {
+      if (!kDl && a.do_update && warp == kCsThreads / 32 - 1) {
         for (int k = lane; k < G; k += 32) {
           const double d2 = global_damp(k, b.C[k * G + k], sc[k], rinv, a.D2x, nfp);
           const double dk = bd ? 0.0 : rhs[k];
@@ -1255,7 +1441,7 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
           if (lane >= o) { gs0 += t0; gs1 += t1; }
         }
       }
-      if (a.do_update && tid == kCsThreads - 1) {
+      if (!kDl && a.do_update && tid == kCsThreads - 1) {
         const double* x_cur = a.state[a.ctl->cur];
         double* x_new = a.state[1 - a.ctl->cur];
         double g4[4] = {gs0, gs1, 0.0, 0.0};
@@ -1345,10 +1531,13 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
     }
     }
     if (!a.do_update) continue;
+    if constexpr (kDl) {
+      if (a.n_levels < 2) scope.sync();  // (no back-substitution: CTA 0's dense phase wrote every step)
+      chain_dogleg_update(a, scope, rinv, smem, acc);
+    } else {
     // ---------------------------------------------------------- x (+) step of every frame, one thread each (the top
     // nodes' frames were done with the dense solve); a serial tail per node inside the level loop above cost more than
     // this one barrier
-    {
       const ChainLevel top = a.lev[a.n_levels - 1];
       int ct = 1;  // c^(n_levels - 1): frame of top node t on one GPU
       for (int k = 1; k < a.n_levels; ++k) ct *= kCsChunk;
@@ -1390,11 +1579,13 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
 __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_kernel(ChainSolveArgs a) { chain_solve(a, GridScope()); }
 
 // A batch of rigs, one thread-block cluster each (launched with a cluster dimension; no cooperative launch): cluster k
-// solves args[k].  The arguments are read where they are, through the read-only data path: staged in shared memory they
-// would leave too little of it for the two groups' workspaces of the largest rig that fits (G = 67).
+// solves args[k], an LM or a DOGLEG iteration's solve and update by Str.  The arguments are read where they are, through
+// the read-only data path: staged in shared memory they would leave too little of it for the two groups' workspaces of
+// the largest rig that fits (G = 67).
+template <Strategy Str>
 __global__ void __launch_bounds__(kCsThreads, 1) chain_solve_batch_kernel(const ChainSolveArgs* __restrict__ args) {
   ClusterScope scope;
-  chain_solve(args[blockIdx.x / scope.nb()], scope);
+  chain_solve<ClusterScope, false, false, Str>(args[blockIdx.x / scope.nb()], scope);
 }
 
 // a rig as chain_cov_batch_kernel takes it: the solve's arguments (D2x set, scalars[kScNotPD] zeroed: set where a pivot

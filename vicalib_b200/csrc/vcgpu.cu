@@ -770,6 +770,12 @@ extern "C" int vcgpu_solve_batch_inertial(vcgpu_handle* const* handles, int n, v
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   return run_solve_batch_inertial(handles, n, out);
 }
+extern "C" int vcgpu_calibrate_batch(vcgpu_handle* const* handles, int n, const vcgpu_flow* flow, vcgpu_flow_summary* out,
+                                     double* const* cam_rmse) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!flow) return batch_refuse(handles, n, 0, "null flow", "vcgpu_calibrate_batch");
+  return run_calibrate_batch(handles, n, *flow, out, cam_rmse);
+}
 extern "C" int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int* resident_clusters) {
   if (!h) return VCGPU_ERR_INVALID;
   return imu_batch_plan_of(h, cluster_size, resident_clusters);
