@@ -390,6 +390,36 @@ int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov /* n_frames * fd * f
  * KB of kernel arguments per rig, held by handle 0. */
 int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov /* n pointers */,
                                      int* status /* n, or NULL */);
+/* The frame blocks of (J^T J)^-1 off its block diagonal (ceres::Covariance::GetCovarianceBlock(t_wp[f], globals) and
+ * (t_wp[f], t_wp[f+1]), with v_w the same way when the inertial terms are on), on the system
+ * vcgpu_get_frame_covariance inverts, by the same selected inversion of the frame elimination.
+ * cov_fg: n_frames blocks of fd x G, row-major: Σ[frame f, globals].  Rows follow the frame's rows of
+ *         vcgpu_normal_equations' B; columns follow vcgpu_get_covariance's tangent layout.
+ * cov_fn: n_frames - 1 blocks of fd x fd: Σ[frame f, frame f+1], rows frame f, columns frame f+1.
+ * Either may be NULL, but not both.  With vcgpu_get_frame_covariance's Σ_ff, the covariance of the relative motion of
+ * frames f and f+1 is Σ_ff + Σ_f+1,f+1 - Σ_f,f+1 - Σ_f,f+1^T.  On vision rigs Σ_f,f+1 = X_f Σ_gg X_f+1^T (X_f =
+ * B_f^-1 E_f), off the pattern of J^T J but well defined, so both kinds of rig share one layout.
+ * Exactly 0.0: the columns of constant or unused globals, every row and column of a vision frame no active observation
+ * sees, and the velocity rows and columns of a rotation-only run.  Options play no part.  Nothing on the handle changes:
+ * state, IMU weights and what a later vcgpu_solve computes stay as they were.
+ * VCGPU_ERR_NUMERIC: J^T J is not positive definite at the current state; nothing is written.  VCGPU_ERR_INVALID: a null
+ * handle, both outputs null, or frame shards (the call is one-GPU only).
+ * Device memory, kept on the handle: vision G^2 + n_frames (6 G + 36) doubles; inertial (G + 9 t)^2 + n_frames (9 G + 81)
+ * + about 8/7 n_frames (162 + 9 G) doubles, t <= 4 the nodes of the chain's top level. */
+int vcgpu_get_frame_cross_covariance(vcgpu_handle* h, double* cov_fg /* n_frames * fd * G, or NULL */,
+                                     double* cov_fn /* (n_frames - 1) * fd * fd, or NULL */);
+/* vcgpu_get_frame_cross_covariance of n independent rigs in one call, one thread-block cluster per rig, as
+ * vcgpu_get_frame_covariance_batch runs them; vision and inertial rigs may be mixed.  cov_fg[i] and cov_fn[i] receive rig
+ * i's blocks as vcgpu_get_frame_cross_covariance lays them out, equal to its result to rounding and with the same exact
+ * zeros; each rig takes the cluster size its batch solve takes, so its blocks are the same bits whatever else is in the
+ * batch and in whatever order.  Either array may be NULL (n NULL pointers), and either pointer of a rig may be NULL, but
+ * not both of one rig.  Nothing on the handle changes.
+ * status, VCGPU_ERR_NUMERIC and VCGPU_ERR_INVALID: as vcgpu_get_frame_covariance_batch, each refusal naming the index,
+ * with both pointers of a rig null in place of a null cov[i].
+ * Device memory: per handle the workspace of vcgpu_get_frame_cross_covariance and that of vcgpu_get_covariance_batch,
+ * and a few KB of kernel arguments per rig, held by handle 0. */
+int vcgpu_get_frame_cross_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov_fg /* n pointers, or NULL */,
+                                           double* const* cov_fn /* n pointers, or NULL */, int* status /* n, or NULL */);
 
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */

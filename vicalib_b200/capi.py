@@ -27,6 +27,7 @@ EXPORTS = [
     "vcgpu_set_profiling", "vcgpu_get_stage_times", "vcgpu_fp64_peak", "vcgpu_get_phase_clocks", "vcgpu_get_covariance", "vcgpu_get_covariance_batch",
     "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch", "vcgpu_evaluate_batch", "vcgpu_remove_outliers_batch",
     "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch", "vcgpu_calibrate_batch",
+    "vcgpu_get_frame_cross_covariance", "vcgpu_get_frame_cross_covariance_batch",
 ]
 
 
@@ -361,6 +362,15 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_frame_covariance(self.h, _p(cov)))
         return cov
 
+    def frame_cross_covariance(self):
+        """GetCovarianceBlock(t_wp[f], globals) and (t_wp[f], t_wp[f+1]) of every frame (with v_w likewise when the
+        inertial terms are on): (fg [n_frames, fd, G], fn [n_frames - 1, fd, fd]); rows as frame_covariance()'s,
+        columns of fg as covariance()'s"""
+        fd, nf = self.fd, self.n_frames
+        fg, fn = np.zeros((nf, fd, self.G)), np.zeros((max(nf - 1, 0), fd, fd))
+        self._chk(self.L.vcgpu_get_frame_cross_covariance(self.h, _p(fg), _p(fn)))
+        return fg, fn
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -447,6 +457,30 @@ def frame_covariance_batch(calibrators, out=None):
     if out is None:
         out = [None if g is None else np.zeros((g.n_frames, g.fd, g.fd)) for g in calibrators]
     return _covariances(lib().vcgpu_get_frame_covariance_batch, "frame_covariance_batch", calibrators, out)
+
+
+def frame_cross_covariance_batch(calibrators):
+    """vcgpu_get_frame_cross_covariance_batch: Calibrator.frame_cross_covariance() of every Calibrator of the list
+    (vision and inertial rigs may be mixed), each rig in its own thread-block cluster.  Returns one (fg, fn) per
+    calibrator, in order.  Raises VcgpuError as covariance_batch does; its `covariances` then holds (fg, fn) or None."""
+    n = len(calibrators)
+    L = lib()
+    fg = [None if g is None else np.zeros((g.n_frames, g.fd, g.G)) for g in calibrators]
+    fn = [None if g is None else np.zeros((max(g.n_frames - 1, 0), g.fd, g.fd)) for g in calibrators]
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    pg = (C.c_void_p * max(n, 1))(*[None if a is None else a.ctypes.data for a in fg])
+    pn = (C.c_void_p * max(n, 1))(*[None if a is None else a.ctypes.data for a in fn])
+    status = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_frame_cross_covariance_batch(hs, C.c_int(n), pg, pn, status)
+    out = list(zip(fg, fn))
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:
+            e.status = [status[i] for i in range(n)]
+            e.covariances = [out[i] if status[i] == 0 else None for i in range(n)]
+        raise e
+    return out
 
 
 def _covariances(entry, name, calibrators, out):

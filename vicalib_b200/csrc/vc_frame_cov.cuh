@@ -12,6 +12,9 @@
 //   Σ_py = -M_p Σ_yy,   Σ_pq = K_pq + M_p Σ_yy M_q^T.
 // The walk starts at the inverse of the dense [globals | top nodes] system and goes down the levels; at every level it
 // keeps what the level below needs as its boundary: Σ_kk, Σ_k,k+1 and Σ_kg of every node (SigmaLevel).
+//
+// The blocks off the diagonal (vcgpu_get_frame_cross_covariance) come from the same two routes: vision Σ_fg = -X_f Σ_gg
+// and Σ_f,f+1 = X_f Σ_gg X_f+1^T (frame_cross_cov_block), inertial level 0's Σ_kg and Σ_k,k+1 (frame_cross_cov_out_entry).
 #pragma once
 #include "vc_chain.cuh"
 
@@ -111,6 +114,77 @@ __global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cov_vision_kernel(F
   const Blocks& b = a.b[a.ctl->cur];
   const int G = a.dp.G, M = G + 1;
   frame_cov_block<FD>(b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, a.X + static_cast<int64_t>(f) * FD * M, M, a.Sgg, G, lane, out);
+}
+
+// Frame f's blocks off the diagonal (vcgpu_get_frame_cross_covariance), unscaled, by one warp: P_f = X_f Σ_gg is formed
+// once, and gives Σ_fg = -P_f and Σ_f,f+1 = P_f X_f+1^T (frame_cross_cov_vision_kernel, cov_frame_cross_mega_batch_kernel).
+// Xf, Xn: X_f and X_f+1, [FD][ldx]; Xn null where frame f is the last or frame f+1 unused (its columns of fn are 0, as
+// are the columns of fg where mask[q] is 0).  sf, sn, scg: the Jacobi scales of frames f, f+1 and of the globals.  fn
+// null: frame f is the last.
+template <int FD>
+__device__ __forceinline__ void frame_cross_cov_block(const double* Xf, const double* Xn, int ldx, const double* Sgg, int G,
+                                                      const double* sf, const double* sn, const double* scg, const double* mask,
+                                                      int lane, double* fg, double* fn) {
+  constexpr int kOwn = (FD * FD + 31) / 32;  // entry t of Σ_f,f+1 (row-major) is summed by lane t mod 32
+  const int M = ldx;
+  double own[kOwn];
+#pragma unroll
+  for (int i = 0; i < kOwn; ++i) own[i] = 0.0;
+  for (int q0 = 0; q0 < G; q0 += 32) {  // the lanes split the columns q of P, 32 at a time
+    const int q = q0 + lane;
+    double p[FD];
+#pragma unroll
+    for (int r = 0; r < FD; ++r) p[r] = 0.0;
+    if (q < G) {
+      for (int k = 0; k < G; ++k) {
+        const double s = Sgg[static_cast<int64_t>(k) * G + q];
+#pragma unroll
+        for (int r = 0; r < FD; ++r) p[r] += Xf[r * M + k] * s;
+      }
+      const bool free_q = mask[q] != 0.0;
+      const double sq = scg[q];
+#pragma unroll
+      for (int r = 0; r < FD; ++r) fg[static_cast<int64_t>(r) * G + q] = free_q ? -(p[r] * (sf[r] * sq)) : 0.0;
+    }
+    if (Xn) {  // this tile's share of P X_f+1^T, summed over the warp one entry at a time (few registers held)
+#pragma unroll
+      for (int t = 0; t < FD * FD; ++t) {
+        double v = q < G ? p[t / FD] * Xn[(t % FD) * M + q] : 0.0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((t & 31) == lane) own[t >> 5] += v;
+      }
+    }
+  }
+  if (!fn) return;
+#pragma unroll
+  for (int t = 0; t < FD * FD; ++t)
+    if ((t & 31) == lane) fn[t] = Xn ? own[t >> 5] * (sf[t / FD] * sn[t % FD]) : 0.0;
+}
+
+// the arguments of frame_cross_cov_vision_kernel: f.out is Σ_fg [nf][FD][G]
+struct FrameCrossCovArgs {
+  FrameCovArgs f;
+  const double* mask;  // [G] 0: constant or unused global
+  double* fn;          // [nf - 1][FD][FD] Σ_f,f+1
+};
+template <int FD>
+__global__ void __launch_bounds__(32 * kFrameCovWarps) frame_cross_cov_vision_kernel(FrameCrossCovArgs a) {
+  const int lane = threadIdx.x & 31, f = blockIdx.x * kFrameCovWarps + (threadIdx.x >> 5);
+  const int nf = a.f.dp.n_frames, G = a.f.dp.G, M = G + 1;
+  if (f >= nf) return;
+  double* fg = a.f.out + static_cast<int64_t>(f) * FD * G;
+  double* fn = f + 1 < nf ? a.fn + static_cast<int64_t>(f) * FD * FD : nullptr;
+  if (!a.f.frame_used[f]) {
+    for (int e = lane; e < FD * G; e += 32) fg[e] = 0.0;
+    if (fn)
+      for (int e = lane; e < FD * FD; e += 32) fn[e] = 0.0;
+    return;
+  }
+  const double* Xn = fn && a.f.frame_used[f + 1] ? a.f.X + static_cast<int64_t>(f + 1) * FD * M : nullptr;
+  const double* sf = a.f.scale + static_cast<int64_t>(f) * FD;
+  frame_cross_cov_block<FD>(a.f.X + static_cast<int64_t>(f) * FD * M, Xn, M, a.f.Sgg, G, sf, sf + FD,
+                            a.f.scale + static_cast<int64_t>(nf) * FD, a.mask, lane, fg, fn);
 }
 
 // ---------------------------------------------------------------- inertial: one CTA per chunk of a level
@@ -281,6 +355,35 @@ __global__ void __launch_bounds__(256) frame_cov_out_kernel(int n_frames, int li
   const int64_t e = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (e >= static_cast<int64_t>(n_frames) * FD * FD) return;
   out[e] = frame_cov_out_entry<FD>(e, live, kk, scale);
+}
+
+// Level 0's blocks off the diagonal (vcgpu_get_frame_cross_covariance), unscaled: entry e of Σ_fg [nf][FD][G] (e below
+// nf FD G) or of Σ_f,f+1 [nf - 1][FD][FD] (the entries after).  Rows and columns of a frame from `live` on, and the
+// columns of constant or unused globals (mask 0), are 0.
+template <int FD>
+__device__ __forceinline__ void frame_cross_cov_out_entry(int64_t e, int nf, int G, int live, const SigmaLevel& sig, const double* scale,
+                                                          const double* mask, double* fg, double* fn) {
+  const int64_t ng = static_cast<int64_t>(nf) * FD * G;
+  if (e < ng) {
+    const int64_t f = e / (FD * G);
+    const int r = static_cast<int>((e / G) % FD), q = static_cast<int>(e % G);
+    fg[e] = r < live && mask[q] != 0.0 ? sig.kg[e] * (scale[f * FD + r] * scale[static_cast<int64_t>(nf) * FD + q]) : 0.0;
+  } else {
+    const int64_t k = e - ng, f = k / (FD * FD);
+    const int r = static_cast<int>((k / FD) % FD), c = static_cast<int>(k % FD);
+    fn[k] = r < live && c < live ? sig.kn[k] * (scale[f * FD + r] * scale[(f + 1) * FD + c]) : 0.0;
+  }
+}
+template <int FD>
+__host__ __device__ inline int64_t frame_cross_cov_entries(int nf, int G) {
+  return static_cast<int64_t>(nf) * FD * G + static_cast<int64_t>(nf - 1) * FD * FD;
+}
+template <int FD>
+__global__ void __launch_bounds__(256) frame_cross_cov_out_kernel(int nf, int G, int live, SigmaLevel sig, const double* scale,
+                                                                  const double* mask, double* fg, double* fn) {
+  const int64_t e = static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (e >= frame_cross_cov_entries<FD>(nf, G)) return;
+  frame_cross_cov_out_entry<FD>(e, nf, G, live, sig, scale, mask, fg, fn);
 }
 
 }  // namespace vc

@@ -1600,6 +1600,9 @@ struct ChainCovArgs {
   double* inv;
   double* out;
   int live;
+  // cross mode (chain_frame_cross_cov_batch_kernel): frame mode's, with out Σ_fg [nf][9][G] and out_next Σ_f,f+1
+  // [nf - 1][81]
+  double* out_next;
 };
 // A batch of inertial rigs, one thread-block cluster each: cluster k writes the covariance of args[k] (vcgpu_get_covariance_batch).
 __global__ void __launch_bounds__(kCsThreads, 1) chain_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
@@ -1618,16 +1621,15 @@ __host__ __device__ inline size_t chain_frame_cov_smem_bytes(int G) {
   const size_t solve = chain_solve_smem_doubles(G) * sizeof(double), walk = chain_walk_chunks(G) * chain_selinv_smem_bytes<9>(G, kCsChunk);
   return solve > walk ? solve : walk;
 }
-// A batch of inertial rigs, one thread-block cluster each: cluster k writes the frame covariance of args[k].  The
-// elimination and the dense factorisation of chain_solve; CTA 0's warps solve the N unit right-hand sides (the whole
-// inverse of [globals | top nodes], as dense_solve_kernel's inversion gives it) and leave the top nodes' blocks; then the
-// levels top-down, a cluster barrier between two, their chunks spread over the CTAs (chain_selinv_chunk); then level 0
-// unscaled.
-__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
+// The walk of one inertial rig by its thread-block cluster: the elimination and the dense factorisation of chain_solve;
+// CTA 0's warps solve the N unit right-hand sides (the whole inverse of [globals | top nodes], as dense_solve_kernel's
+// inversion gives it) and leave the top nodes' blocks; then the levels top-down, a cluster barrier between two, their
+// chunks spread over the CTAs (chain_selinv_chunk).  Then out(tid, bid, nb, nf) writes what the call returns from level
+// 0's blocks in a.sig[0].
+template <class Out>
+__device__ __forceinline__ void chain_frame_cov_walk(const ChainCovArgs& a, ClusterScope scope, Out out) {
   extern __shared__ double smem[];
   constexpr int FD = 9;
-  ClusterScope scope;
-  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
   chain_solve<ClusterScope, true, true>(a.s, scope);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, grp = tid / kCsGroup, gtid = tid - grp * kCsGroup;
   const int bid = scope.bid(), nb = scope.nb();
@@ -1685,9 +1687,31 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(co
     }
     scope.sync();
   }
-  const double* kk = a.sig[0].kk;
-  for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < static_cast<int64_t>(nf) * FD * FD; e += static_cast<int64_t>(nb) * kCsThreads)
-    a.out[e] = frame_cov_out_entry<FD>(e, a.live, kk, a.s.scale);
+  out(tid, bid, nb, nf);
+}
+// A batch of inertial rigs, one thread-block cluster each: cluster k writes the frame covariance of args[k], the walk's
+// level 0 Σ_kk unscaled.
+__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
+  constexpr int FD = 9;
+  ClusterScope scope;
+  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
+  chain_frame_cov_walk(a, scope, [&](int tid, int bid, int nb, int nf) {
+    const double* kk = a.sig[0].kk;
+    for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < static_cast<int64_t>(nf) * FD * FD; e += static_cast<int64_t>(nb) * kCsThreads)
+      a.out[e] = frame_cov_out_entry<FD>(e, a.live, kk, a.s.scale);
+  });
+}
+// ... the frame blocks off the diagonal of args[k] (vcgpu_get_frame_cross_covariance_batch): level 0's Σ_kg and
+// Σ_k,k+1 unscaled
+__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cross_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
+  constexpr int FD = 9;
+  ClusterScope scope;
+  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
+  chain_frame_cov_walk(a, scope, [&](int tid, int bid, int nb, int nf) {
+    const int G = a.s.dp.G;
+    for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < frame_cross_cov_entries<FD>(nf, G); e += static_cast<int64_t>(nb) * kCsThreads)
+      frame_cross_cov_out_entry<FD>(e, nf, G, a.live, a.sig[0], a.s.scale, a.mask, a.out, a.out_next);
+  });
 }
 
 }  // namespace vc

@@ -935,6 +935,9 @@ struct CovArgs {
   // blocks of fcov [nf][36] are 0
   const uint8_t* frame_used;
   double* fcov;
+  // cross mode (cov_frame_cross_mega_batch_kernel): frame mode's D2x and frame_used; fcov Σ_fg [nf][6][G], fcov_next
+  // Σ_f,f+1 [nf - 1][36]
+  double* fcov_next;
 };
 // dynamic shared memory of cov_mega_batch_kernel: per warp its frame's scaled [E | g] and X, the reduced system, pivots
 __host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
@@ -943,10 +946,12 @@ __host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
 
 // One vision rig by one thread-block cluster.  Frames are owned as in mega_solve (frame f -> CTA f mod cluster size, warp
 // (f / size) mod warps); every CTA forms and factors the reduced system (the same bits everywhere), then the cluster's
-// warps share the right-hand sides.  kFrames = false: the covariance of the globals.  kFrames = true: all G unit
-// right-hand sides give Σ_gg; after a cluster barrier one warp per frame refactors B_f, forms X_f = B_f^-1 E_f again
-// and writes B_f^-1 + X_f Σ_gg X_f^T (frame_cov_block).
-template <bool kFrames>
+// warps share the right-hand sides.  kCovGlobals: the covariance of the globals.  kCovFrames: all G unit right-hand
+// sides give Σ_gg; after a cluster barrier one warp per frame refactors B_f, forms X_f = B_f^-1 E_f again and writes
+// B_f^-1 + X_f Σ_gg X_f^T (frame_cov_block).  kCovCross: as kCovFrames, but the warp forms X_f and X_f+1 and writes
+// -X_f Σ_gg and X_f Σ_gg X_f+1^T (frame_cross_cov_block).
+enum CovMode { kCovGlobals, kCovFrames, kCovCross };
+template <CovMode kMode>
 __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
   extern __shared__ double smem[];
   constexpr int FD = 6;
@@ -963,11 +968,9 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
   for (int e = tid; e < NS; e += nthreads) S[e] = 0.0;
   if (tid == 0) bad = 0;
   bool frame_bad = false;
-  // this warp's frame f: its damped, scaled block factored in registers, then its scaled [E | 0] and X into the warp's
-  // slots of wmem
-  auto frame_x = [&](int f) {
-    double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
-    double* Xw = Esw + FD * M;
+  // this warp's frame f: its damped, scaled block factored in registers, then its scaled [E | 0] and X into Esw and Xw
+  // (the warp's slots of wmem; kCovCross passes one slot as both, which leaves X there)
+  auto frame_x = [&](int f, double* Esw, double* Xw) {
     const double* sf = a.scale + static_cast<int64_t>(f) * FD;
     const double* Bf = a.b.B + static_cast<int64_t>(f) * FD * FD;
     const double* Ef = a.b.E + static_cast<int64_t>(f) * FD * G;
@@ -1030,7 +1033,8 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
   for (int base = 0; base < nk; base += nwarps) {
     const int k = base + warp;
     __syncthreads();
-    if (k < nk) frame_x(bid + k * nb);
+    double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
+    if (k < nk) frame_x(bid + k * nb, Esw, Esw + FD * M);
     __syncthreads();
     schur_accumulate<FD>(S, wmem, 2 * FD * M, min(nwarps, nk - base), G, tid, nthreads);
   }
@@ -1052,7 +1056,7 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
     if (bid == 0 && tid == 0) *a.notpd = 1.0;
     return;
   }
-  if constexpr (!kFrames) {
+  if constexpr (kMode == kCovGlobals) {
     for (int j = bid * nwarps + warp; j < G; j += nb * nwarps) {
       double x[kCovQ] = {0.0, 0.0, 0.0, 0.0};
       if (a.mask[j] != 0.0) warp_inverse_column<kCovQ, false>(S, G, invd, G, j, lane, x);
@@ -1067,18 +1071,43 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
         if (32 * q + lane < G) a.cov[static_cast<int64_t>(32 * q + lane) * G + j] = x[q];
     }
     scope.sync();
-    for (int k = warp; k < nk; k += nwarps) {
-      const int f = bid + k * nb;
-      double* out = a.fcov + static_cast<int64_t>(f) * FD * FD;
-      if (!a.frame_used[f]) {
-        for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
-        continue;
+    if constexpr (kMode == kCovFrames) {
+      for (int k = warp; k < nk; k += nwarps) {
+        const int f = bid + k * nb;
+        double* out = a.fcov + static_cast<int64_t>(f) * FD * FD;
+        if (!a.frame_used[f]) {
+          for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
+          continue;
+        }
+        double* Esw = wmem + static_cast<size_t>(warp) * 2 * FD * M;
+        frame_x(f, Esw, Esw + FD * M);
+        __syncwarp();
+        const double* Xw = wmem + static_cast<size_t>(warp) * 2 * FD * M + FD * M;
+        frame_cov_block<FD>(a.b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, Xw, M, a.cov, G, lane, out);
+        __syncwarp();
       }
-      frame_x(f);
-      __syncwarp();
-      const double* Xw = wmem + static_cast<size_t>(warp) * 2 * FD * M + FD * M;
-      frame_cov_block<FD>(a.b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, Xw, M, a.cov, G, lane, out);
-      __syncwarp();
+    } else {
+      // X_f into the warp's second slot, X_f+1 (its owner's bits: the same routine on the same inputs) into its first
+      for (int k = warp; k < nk; k += nwarps) {
+        const int f = bid + k * nb;
+        double* fg = a.fcov + static_cast<int64_t>(f) * FD * G;
+        double* fn = f + 1 < nf ? a.fcov_next + static_cast<int64_t>(f) * FD * FD : nullptr;
+        if (!a.frame_used[f]) {
+          for (int e = lane; e < FD * G; e += 32) fg[e] = 0.0;
+          if (fn)
+            for (int e = lane; e < FD * FD; e += 32) fn[e] = 0.0;
+          continue;
+        }
+        double* Xn = wmem + static_cast<size_t>(warp) * 2 * FD * M;
+        double* Xf = Xn + FD * M;
+        frame_x(f, Xf, Xf);
+        const bool next = fn && a.frame_used[f + 1];
+        if (next) frame_x(f + 1, Xn, Xn);
+        __syncwarp();
+        const double* sf = a.scale + static_cast<int64_t>(f) * FD;
+        frame_cross_cov_block<FD>(Xf, next ? Xn : nullptr, M, a.cov, G, sf, sf + FD, scg, a.mask, lane, fg, fn);
+        __syncwarp();
+      }
     }
   }
 }
@@ -1086,12 +1115,17 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
 // A batch of vision rigs, one thread-block cluster each: cluster k writes the covariance of args[k].
 __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_mega_batch_kernel(const CovArgs* __restrict__ args) {
   ClusterScope scope;
-  cov_mega<false>(args[blockIdx.x / scope.nb()], scope);
+  cov_mega<kCovGlobals>(args[blockIdx.x / scope.nb()], scope);
 }
 // ... the frame covariance of args[k] (vcgpu_get_frame_covariance_batch)
 __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_mega_batch_kernel(const CovArgs* __restrict__ args) {
   ClusterScope scope;
-  cov_mega<true>(args[blockIdx.x / scope.nb()], scope);
+  cov_mega<kCovFrames>(args[blockIdx.x / scope.nb()], scope);
+}
+// ... the frame blocks off the diagonal of args[k] (vcgpu_get_frame_cross_covariance_batch)
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_cross_mega_batch_kernel(const CovArgs* __restrict__ args) {
+  ClusterScope scope;
+  cov_mega<kCovCross>(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

@@ -783,7 +783,7 @@ extern "C" int vcgpu_batch_plan_inertial(vcgpu_handle* h, int* cluster_size, int
 extern "C" int vcgpu_get_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_covariance_batch");
-  return run_cov_batch(handles, n, cov, status, false);
+  return run_cov_batch(handles, n, cov, status, kCovGlobals);
 }
 extern "C" int vcgpu_iterate(vcgpu_handle* h, int n, vcgpu_summary* out) {
   if (!h || n <= 0) return VCGPU_ERR_INVALID;
@@ -972,9 +972,10 @@ extern "C" int vcgpu_solve_arrow(vcgpu_handle* h, const double* scale, const dou
 }
 
 // The frames' elimination and the inverse of the system it leaves into w.inv [N*N]: vision: the solve's frame
-// elimination and Schur sum (summed over frame shards), then the inverse of the reduced system [globals].  frames: then
-// the blocks (vc_frame_cov.cuh) into w.out [nf][fd*fd], one warp per frame.
-static int cov_vision(vcgpu_handle* h, const double* D2x, bool frames, const CovSpace& w) {
+// elimination and Schur sum (summed over frame shards), then the inverse of the reduced system [globals].  kCovFrames:
+// then the blocks (vc_frame_cov.cuh) into w.out [nf][fd*fd]; kCovCross: Σ_fg into w.out and Σ_f,f+1 into w.out_next;
+// one warp per frame.
+static int cov_vision(vcgpu_handle* h, const double* D2x, CovMode mode, const CovSpace& w) {
   const DevProblem& dp = h->dp;
   const int G = dp.G;
   VC_TRY(vision_frame_solve(h, D2x));
@@ -985,27 +986,29 @@ static int cov_vision(vcgpu_handle* h, const double* D2x, bool frames, const Cov
   VC_TRY(kernel_smem_optin(h));
   dense_solve_kernel<6><<<1, 256, vc::chain_dense_smem_bytes(G), h->stream>>>(da);
   ++h->launches;
-  if (frames) {
+  if (mode != kCovGlobals) {
     vc::FrameCovArgs fa;
     fa.dp = dp; fa.b[0] = h->blk[0]; fa.b[1] = h->blk[1]; fa.ctl = h->d_ctl; fa.scale = h->d_scale; fa.D2x = D2x; fa.X = h->d_X;
     fa.Sgg = w.inv; fa.frame_used = h->d_frame_used; fa.out = w.out;
-    vc::frame_cov_vision_kernel<6><<<(dp.n_frames + vc::kFrameCovWarps - 1) / vc::kFrameCovWarps, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
+    const int grid = (dp.n_frames + vc::kFrameCovWarps - 1) / vc::kFrameCovWarps;
+    if (mode == kCovFrames) vc::frame_cov_vision_kernel<6><<<grid, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
+    else vc::frame_cross_cov_vision_kernel<6><<<grid, 32 * vc::kFrameCovWarps, 0, h->stream>>>({fa, h->d_mask, w.out_next});
     ++h->launches;
   }
   CUDA_TRY(h, cudaGetLastError());
   return VCGPU_OK;
 }
 // Inertial: the chain elimination, the inverse of [globals | top nodes] (on frame shards: of the ranks' summed
-// partials).  frames: with the top nodes' blocks, then the levels top-down (chain_selinv_kernel); rows and columns
-// from `live` on are 0.
-static int cov_inertial(vcgpu_handle* h, const double* D2x, bool frames, int live, const CovSpace& w) {
+// partials).  Frame modes: with the top nodes' blocks, then the levels top-down (chain_selinv_kernel), then level 0's
+// Σ_kk (kCovFrames) or Σ_kg and Σ_k,k+1 (kCovCross) unscaled; rows and columns from `live` on are 0.
+static int cov_inertial(vcgpu_handle* h, const double* D2x, CovMode mode, int live, const CovSpace& w) {
   constexpr int FD = 9;
   vc::ImuDev* d = imu_dev(h);
   const DevProblem& dp = h->dp;
   const int G = dp.G, nl = static_cast<int>(d->levels.size());
   VC_TRY(imu_chain_eliminate(h, D2x));
-  VC_TRY(imu_chain_dense(h, D2x, w.inv, frames ? &w.sig.back() : nullptr));
-  if (!frames) return VCGPU_OK;
+  VC_TRY(imu_chain_dense(h, D2x, w.inv, mode != kCovGlobals ? &w.sig.back() : nullptr));
+  if (mode == kCovGlobals) return VCGPU_OK;
   const size_t sm = vc::chain_selinv_smem_bytes<FD>(G, kChainC);
   if (nl > 1 && sm > h->selinv_smem_max)
     return fail(h, VCGPU_ERR_INVALID, "frame covariance: G = " + std::to_string(G) + " needs " + std::to_string(sm) +
@@ -1018,18 +1021,26 @@ static int cov_inertial(vcgpu_handle* h, const double* D2x, bool frames, int liv
     vc::chain_selinv_kernel<FD><<<d->levels[l + 1].n, vc::kChainThreads, sm, h->stream>>>(sa);
     ++h->launches;
   }
-  const int64_t ne = static_cast<int64_t>(dp.n_frames) * FD * FD;
-  vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, w.sig[0].kk, h->d_scale, w.out);
+  if (mode == kCovFrames) {
+    const int64_t ne = static_cast<int64_t>(dp.n_frames) * FD * FD;
+    vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, w.sig[0].kk, h->d_scale, w.out);
+  } else {
+    const int64_t ne = vc::frame_cross_cov_entries<FD>(dp.n_frames, G);
+    vc::frame_cross_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, G, live, w.sig[0], h->d_scale,
+                                                                                                  h->d_mask, w.out, w.out_next);
+  }
   ++h->launches;
   CUDA_TRY(h, cudaGetLastError());
   return VCGPU_OK;
 }
 
-// vcgpu_get_covariance (frames false) and vcgpu_get_frame_covariance (frames true) of one handle, the per-handle
-// counterpart of run_cov_batch: cov_prelude, the frames' elimination and one inversion of the system it leaves; the
-// globals' block of that inverse (frames false) or the frames' blocks from it (frames true).  Writes no state buffer.
-static int run_cov(vcgpu_handle* h, double* cov, bool frames) {
+// vcgpu_get_covariance (kCovGlobals), vcgpu_get_frame_covariance (kCovFrames) and vcgpu_get_frame_cross_covariance
+// (kCovCross) of one handle, the per-handle counterpart of run_cov_batch: cov_prelude, the frames' elimination and one
+// inversion of the system it leaves; the globals' block of that inverse, or the frames' blocks from it.  kCovCross:
+// Σ_fg into cov and Σ_f,f+1 into cov_next, either of them null.  Writes no state buffer.
+static int run_cov(vcgpu_handle* h, double* cov, CovMode mode, double* cov_next = nullptr) {
   VC_TRY(prepare(h));
+  const bool frames = mode != kCovGlobals;
   std::vector<double> D2;
   int live = 0;
   VC_TRY(cov_prelude(h, frames, &D2, &live));
@@ -1038,8 +1049,8 @@ static int run_cov(vcgpu_handle* h, double* cov, bool frames) {
   const double* D2x = h->d_scale + nfp + G;
   CUDA_TRY(h, cudaMemsetAsync(h->d_scalars + kScNotPD, 0, sizeof(double), h->stream));
   CovSpace w;
-  int rc = cov_space(h, frames, &w);
-  if (rc == VCGPU_OK) rc = dp.inertial ? cov_inertial(h, D2x, frames, live, w) : cov_vision(h, D2x, frames, w);
+  int rc = cov_space(h, mode, &w);
+  if (rc == VCGPU_OK) rc = dp.inertial ? cov_inertial(h, D2x, mode, live, w) : cov_vision(h, D2x, mode, w);
   h->blocks_valid = false;  // the Jacobi scale is the next solve's to set
   if (rc != VCGPU_OK) return rc;
   std::vector<double> inv(frames ? 0 : G * G), sc(frames ? 0 : G);
@@ -1050,9 +1061,16 @@ static int run_cov(vcgpu_handle* h, double* cov, bool frames) {
   }
   VC_TRY(read_scalars(h));
   if (h->h_scalars[kScNotPD] > 0)
-    return fail(h, VCGPU_ERR_NUMERIC, std::string(frames ? "frame covariance" : "covariance") + ": J^T J is singular at the current state");
-  if (frames) {
+    return fail(h, VCGPU_ERR_NUMERIC, std::string(mode == kCovCross ? "frame cross covariance" : frames ? "frame covariance" : "covariance") +
+                                          ": J^T J is singular at the current state");
+  if (mode == kCovFrames) {
     CUDA_TRY(h, cudaMemcpy(cov, w.out, nfp * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
+    return VCGPU_OK;
+  }
+  if (mode == kCovCross) {
+    if (cov) CUDA_TRY(h, cudaMemcpy(cov, w.out, nfp * G * sizeof(double), cudaMemcpyDeviceToHost));
+    if (cov_next && dp.n_frames > 1)
+      CUDA_TRY(h, cudaMemcpy(cov_next, w.out_next, (nfp - dp.fd) * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
     return VCGPU_OK;
   }
   // as cov_store_column: the lower triangle unscaled by s_i s_j and mirrored; constant or unused globals exactly 0
@@ -1073,7 +1091,7 @@ static int run_cov(vcgpu_handle* h, double* cov, bool frames) {
 // (fill_mask) are zero like ceres::Covariance's.
 extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
-  return run_cov(h, cov, false);
+  return run_cov(h, cov, kCovGlobals);
 }
 
 // Marginal covariance of every frame's tangent (GetCovarianceBlock(t_wp, t_wp) and (v_w, v_w) of ceres::Covariance):
@@ -1082,12 +1100,35 @@ extern "C" int vcgpu_get_covariance(vcgpu_handle* h, double* cov) {
 extern "C" int vcgpu_get_frame_covariance(vcgpu_handle* h, double* cov) {
   if (!h || !cov) return VCGPU_ERR_INVALID;
   if (h->nranks > 1) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_frame_covariance is one-GPU only: frame shards are not supported");
-  return run_cov(h, cov, true);
+  return run_cov(h, cov, kCovFrames);
 }
 extern "C" int vcgpu_get_frame_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov, int* status) {
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!cov) return batch_refuse(handles, n, 0, "null cov array", "vcgpu_get_frame_covariance_batch");
-  return run_cov_batch(handles, n, cov, status, true);
+  return run_cov_batch(handles, n, cov, status, kCovFrames);
+}
+
+// The frame blocks off the block diagonal of (J^T J)^-1 (GetCovarianceBlock(t_wp[f], globals) and (t_wp[f], t_wp[f+1])
+// of ceres::Covariance, with v_w[f] on the inertial path), on the system vcgpu_get_frame_covariance inverts, from the
+// same selected inversion: vision Σ_fg = -X_f Σ_gg and Σ_f,f+1 = X_f Σ_gg X_f+1^T, inertial level 0's Σ_kg and Σ_k,k+1
+// of the level walk (vc_frame_cov.cuh).
+extern "C" int vcgpu_get_frame_cross_covariance(vcgpu_handle* h, double* cov_fg, double* cov_fn) {
+  if (!h) return VCGPU_ERR_INVALID;
+  if (!cov_fg && !cov_fn) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_frame_cross_covariance: cov_fg and cov_fn are both null");
+  if (h->nranks > 1) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_frame_cross_covariance is one-GPU only: frame shards are not supported");
+  return run_cov(h, cov_fg, kCovCross, cov_fn);
+}
+extern "C" int vcgpu_get_frame_cross_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov_fg,
+                                                      double* const* cov_fn, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!cov_fg && !cov_fn) return batch_refuse(handles, n, 0, "null cov_fg and cov_fn arrays", "vcgpu_get_frame_cross_covariance_batch");
+  // one null array stands for n null pointers
+  std::vector<double*> fg(n, nullptr), fn(n, nullptr);
+  for (int i = 0; i < n; ++i) {
+    if (cov_fg) fg[i] = cov_fg[i];
+    if (cov_fn) fn[i] = cov_fn[i];
+  }
+  return run_cov_batch(handles, n, fg.data(), status, kCovCross, fn.data());
 }
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp

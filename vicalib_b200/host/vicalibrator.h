@@ -489,6 +489,25 @@ class ViCalibrator {
     return cov;
   }
 
+  // GetCovarianceBlock(t_wp[f], calibration) and (t_wp[f], t_wp[f+1]) for every frame, with v_w likewise when the
+  // inertial terms are on: *frame_globals gets NumFrames() blocks of fd x G row-major (rows as GetFrameCovariance's,
+  // columns as GetSolutionCovariance's), *frame_next NumFrames() - 1 blocks of fd x fd (rows frame f, columns frame
+  // f+1); either may be null, not both.  With GetFrameCovariance, the covariance of the motion from frame f to f+1 is
+  // S_ff + S_f+1,f+1 - S_f,f+1 - S_f,f+1^T.  Call after the solve has finished (not while IsRunning()).
+  void GetFrameCrossCovariance(std::vector<double>* frame_globals, std::vector<double>* frame_next, int* frame_dim = nullptr,
+                               int* n_globals = nullptr) {
+    int fd = 0, G = 0;
+    Check(vcgpu_frame_dim(h_, &fd), "frame_dim");
+    Check(vcgpu_num_globals(h_, &G), "num_globals");
+    const size_t nf = NumFrames();
+    if (frame_globals) frame_globals->assign(nf * fd * G, 0.0);
+    if (frame_next) frame_next->assign((nf > 0 ? nf - 1 : 0) * fd * fd, 0.0);
+    Check(vcgpu_get_frame_cross_covariance(h_, frame_globals ? frame_globals->data() : nullptr, frame_next ? frame_next->data() : nullptr),
+          "get_frame_cross_covariance");
+    if (frame_dim) *frame_dim = fd;
+    if (n_globals) *n_globals = G;
+  }
+
   // Pose seeds for AddFrame: what VicalibTask::AddSuperFrame computes per frame and camera with
   // calibu::PosePnPRansac(camera, ellipses, target.Circles3D(), ellipse_target_map, 0, 0, &t_cw) and
   // t_wp = t_cw.inverse() * t_ck (src/vicalib-task.cc:322-325, 341-349) — here for ALL views in one device call.
