@@ -114,12 +114,18 @@ const char* vcgpu_last_error(const vcgpu_handle* h);
  * replaces AddParameterBlock / AddResidualBlock (vicalibrator.h:559-604, 628-632, 645-654) */
 int vcgpu_set_cameras(vcgpu_handle* h, int n_cams, const int32_t* model, const double* intr /*n*10*/,
                       const double* q_ck /*n*4*/, const double* p_ck /*n*3*/);
+/* time: absolute stamps on the IMU's clock, Unix time included (the reference stamps frames and samples with the host's
+ * clock by default).  Every time sum is formed in binary64 in the reference's order (t_i + ts, z0.time + dt / 2,
+ * z0.time + dt), and results depend on the stamps only through those roundings: no stamp is rebased or narrowed.  At
+ * current Unix times (2^30 s < t < 2^31 s) a sum t + ts resolves 2^-22 s, so a change of ts below ~1.2e-7 s does not
+ * move the residual although the Jacobian's ts column is not zero.  That is the reference's behaviour. */
 int vcgpu_set_frames(vcgpu_handle* h, int n_frames, const double* T_wp /*n*7*/, const double* v_w /*n*3*/,
                      const double* time /*n*/);
 /* any order; the library groups by (camera, frame) internally and keeps the caller's order for outputs */
 int vcgpu_set_observations(vcgpu_handle* h, int64_t n_obs, const int32_t* frame_id, const int32_t* cam_id,
                            const double* p_w /*n*3*/, const double* p_c /*n*2*/);
-/* strictly increasing timestamps (vicalibrator.h:373-378) */
+/* strictly increasing timestamps (vicalibrator.h:373-378), absolute like vcgpu_set_frames' (Unix time included) and
+ * used as given: the time arithmetic and its rounding are vcgpu_set_frames' */
 int vcgpu_set_imu(vcgpu_handle* h, int n, const double* t, const double* w /*n*3*/, const double* a /*n*3*/,
                   double sigma_g, double sigma_a);
 int vcgpu_set_imu_params(vcgpu_handle* h, const double g[2], const double b[6], const double sf[6], double ts);

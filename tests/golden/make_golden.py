@@ -212,8 +212,8 @@ def get_range(t, w, a, ts, t0, t1):
     return out
 
 
-def imu_residual(t, w, a, t0, t1, R2, p2, v2, R1, p1, v1, g, b, sf, ts, W, switch):
-    p, R, v = integrate(t, w, a, t0, t1, R1, p1, v1, g, b, sf, ts)
+def imu_residual(t, w, a, t0, t1, R2, p2, v2, R1, p1, v1, g, b, sf, ts, W, switch, integrator=None):
+    p, R, v = (integrator or integrate)(t, w, a, t0, t1, R1, p1, v1, g, b, sf, ts)
     Re = R * R2.T
     te = p - Re * p2
     raw = se3_log(Re, te) + list(v - v2)
@@ -275,8 +275,8 @@ def imu_kat(rng):
                 W=W, r=np.array(out_r).reshape(2, nf - 1, 9), J=np.array(out_J).reshape(2, nf - 1, 9, 33))
 
 
-def imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, switches):
-    """residual and exact central-difference 9 x 33 Jacobian of every interval, for each switch value"""
+def imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, switches, integrator=None, jac=True):
+    """residual and exact central-difference 9 x 33 Jacobian (jac) of every interval, for each switch value"""
     nf = len(ftime)
     tm, wm, am = [mp.mpf(float(x)) for x in t], [V(x) for x in w], [V(x) for x in a]
     Wm = M(W)
@@ -291,9 +291,12 @@ def imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, switches):
             def ev(**kw):
                 d = dict(base); d.update(kw)
                 return imu_residual(tm, wm, am, mp.mpf(float(ftime[k])), mp.mpf(float(ftime[k + 1])), d["R2"], d["p2"], d["v2"],
-                                    d["R1"], d["p1"], d["v1"], d["g"], d["b"], d["sf"], d["ts"], Wm, sw)
+                                    d["R1"], d["p1"], d["v1"], d["g"], d["b"], d["sf"], d["ts"], Wm, sw, integrator)
 
             r0 = ev()
+            out_r.append([float(x) for x in r0])
+            if not jac:
+                continue
             cols = []
 
             def fd(kp, km):
@@ -319,7 +322,6 @@ def imu_rows(t, w, a, ftime, q, p, v, g, b, sf, ts, W, switches):
                     lp[j] += h; lm[j] -= h
                     fd({name: lp}, {name: lm})
             fd({"ts": base["ts"] + h}, {"ts": base["ts"] - h})
-            out_r.append([float(x) for x in r0])
             out_J.append(np.array(cols).T)
     return out_r, out_J
 
@@ -434,6 +436,129 @@ def imu_vigorous_kat():
                 J=np.array(out_J).reshape(2, nf - 1, 9, 33))
 
 
+# ------------------------------------------------------------------ IMU at Unix time
+EPOCH = 1_760_000_000.0  # in [2^30, 2^31): one binary64 ulp is 2^-22 s
+EPOCH_RATE = 300.0
+EPOCH_TS = 0.0031
+
+
+class T64:
+    """A time as the reference's Jet<double> carries it: a binary64 scalar part f, which every sum rounds, and an
+    exact part d, the derivative part times (ts - ts0), which never rounds; its value is f + d.  Decisions (which
+    samples an interval takes, zero-length steps) read f alone, as GetElement, GetNext and HasElement read the scalar."""
+
+    def __init__(self, f, d=0):
+        self.f, self.d = float(f), mp.mpf(d)
+
+    @property
+    def v(self):
+        return mp.mpf(self.f) + self.d
+
+    def __add__(self, o):  # the scalar sum rounds to binary64 (Python float)
+        return T64(self.f + o.f, self.d + o.d)
+
+    def __sub__(self, o):  # exact: the stamps here are within a factor 2 of each other (Sterbenz)
+        f = self.f - o.f
+        assert mp.mpf(f) == mp.mpf(self.f) - mp.mpf(o.f)
+        return T64(f, self.d - o.d)
+
+
+def integrate_rounded(t, w, a, t0, t1, R1, p1, v1, g, b, sf, ts):
+    """integrate() with every time sum the reference forms in binary64, in its order: t_i + ts, dt / 2 then
+    z0.time + dt / 2, and z0.time + dt.  ts - ts0 (the perturbation of the ts column's differences) is carried as the
+    exact part, so that each rounded sum s(ts0) continues as s(ts0) + (ts - ts0): the Jet semantics."""
+    ts0 = float(ts)
+    dts = ts - mp.mpf(ts0)
+    assert abs(dts) < mp.mpf(10) ** -20
+    tt = [T64(float(x) + ts0, dts) for x in t]
+    t0, t1 = float(t0), float(t1)
+
+    def interp(time):  # GetElement; no sample ties a frame and the frames lie inside the stream
+        i = max(k for k in range(len(tt)) if tt[k].f <= time)
+        tm = T64(time)
+        fr = (tm - tt[i]).v / (tt[i + 1] - tt[i]).v
+        return (tm, w[i] * (1 - fr) + w[i + 1] * fr, a[i] * (1 - fr) + a[i + 1] * fr)
+
+    assert tt[0].f < t0 and t1 < tt[-1].f
+    meas = [interp(t0)] + [(x, w[k], a[k]) for k, x in enumerate(tt) if t0 < x.f <= t1] + [interp(t1)]
+    gv = gravity_vec(g)
+    bg, ba = mp.matrix(b[:3]), mp.matrix(b[3:])
+    p, R, v = p1, R1, v1
+
+    def deriv(p_, R_, v_, z0, z1, st):
+        al = (z1[0] - (z0[0] + st)).v / (z1[0] - z0[0]).v
+        zg = z0[1] * al + z1[1] * (1 - al)
+        za = z0[2] * al + z1[2] * (1 - al)
+        wv = R_ * mp.matrix([zg[i] * sf[i] + bg[i] for i in range(3)])
+        av = R_ * mp.matrix([za[i] * sf[3 + i] + ba[i] for i in range(3)]) - gv
+        return v_, wv, av
+
+    def step(p_, R_, v_, k, dt):
+        return p_ + k[0] * dt, so3_exp(k[1] * dt) * R_, v_ + k[2] * dt
+
+    for z0, z1 in zip(meas[:-1], meas[1:]):
+        dt = z1[0] - z0[0]
+        if dt.f == 0:
+            continue
+        half = T64(dt.f / 2, dt.d / 2)
+        k1 = deriv(p, R, v, z0, z1, T64(0.0))
+        y1 = step(p, R, v, k1, dt.v / 2)
+        k2 = deriv(*y1, z0, z1, half)
+        y2 = step(p, R, v, k2, dt.v / 2)
+        k3 = deriv(*y2, z0, z1, half)
+        y3 = step(p, R, v, k3, dt.v)
+        k4 = deriv(*y3, z0, z1, dt)
+        k = [k1[i] + 2 * k2[i] + 2 * k3[i] + k4[i] for i in range(3)]
+        p, R, v = step(p, R, v, k, dt.v / 6)
+    return p, R, v
+
+
+def imu_epoch_kat():
+    """The IMU residual at Unix time (tests/golden/imu_epoch_kat.npz, keys of imu_kat.npz with both switch values, and
+    r_exact): a ~300 Hz jittered stream and 7 frames stamped near EPOCH, ts = 0.0031 off the 2^-22 s grid, no sample
+    within 1e-5 s of a frame time.  r and J follow the reference's binary64 time sums (integrate_rounded); r_exact is
+    the same residual with exact sums, at least 1e3 x the KATs' 1e-9 relative bar away from r."""
+    from vicalib_b200.synth import mat_to_quat, quat_mul, so3_exp as np_exp
+    rng = np.random.default_rng(20261019)
+    nf = 7
+    ftime = EPOCH + 0.15 + np.concatenate([[0.0], np.cumsum(rng.uniform(0.03, 0.05, nf - 1))])
+    n = int((ftime[-1] - EPOCH - 0.1) * EPOCH_RATE) + 15
+    t = EPOCH + 0.1 + (np.arange(n) + 0.5 * rng.random(n)) / EPOCH_RATE
+    w = rng.normal(0, 0.4, (n, 3)); a = rng.normal(0, 1.0, (n, 3)) + np.array([0.3, 9.7, 0.5])
+    tt = t + EPOCH_TS
+    assert np.all(np.diff(t) > 0) and tt[0] < ftime[0] and tt[-1] > ftime[-1]
+    assert np.abs(tt[:, None] - ftime[None, :]).min() > 1e-5  # no sample near a frame time: no ts kink
+    assert np.mean((t + EPOCH_TS) - t != EPOCH_TS) >= 0.9  # the sums t_i + ts round
+    g = np.array([0.05, -0.03]); b = np.concatenate([rng.normal(0, 1e-2, 3), rng.normal(0, 1e-1, 3)])
+    sf = 1 + 0.02 * rng.normal(size=6)
+    W = 500 * np.eye(9) + 20 * rng.normal(size=(9, 9))
+    # each frame near the exact integration of the one before, so that |r| is small beside the rounding's effect on it
+    q = np.zeros((nf, 4)); p = np.zeros((nf, 3)); v = np.zeros((nf, 3))
+    q[0] = np_exp(rng.normal(0, 0.5, 3)); p[0] = rng.normal(0, 0.3, 3); v[0] = rng.normal(0, 0.5, 3)
+    tm, wm, am = [mp.mpf(float(x)) for x in t], [V(x) for x in w], [V(x) for x in a]
+    mpl = lambda x: [mp.mpf(float(y)) for y in x]  # noqa: E731
+    for k in range(nf - 1):
+        pe, Re, ve = integrate(tm, wm, am, mp.mpf(float(ftime[k])), mp.mpf(float(ftime[k + 1])), quat_R(q[k]), V(p[k]),
+                               V(v[k]), mpl(g), mpl(b), mpl(sf), mp.mpf(EPOCH_TS))
+        qe = mat_to_quat(np.array(Re.tolist(), dtype=np.float64))
+        qe = qe if qe @ q[k] >= 0 else -qe
+        q[k + 1] = quat_mul(qe, np_exp(0.02 * rng.normal(size=3)))
+        p[k + 1] = np.array([float(x) for x in pe]) + 0.002 * rng.normal(size=3)
+        v[k + 1] = np.array([float(x) for x in ve]) + 0.005 * rng.normal(size=3)
+    out_r, out_J = imu_rows(t, w, a, ftime, q, p, v, g, b, sf, EPOCH_TS, W, (0,), integrator=integrate_rounded)
+    r_exact, _ = imu_rows(t, w, a, ftime, q, p, v, g, b, sf, EPOCH_TS, W, (0,), jac=False)
+    r0, J0, rx = np.array(out_r), np.array(out_J), np.array(r_exact)
+    rot = [0, 1, 2, 6, 7, 8]  # rotation_only zeroes these residual rows (imu_residual's switch)
+    r1, J1, rx1 = r0.copy(), J0.copy(), rx.copy()
+    r1[:, rot], J1[:, rot], rx1[:, rot] = 0.0, 0.0, 0.0
+    r, J, rx = np.stack([r0, r1]), np.stack([J0, J1]), np.stack([rx, rx1])
+    sep = [np.abs(r[s] - rx[s]).max() / np.abs(r[s]).max() for s in (0, 1)]
+    print(f"epoch: |r| max {np.abs(r0).max():.3g}, |r - r_exact| / |r| {sep[0]:.2e} / {sep[1]:.2e}", flush=True)
+    assert min(sep) >= 1e3 * 1e-9, sep
+    return dict(imu_t=t, imu_w=w, imu_a=a, ftime=ftime, T_wp=np.concatenate([q, p], 1), v_w=v, g=g, b=b, sf=sf,
+                ts=np.array(EPOCH_TS), W=W, r=r, J=J, r_exact=rx)
+
+
 def edge_kat():
     """Branch and boundary cases of the camera models (each model's own small-argument branches, the image
     centre, the image border).  Written to reproj_edge_kat.npz with the keys of reproj_kat.npz."""
@@ -468,6 +593,9 @@ if __name__ == "__main__":
         sys.exit(0)
     if "--imu-vigorous" in sys.argv:  # only the vigorous-motion fixture (the others are unchanged)
         np.savez_compressed(os.path.join(HERE, "imu_vigorous_kat.npz"), **imu_vigorous_kat())
+        sys.exit(0)
+    if "--imu-epoch" in sys.argv:  # only the Unix-time fixture (the others are unchanged)
+        np.savez_compressed(os.path.join(HERE, "imu_epoch_kat.npz"), **imu_epoch_kat())
         sys.exit(0)
     rng = np.random.default_rng(20260924)
     out = {}
