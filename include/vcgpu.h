@@ -427,6 +427,37 @@ int vcgpu_get_frame_cross_covariance(vcgpu_handle* h, double* cov_fg /* n_frames
 int vcgpu_get_frame_cross_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov_fg /* n pointers, or NULL */,
                                            double* const* cov_fn /* n pointers, or NULL */, int* status /* n, or NULL */);
 
+/* Each IMU interval's Mahalanobis distance, as UpdateImuWeights computes it and logs it against chi2inv(0.95, 9) =
+ * 16.9190 (vicalibrator.h:786-794): per interval k (n_frames - 1 of them),
+ *   r = [SE3::log(T_end * T_w,k+1^-1) (upsilon 3, omega 3); v_end - v_w[k+1]]   (the reference's `residuals`)
+ *   dist[k] = r^T (Jt C Jt^T)^-1 r
+ * where T_end, v_end and C are the interval's integrated end pose, velocity and covariance and Jt the Jacobian of r, the
+ * same RK4 covariance chain, Jt and symmetrised P = Jt C Jt^T the weight update forms.  P = V diag(lambda) V^T by the
+ * weight update's cyclic Jacobi sweeps, started from the identity; dist[k] = sum_k (V[:,k] . r)^2 / lambda_k, summed in
+ * k order.  r_or_null: NULL, or (n_frames - 1) * 9 doubles.  Reading it against 16.919 is an observation: the reference's
+ * covariance chain is approximate, and whether the distances follow chi-square with 9 degrees of freedom is not known.
+ * NaN: dist[k] and r[k] of an interval with no measurements (the reference skips it and logs nothing); dist[k] where
+ * some lambda_k <= 0 (there the weight update leaves the interval's weight as it is).
+ * Evaluated at the handle's current accepted state, with its IMU parameters, sigmas and time offset; after a solve that
+ * ended on an accepted step, that is the state of the reference's last UpdateImuWeights log.  Runs whenever the inertial
+ * terms are on, rotation-only included, though the reference runs no weight update in a rotation-only stage.  Nothing on
+ * the handle changes: state, IMU weights, the weight update's stored eigenvectors and what a later vcgpu_solve or batch
+ * computes stay as they were.  Runs as vcgpu_get_imu_mahalanobis_batch of this handle alone: the same refusals and memory.
+ * VCGPU_ERR_INVALID: a null handle or dist, inertial terms off, fewer than two frames, or frame shards (one GPU only). */
+int vcgpu_get_imu_mahalanobis(vcgpu_handle* h, double* dist /* n_frames - 1 */, double* r_or_null /* (n_frames - 1) * 9 */);
+/* vcgpu_get_imu_mahalanobis of n rigs in one call: dist[i] and r[i] receive rig i's values, the bits
+ * vcgpu_get_imu_mahalanobis(handles[i]) writes whatever else is in the batch and in whatever order (each interval reads
+ * only its own rig).  r: NULL, or n pointers of which any may be NULL.  Per handle, on its own stream, the uploads of
+ * the handle; then one launch over every interval of every rig (a team of 16 threads per interval) and one download of
+ * every output, on handle 0's stream.
+ * Returns VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in
+ * vcgpu_last_error of every non-null handle, for: n <= 0, a null dist, a null or repeated handle, a null dist[i], handles
+ * on different devices, and a handle vcgpu_get_imu_mahalanobis refuses.
+ * Device memory, held by handle 0 and grown to the largest batch, never freed per call: 80 bytes per interval of
+ * outputs and 104 bytes per rig of kernel arguments. */
+int vcgpu_get_imu_mahalanobis_batch(vcgpu_handle* const* handles, int n, double* const* dist /* n pointers */,
+                                    double* const* r /* n pointers, or NULL; an entry may be NULL */);
+
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */
 /* loss-free residuals and tangent-space Jacobians per observation, caller order.

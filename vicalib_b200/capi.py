@@ -28,7 +28,10 @@ EXPORTS = [
     "vcgpu_get_frame_covariance", "vcgpu_get_frame_covariance_batch", "vcgpu_evaluate_batch", "vcgpu_remove_outliers_batch",
     "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch", "vcgpu_calibrate_batch",
     "vcgpu_get_frame_cross_covariance", "vcgpu_get_frame_cross_covariance_batch",
+    "vcgpu_get_imu_mahalanobis", "vcgpu_get_imu_mahalanobis_batch",
 ]
+
+CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
 
 
 class Flags(C.Structure):
@@ -371,6 +374,17 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_frame_cross_covariance(self.h, _p(fg), _p(fn)))
         return fg, fn
 
+    def imu_mahalanobis(self, residuals=False):
+        """Each IMU interval's Mahalanobis distance as UpdateImuWeights logs it against CHI2_95_9 (vicalibrator.h:786-794),
+        at the current state: (n_frames - 1,) distances, NaN where an interval has no measurements or its covariance
+        is not positive definite; residuals=True also returns the reference's 9-vector residuals, (n_frames - 1, 9)
+        (NaN rows without measurements).  Nothing on the handle changes."""
+        n = max(self.n_frames - 1, 0)
+        d = np.zeros(max(n, 1))
+        r = np.zeros((max(n, 1), 9)) if residuals else None
+        self._chk(self.L.vcgpu_get_imu_mahalanobis(self.h, _p(d), _p(r)))
+        return (d[:n], r[:n]) if residuals else d[:n]
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -481,6 +495,24 @@ def frame_cross_covariance_batch(calibrators):
             e.covariances = [out[i] if status[i] == 0 else None for i in range(n)]
         raise e
     return out
+
+
+def imu_mahalanobis_batch(calibrators, residuals=False):
+    """vcgpu_get_imu_mahalanobis_batch: Calibrator.imu_mahalanobis() of every Calibrator of the list in one launch; each
+    rig's values are the bits its own call returns.  Returns one distance array per calibrator, in order, or with
+    residuals=True one (distances, residuals) pair."""
+    n = len(calibrators)
+    L = lib()
+    ni = [0 if g is None else max(g.n_frames - 1, 0) for g in calibrators]
+    d = [np.zeros(max(k, 1)) for k in ni]
+    r = [np.zeros((max(k, 1), 9)) for k in ni] if residuals else None
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    dp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in d])
+    rp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in r]) if residuals else None
+    _batch_check(L, L.vcgpu_get_imu_mahalanobis_batch(hs, C.c_int(n), dp, rp), calibrators)
+    if residuals:
+        return [(d[i][: ni[i]], r[i][: ni[i]]) for i in range(n)]
+    return [d[i][: ni[i]] for i in range(n)]
 
 
 def _covariances(entry, name, calibrators, out):

@@ -325,8 +325,15 @@ constexpr int kWtTeams = kWtWarps * (32 / kTeam);        // intervals per CTA
 // `on` team-uniform.  Writes the 9x9 weight_sqrt_ to `out` (left untouched when the information matrix is singular).
 // `vec` holds the interval's eigenvectors from its last update (all NaN: none, start from the identity); the
 // eigen-decomposition starts from them and leaves its own there.
+// kMeasure: the interval's Mahalanobis distance instead (vicalibrator.h:786-794), from the same P and the same Jacobi
+// sweeps, always from the identity; `vec` is not touched.  Writes to `out` (null: a tail team, nothing) kMahalOut doubles:
+// the residual r = [se3_log(t12) (upsilon, omega); v_end - v2] and d = sum_k (V[:,k] . r)^2 / lambda_k, summed by one
+// lane in k order; d is NaN where some lambda_k <= 0 (there the weight update leaves W as it is), and all ten are NaN
+// without measurements (!on).
+constexpr int kMahalOut = 10;
+template <bool kMeasure = false>
 __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const double* X2, Work* W, int tl, bool on, double* out,
-                                                double* vec) {
+                                                double* vec, const double* v2 = nullptr) {
   // t12 = T_end * T_2w, T_2w = T_w2^-1
   const Quat<double> q2i = imu::qconj(Quat<double>{X2[0], X2[1], X2[2], X2[3]});
   const Vec<double> t2 = imu::qrot(q2i, Vec<double>{X2[4], X2[5], X2[6]});
@@ -372,14 +379,16 @@ __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const dou
   // eigenvectors of its last update, V_prev, with A = V_prev^T sym(P) V_prev — nearly diagonal when the state moved
   // little.  Without them (NaN: after an upload, a weights upload, a flag change, at the start of a solve) V starts as
   // the identity, and the products below are exact: A = sym(P) bit for bit.
-  bool cold = false;
-  if (on)
-    for (int e = tl; e < 81; e += kTeam) {
-      const double v = vec[e];
-      cold = cold || v != v;
-      V[e] = v;
-    }
-  cold = ((__ballot_sync(0xffffffffu, cold) >> (threadIdx.x & 16)) & 0xffffu) != 0;  // any lane of this team
+  bool cold = kMeasure;
+  if constexpr (!kMeasure) {
+    if (on)
+      for (int e = tl; e < 81; e += kTeam) {
+        const double v = vec[e];
+        cold = cold || v != v;
+        V[e] = v;
+      }
+    cold = ((__ballot_sync(0xffffffffu, cold) >> (threadIdx.x & 16)) & 0xffffu) != 0;  // any lane of this team
+  }
   if (on && cold)
     for (int e = tl; e < 81; e += kTeam) V[e] = (e % 10 == 0) ? 1.0 : 0.0;
   __syncwarp();
@@ -462,6 +471,40 @@ __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const dou
       __syncwarp();
     }
   }
+  if constexpr (kMeasure) {
+    if (!out) return;
+    const double nan = __longlong_as_double(0x7ff8000000000000ll);
+    if (!on) {
+      if (tl < kMahalOut) out[tl] = nan;
+      return;
+    }
+    double* r = W->t1;  // r (9), then z_k = V[:,k] . r (9)
+    if (tl == 0) {
+      imu::se3_log<double>(q12, t12, r);
+      r[6] = y.v.x - v2[0]; r[7] = y.v.y - v2[1]; r[8] = y.v.z - v2[2];
+    }
+    __syncwarp(0xffffu << (threadIdx.x & 16));  // this team only: the other one may have left
+    if (tl < 9) {
+      double z = 0.0;
+#pragma unroll
+      for (int i = 0; i < 9; ++i) z += V[i * 9 + tl] * r[i];
+      r[9 + tl] = z;
+      out[tl] = r[tl];
+    }
+    __syncwarp(0xffffu << (threadIdx.x & 16));
+    if (tl == 0) {
+      double d = 0.0;
+      bool pd = true;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) {
+        const double l = A[k * 9 + k];
+        pd = pd && l > 0.0;
+        d += r[9 + k] * r[9 + k] / l;
+      }
+      out[9] = pd ? d : nan;
+    }
+    return;
+  }
   if (!on) return;
   for (int e = tl; e < 81; e += kTeam) vec[e] = V[e];  // the next update of this interval starts from them
   bool singular = false;
@@ -479,8 +522,9 @@ __device__ __forceinline__ void weight_from_cov(const Pose<double>& y, const dou
   }
 }
 
-// UpdateImuWeights for interval kk by the team of 16 lanes `tl` belongs to (kk >= ni: the team idles along)
-template <class A>
+// UpdateImuWeights for interval kk by the team of 16 lanes `tl` belongs to (kk >= ni: the team idles along).
+// kMeasure: the interval's Mahalanobis distance into a.out instead (weight_from_cov)
+template <bool kMeasure = false, class A>
 __device__ __forceinline__ void imu_weights_team(const A& a, const double* state, int kk, Work* W, int tl) {
   const int ki = min(kk, a.ni - 1);  // an odd tail team shadows the last interval (never written)
   const double* X1 = state + 7 * static_cast<int64_t>(ki);
@@ -511,7 +555,11 @@ __device__ __forceinline__ void imu_weights_team(const A& a, const double* state
     y = integrate_imu_cov(y, prev, cur, bg, ba, sf, g, sg2, sa2, W, tl, step);
     if (step) prev = cur;
   }
-  weight_from_cov(y, X2, W, tl, on, a.wsqrt + static_cast<int64_t>(ki) * 81, a.wsqrt + static_cast<int64_t>(a.ni + ki) * 81);
+  if constexpr (kMeasure)
+    weight_from_cov<true>(y, X2, W, tl, on, kk < a.ni ? a.out + static_cast<int64_t>(kk) * kMahalOut : nullptr, nullptr,
+                          state + a.dp.off_v + 3 * static_cast<int64_t>(ki + 1));
+  else
+    weight_from_cov(y, X2, W, tl, on, a.wsqrt + static_cast<int64_t>(ki) * 81, a.wsqrt + static_cast<int64_t>(a.ni + ki) * 81);
 }
 
 __global__ void __launch_bounds__(32 * kWtWarps, 2) imu_weights_kernel(WeightArgs a) {
@@ -527,6 +575,34 @@ __global__ void __launch_bounds__(32 * kWtWarps, 2) imu_weights_kernel(WeightArg
   }
   if (blockIdx.x * kWtTeams + (threadIdx.x >> 5) * (32 / kTeam) >= a.ni) return;  // whole warp past the end
   imu_weights_team(a, a.states[a.ctl->cur], blockIdx.x * kWtTeams + team, &work[team], tl);
+}
+
+// vcgpu_get_imu_mahalanobis(_batch): one rig's entry in the argument table.  Its intervals take teams [team0, team0 +
+// ni rounded up to even): a warp never holds two rigs, and interval k keeps its warp mate k ^ 1 whatever the batch.
+struct MahalRig {
+  struct { int64_t off_v, off_imu; } dp;  // the state layout imu_weights_team reads
+  imu::ImuBuf buf;
+  const double* ftime;
+  const double* state;  // the accepted state
+  double* out;          // [ni][kMahalOut]
+  int ni, team0;
+  double sigma_g, sigma_a;
+};
+// The distances of every interval of n_rigs rigs, imu_weights_kernel's launch shape; teams: the table's total
+__global__ void __launch_bounds__(32 * kWtWarps, 2) imu_mahalanobis_kernel(const MahalRig* rigs, int n_rigs, int teams) {
+  __shared__ Work work[kWtTeams];
+  const int tl = threadIdx.x & (kTeam - 1);
+  const int t = blockIdx.x * kWtTeams + threadIdx.x / kTeam;
+  const int t0 = blockIdx.x * kWtTeams + (threadIdx.x >> 5) * (32 / kTeam);  // the warp's first team
+  if (t0 >= teams) return;  // whole warp past the end
+  int lo = 0, hi = n_rigs - 1;  // the warp's rig: the last with team0 <= t0
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (rigs[mid].team0 <= t0) lo = mid;
+    else hi = mid - 1;
+  }
+  const MahalRig& a = rigs[lo];
+  imu_weights_team<true>(a, a.state, t - a.team0, &work[threadIdx.x / kTeam], tl);
 }
 
 }  // namespace wts

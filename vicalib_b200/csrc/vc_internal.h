@@ -201,6 +201,8 @@ struct vcgpu_handle {
   // (d_pnp), and the packed inputs and outputs in page-locked host memory (h_pnp) (vc_batch.inl: run_pnp_batch)
   unsigned char* d_pnp = nullptr;
   std::vector<unsigned char, PinnedAlloc<unsigned char>> h_pnp;
+  // vcgpu_get_imu_mahalanobis(_batch) with this handle as handle 0: every rig's [ni][10] outputs (vc_batch.inl)
+  double* d_mahal = nullptr;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

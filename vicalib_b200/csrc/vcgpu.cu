@@ -220,7 +220,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -1177,6 +1177,18 @@ extern "C" int vcgpu_set_imu_weights(vcgpu_handle* h, const double* w) {
   if (h->n_frames < 2 || !h->d_wsqrt) return VCGPU_OK;
   CUDA_TRY(h, cudaMemcpy(h->d_wsqrt, w, static_cast<size_t>(h->n_frames - 1) * 81 * sizeof(double), cudaMemcpyHostToDevice));
   return VCGPU_OK;
+}
+
+// Each IMU interval's Mahalanobis distance as UpdateImuWeights logs it (vicalibrator.h:786-794): run_imu_mahalanobis_batch
+// of this handle alone
+extern "C" int vcgpu_get_imu_mahalanobis(vcgpu_handle* h, double* dist, double* r_or_null) {
+  if (!h) return VCGPU_ERR_INVALID;
+  return run_imu_mahalanobis_batch(&h, 1, &dist, &r_or_null, "vcgpu_get_imu_mahalanobis");
+}
+extern "C" int vcgpu_get_imu_mahalanobis_batch(vcgpu_handle* const* handles, int n, double* const* dist, double* const* r) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!dist) return batch_refuse(handles, n, 0, "null dist array", "vcgpu_get_imu_mahalanobis_batch");
+  return run_imu_mahalanobis_batch(handles, n, dist, r, "vcgpu_get_imu_mahalanobis_batch");
 }
 
 extern "C" int vcgpu_comm_unique_id(uint8_t id[VCGPU_UNIQUE_ID_BYTES]) {

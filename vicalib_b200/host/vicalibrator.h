@@ -508,6 +508,17 @@ class ViCalibrator {
     if (n_globals) *n_globals = G;
   }
 
+  // The Mahalanobis distance UpdateImuWeights logs for each IMU interval against chi2inv(0.95, 9) = 16.919
+  // (vicalibrator.h:786-794), at the current solution: NumFrames() - 1 entries, NaN for an interval with no measurements
+  // (the reference logs nothing there) or whose covariance is not positive definite.  The inertial terms must be on.
+  // Call after the solve has finished (not while IsRunning()).
+  std::vector<double> GetImuMahalanobis() {
+    const size_t nf = NumFrames();
+    std::vector<double> dist(nf > 1 ? nf - 1 : 0, 0.0);
+    Check(vcgpu_get_imu_mahalanobis(h_, dist.data(), nullptr), "get_imu_mahalanobis");
+    return dist;
+  }
+
   // Pose seeds for AddFrame: what VicalibTask::AddSuperFrame computes per frame and camera with
   // calibu::PosePnPRansac(camera, ellipses, target.Circles3D(), ellipse_target_map, 0, 0, &t_cw) and
   // t_wp = t_cw.inverse() * t_ck (src/vicalib-task.cc:322-325, 341-349) — here for ALL views in one device call.
