@@ -584,9 +584,61 @@ def edge_kat():
     np.savez_compressed(os.path.join(HERE, "reproj_edge_kat.npz"), **out)
 
 
+# ------------------------------------------------------------------ wide-angle and fisheye lenses
+KB4_FISHEYE = [0.04, -0.02, 0.005, -0.0005]  # d(theta) monotone to ~139 degrees
+POLY2_BARREL = [-0.32, 0.04]                 # fold (first maximum of r f(r^2)) at r = 1.236
+POLY3_BARREL = [-0.3, 0.06, -0.005]          # fold at r = 1.932
+WIDE_KB4_THETA = [10.0, 45.0, 80.0, 89.9, 90.0, 95.0, 100.0]  # degrees; 90 exactly: Z = 0
+WIDE_FOV_W = [0.9, 1.2]
+WIDE_FOV_RAD = [1e-3, 0.1, 0.5, 1.0, 2.0, 3.5, float(np.tan(np.radians(80.0)))]
+WIDE_POLY_RAD = {POLY2: [0.05, 0.4, 0.8, 1.1, 1.2], POLY3: [0.05, 0.6, 1.2, 1.6, 1.85]}
+WIDE_LINEAR_RAD = [0.5, 1.5, 2.2, 3.0]
+
+
+def wide_kat():
+    """The camera models far from the axis (tests/golden/reproj_wide_kat.npz, keys of reproj_kat.npz): KB4 at fisheye
+    distortion at WIDE_KB4_THETA, behind the image plane included; FOV at both WIDE_FOV_W from rad = 1e-3 (its small-
+    argument branch) to tan 80 degrees; strong barrel poly2 / poly3 up to 0.97 of the fold; linear to rad = 3.  The
+    90-degree KB4 row has identity poses, so that Z is exactly 0 in binary64 as in mpmath."""
+    rng = np.random.default_rng(20261020)
+    out = {}
+
+    def ray(rad, scale=0.5):
+        phi = rng.uniform(0, 2 * np.pi)
+        return [scale * rad * np.cos(phi), scale * rad * np.sin(phi), scale]
+
+    def kb4_samples():
+        for th in WIDE_KB4_THETA:
+            if th == 90.0:
+                s = random_sample(rng, KB4, tgt=[0.3, -0.4, 0.0], dist=KB4_FISHEYE)
+                ident = np.array([0.0, 0.0, 0.0, 1.0])
+                _, _, _, _, intr, _, z = s
+                yield ident, np.zeros(3), ident, np.zeros(3), intr, np.array([0.3, -0.4, 0.0]), z
+                continue
+            phi, t = rng.uniform(0, 2 * np.pi), np.radians(th)
+            yield random_sample(rng, KB4, tgt=0.5 * np.array([np.sin(t) * np.cos(phi), np.sin(t) * np.sin(phi),
+                                                                 np.cos(t)]), dist=KB4_FISHEYE)
+
+    cases = {
+        "kb4": (KB4, list(kb4_samples())),
+        "fov": (FOV, [random_sample(rng, FOV, tgt=ray(r), dist=[w]) for w in WIDE_FOV_W for r in WIDE_FOV_RAD]),
+        "poly2": (POLY2, [random_sample(rng, POLY2, tgt=ray(r), dist=POLY2_BARREL) for r in WIDE_POLY_RAD[POLY2]]),
+        "poly3": (POLY3, [random_sample(rng, POLY3, tgt=ray(r), dist=POLY3_BARREL) for r in WIDE_POLY_RAD[POLY3]]),
+        "linear": (LINEAR, [random_sample(rng, LINEAR, tgt=ray(r)) for r in WIDE_LINEAR_RAD]),
+    }
+    for name, (model, samples) in cases.items():
+        for k, v in reproj_kat(rng, model, samples=samples).items():
+            out[f"{name}_{k}"] = v
+        print(name, "wide done", flush=True)
+    return out
+
+
 if __name__ == "__main__":
     if "--edge" in sys.argv:  # only the branch / boundary fixture (the others are unchanged)
         edge_kat()
+        sys.exit(0)
+    if "--wide" in sys.argv:  # only the wide-angle / fisheye fixture (the others are unchanged)
+        np.savez_compressed(os.path.join(HERE, "reproj_wide_kat.npz"), **wide_kat())
         sys.exit(0)
     if "--imu-edge" in sys.argv:  # only the interpolation-buffer edge fixture (the others are unchanged)
         np.savez_compressed(os.path.join(HERE, "imu_edge_kat.npz"), **imu_edge_kat())

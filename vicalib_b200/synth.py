@@ -254,6 +254,12 @@ def make_problem(
     imu_noise=True,
     spacing=None,
     motion="gentle",  # "gentle" (the default trajectory) or "vigorous" (_vigorous_cam0_pose)
+    focal=None,  # truth focal length in pixels, one or one per camera (default 320), each drawn within +-5 %
+    dist=None,  # truth distortion, one list per camera (default TRUTH_DIST of its model)
+    standoff=None,  # (mean, amplitude) of camera 0's distance from the grid plane in metres (default (0.47, 0.11))
+    tilt=None,  # (mean, amplitude) in radians of camera 0's turn away from the grid, about an axis that rotates
+    #             in the image plane: the grid moves from the image centre towards the rim (default: no turn)
+    cull=False,  # drop corners outside the image, and (every model but KB4) corners not in front of the camera
 ) -> Problem:
     rng = np.random.default_rng(seed)
     models = np.array([MODEL_IDS[m] if isinstance(m, str) else int(m) for m in models], dtype=np.int32)
@@ -268,11 +274,15 @@ def make_problem(
 
     # ---- truth intrinsics / extrinsics
     intr_t = np.zeros((n_cams, 10))
+    focals = np.broadcast_to(np.asarray(320.0 if focal is None else focal, dtype=np.float64), (n_cams,))
     for c, m in enumerate(models):
-        f = 320.0 * (1 + 0.05 * rng.uniform(-1, 1))
+        f = focals[c] * (1 + 0.05 * rng.uniform(-1, 1))
         intr_t[c, :4] = [f, f * (1 + 0.002 * rng.uniform(-1, 1)), width / 2 + rng.uniform(-5, 5),
                          height / 2 + rng.uniform(-5, 5)]
-        intr_t[c, 4:4 + len(TRUTH_DIST[int(m)])] = TRUTH_DIST[int(m)]
+        d = TRUTH_DIST[int(m)] if dist is None else dist[c]
+        if len(d) != NUM_INTR[int(m)] - 4:
+            raise ValueError(f"camera {c}: {len(d)} distortion parameters for model {int(m)}")
+        intr_t[c, 4:4 + len(d)] = d
     R_rdf = np.array([[0.0, 1, 0], [0, 0, 1], [1, 0, 0]])  # RdfRobotics (vi_sim_test.cpp:71-74)
     q_ck_t = np.zeros((n_cams, 4))
     p_ck_t = np.zeros((n_cams, 3))
@@ -293,6 +303,18 @@ def make_problem(
     fr = 2 * np.pi * np.array([0.31, 0.23, 0.17, 0.41, 0.29, 0.13, 0.37, 0.19])
     if motion not in ("gentle", "vigorous"):
         raise ValueError(motion)
+    if motion == "vigorous" and (standoff is not None or tilt is not None):
+        raise ValueError("standoff and tilt shape the gentle trajectory only")
+    d0, d1 = (0.47, 0.11) if standoff is None else standoff
+
+    def turned(R, t):
+        """R turned by tilt about an image-plane axis whose direction rotates with time"""
+        if tilt is None:
+            return R
+        phi = fr[6] * t + ph[6]
+        ang = tilt[0] + tilt[1] * np.sin(fr[7] * t + ph[7])
+        axis = np.stack([np.cos(phi), np.sin(phi), np.zeros_like(phi)], -1)
+        return R @ quat_to_mat(so3_exp(ang[..., None] * axis))
 
     def cam0_pose(t):
         if motion == "vigorous":
@@ -302,7 +324,7 @@ def make_problem(
             [
                 centre[0] + 0.16 * np.sin(fr[0] * t + ph[0]),
                 centre[1] + 0.12 * np.sin(fr[1] * t + ph[1]),
-                -(0.47 + 0.11 * np.sin(fr[2] * t + ph[2])),
+                -(d0 + d1 * np.sin(fr[2] * t + ph[2])),
             ],
             -1,
         )
@@ -315,7 +337,7 @@ def make_problem(
             -1,
         )
         roll = 0.35 * np.sin(fr[5] * t + ph[5])
-        return _look_at(pos, tgt, roll), pos
+        return turned(_look_at(pos, tgt, roll), t), pos
 
     R_ck0 = quat_to_mat(q_ck_t[0])
 
@@ -337,12 +359,19 @@ def make_problem(
         Rck = quat_to_mat(q_ck_t[c])
         pk = np.einsum("fji,fmj->fmi", Rwk, pw_grid[None, :, :] - pwk[:, None, :])  # R^T (p_w - t)
         pc = np.einsum("ij,fmj->fmi", Rck, pk) + p_ck_t[c]
-        z = project(int(models[c]), pc, intr_t[c]) + pixel_sigma * rng.standard_normal((n_frames, M, 2))
-        obs_frame.append(np.repeat(np.arange(n_frames, dtype=np.int32), M))
-        obs_cam.append(np.full(n_frames * M, c, dtype=np.int32))
-        p_w.append(np.tile(pw_grid, (n_frames, 1)))
-        p_c.append(z.reshape(-1, 2))
-        g_idx.append(np.tile(gidx, (n_frames, 1)))
+        with np.errstate(divide="ignore", invalid="ignore"):  # corners behind a pinhole-type camera are culled below
+            z = project(int(models[c]), pc, intr_t[c]) + pixel_sigma * rng.standard_normal((n_frames, M, 2))
+        sel = np.ones(n_frames * M, dtype=bool)
+        if cull:
+            zf = z.reshape(-1, 2)
+            sel = np.isfinite(zf).all(1) & (zf[:, 0] >= 0) & (zf[:, 0] < width) & (zf[:, 1] >= 0) & (zf[:, 1] < height)
+            if int(models[c]) != KB4:
+                sel &= pc.reshape(-1, 3)[:, 2] > 0
+        obs_frame.append(np.repeat(np.arange(n_frames, dtype=np.int32), M)[sel])
+        obs_cam.append(np.full(n_frames * M, c, dtype=np.int32)[sel])
+        p_w.append(np.tile(pw_grid, (n_frames, 1))[sel])
+        p_c.append(z.reshape(-1, 2)[sel])
+        g_idx.append(np.tile(gidx, (n_frames, 1))[sel])
     obs_frame = np.concatenate(obs_frame)
     obs_cam = np.concatenate(obs_cam)
     p_w = np.concatenate(p_w)
