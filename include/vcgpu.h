@@ -458,6 +458,40 @@ int vcgpu_get_imu_mahalanobis(vcgpu_handle* h, double* dist /* n_frames - 1 */, 
 int vcgpu_get_imu_mahalanobis_batch(vcgpu_handle* const* handles, int n, double* const* dist /* n pointers */,
                                     double* const* r /* n pointers, or NULL; an entry may be NULL */);
 
+/* ViCalibrator::GetIntegrationPoses(k) for every interval k = 0 .. n_frames - 2 (vicalibrator.h:508-533): the poses
+ * ImuResidualT::IntegrateResidual's double-precision RK4 (types.h:611-687, IntegrateImu :575-594) passes through from
+ * frame k over the measurements GetRange(t_k, t_k+1, ts) returns, with the handle's biases, scale factors, gravity and
+ * time offset.  Interval k has as many poses as measurements (none: 0 poses): the frame's own ImuPoseT first (its pose,
+ * velocity, w_w = 0 and time t_k), then one per later measurement.  Each pose is 14 doubles:
+ *   q (x y z w) | t (3) | v_w (3) | w_w (3) | time
+ * Two quirks are the reference's, as it writes them:
+ *   - w_w is k.segment<3>(3) of the unnormalised RK4 sum k1 + 2 k2 + 2 k3 + k4: six times the step's mean rate.
+ *   - a step of dt == 0 (a sample on an interval end, frame-tied streams) repeats the previous pose unchanged, its time
+ *     and w_w included.
+ * Times are the measurements' own: sample time + ts in binary64, or the interval end t_k+1 where GetRange interpolates
+ * (the time sums of vcgpu_set_frames).
+ * start: n_frames entries; start[k] is interval k's first pose, start[n_frames-1] the total.
+ * poses: NULL (sizes only) or start[n_frames-1] * 14 doubles, sized from an earlier call at the same state.
+ * Evaluated at the handle's current accepted state.  Rotation-only stages are computed too; the reference returns
+ * nothing there, a gate its callers apply (ViCalibrator::GetAllIntegrationPoses does).  Nothing on the handle changes:
+ * state, IMU weights, the weight update's stored eigenvectors and what a later vcgpu_solve or batch computes stay as
+ * they were.  Runs as vcgpu_get_integration_poses_batch of this handle alone: the same refusals and memory.
+ * VCGPU_ERR_INVALID: a null handle or start, inertial terms off, fewer than two frames, or frame shards (one GPU only). */
+int vcgpu_get_integration_poses(vcgpu_handle* h, int64_t* start, double* poses_or_null);
+/* vcgpu_get_integration_poses of n rigs in one call: start[i] and poses[i] receive rig i's values, the bits
+ * vcgpu_get_integration_poses(handles[i]) writes whatever else is in the batch and in whatever order (each interval
+ * reads only its own rig).  poses: NULL, or n pointers of which any may be NULL (that rig's sizes only).  Per handle, on
+ * its own stream, the uploads of the handle; then on handle 0's stream a count pass over every interval of every rig
+ * (one thread per interval), a prefix sum per rig and one download of the offsets; then, if some poses[i] is given, the
+ * fill pass over those rigs and one download of their poses.
+ * Returns VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in
+ * vcgpu_last_error of every non-null handle, for: n <= 0, a null start, a null or repeated handle, a null start[i],
+ * handles on different devices, and a handle vcgpu_get_integration_poses refuses.
+ * Device memory, held by handle 0 and grown to the largest batch, never freed per call: 8 bytes per frame of offsets,
+ * 112 bytes per returned pose and 96 bytes per rig of kernel arguments. */
+int vcgpu_get_integration_poses_batch(vcgpu_handle* const* handles, int n, int64_t* const* start,
+                                      double* const* poses /* n pointers, or NULL; an entry may be NULL */);
+
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */
 /* loss-free residuals and tangent-space Jacobians per observation, caller order.

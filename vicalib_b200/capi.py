@@ -29,6 +29,7 @@ EXPORTS = [
     "vcgpu_pose_pnp_ransac", "vcgpu_pose_pnp_ransac_batch", "vcgpu_calibrate_batch",
     "vcgpu_get_frame_cross_covariance", "vcgpu_get_frame_cross_covariance_batch",
     "vcgpu_get_imu_mahalanobis", "vcgpu_get_imu_mahalanobis_batch",
+    "vcgpu_get_integration_poses", "vcgpu_get_integration_poses_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -385,6 +386,17 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_imu_mahalanobis(self.h, _p(d), _p(r)))
         return (d[:n], r[:n]) if residuals else d[:n]
 
+    def integration_poses(self):
+        """GetIntegrationPoses(k) of every interval k (vicalibrator.h:508-533) at the current state: n_frames - 1 arrays
+        of (count_k, 14) rows q (x y z w) | t (3) | v_w (3) | w_w (3) | time, the frame's own pose first, count_k the
+        interval's number of IMU measurements (0 without any).  Computed in rotation-only stages too.  Nothing on the
+        handle changes."""
+        start = np.zeros(max(self.n_frames, 1), dtype=np.int64)
+        self._chk(self.L.vcgpu_get_integration_poses(self.h, _p(start), None))
+        poses = np.zeros((max(int(start[-1]), 1), 14))
+        self._chk(self.L.vcgpu_get_integration_poses(self.h, _p(start), _p(poses)))
+        return _split_poses(start, poses)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -513,6 +525,26 @@ def imu_mahalanobis_batch(calibrators, residuals=False):
     if residuals:
         return [(d[i][: ni[i]], r[i][: ni[i]]) for i in range(n)]
     return [d[i][: ni[i]] for i in range(n)]
+
+
+def _split_poses(start, poses):
+    return [poses[start[k]: start[k + 1]] for k in range(len(start) - 1)]
+
+
+def integration_poses_batch(calibrators):
+    """vcgpu_get_integration_poses_batch: Calibrator.integration_poses() of every Calibrator of the list, one count pass
+    and one fill pass for all; each rig's poses are the bits its own call returns.  Returns one list of (count_k, 14)
+    arrays per calibrator, in order."""
+    n = len(calibrators)
+    L = lib()
+    start = [np.zeros(max(0 if g is None else g.n_frames, 1), dtype=np.int64) for g in calibrators]
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    sp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in start])
+    _batch_check(L, L.vcgpu_get_integration_poses_batch(hs, C.c_int(n), sp, None), calibrators)
+    poses = [np.zeros((max(int(a[-1]), 1), 14)) for a in start]
+    pp = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in poses])
+    _batch_check(L, L.vcgpu_get_integration_poses_batch(hs, C.c_int(n), sp, pp), calibrators)
+    return [_split_poses(a, b) for a, b in zip(start, poses)]
 
 
 def _covariances(entry, name, calibrators, out):

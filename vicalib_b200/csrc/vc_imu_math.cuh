@@ -245,10 +245,12 @@ struct AccelTangent {
   }
 };
 
-// ceres-cost-functions.h:138-177 (RK4); `at` follows an AccelTangent along the step
+// ceres-cost-functions.h:138-177 (RK4); `at` follows an AccelTangent along the step.  w_out (null: not asked for)
+// receives k.segment<3>(3) of the unnormalised sum k1 + 2 k2 + 2 k3 + k4, the w_w_ of types.h:592; a zero-length step
+// leaves it untouched, as the reference leaves the whole pose.
 template <class T, class AT>
 __device__ inline Pose<T> integrate_imu(const Pose<T>& y0, const Meas<T>& z0, const Meas<T>& z1, Vec<T> bg, Vec<T> ba,
-                                        const T sf[6], Vec<T> g, AT& at) {
+                                        const T sf[6], Vec<T> g, AT& at, Vec<T>* w_out = nullptr) {
   if (val(z1.time) == val(z0.time)) return y0;
   const T dt = z1.time - z0.time;
   T k1[9], k2[9], k3[9], k4[9];
@@ -267,6 +269,7 @@ __device__ inline Pose<T> integrate_imu(const Pose<T>& y0, const Meas<T>& z0, co
   at.step(val(dt));
 #pragma unroll
   for (int i = 0; i < 9; ++i) k1[i] = k1[i] + T(2.0) * k2[i] + T(2.0) * k3[i] + k4[i];
+  if (w_out) *w_out = Vec<T>{k1[3], k1[4], k1[5]};
   return integrate_pose(y0, k1, dt / T(6.0));
 }
 

@@ -203,6 +203,9 @@ struct vcgpu_handle {
   std::vector<unsigned char, PinnedAlloc<unsigned char>> h_pnp;
   // vcgpu_get_imu_mahalanobis(_batch) with this handle as handle 0: every rig's [ni][10] outputs (vc_batch.inl)
   double* d_mahal = nullptr;
+  // vcgpu_get_integration_poses(_batch) with this handle as handle 0: every rig's [n_frames] offsets and its poses
+  int64_t* d_pstart = nullptr;
+  double* d_poses = nullptr;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

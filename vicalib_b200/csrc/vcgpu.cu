@@ -27,6 +27,7 @@
 #include "vc_mega.cuh"
 #include "vc_dogleg.cuh"
 #include "vc_imu_weights.cuh"
+#include "vc_imu_poses.cuh"
 #include "vc_imu_mega.cuh"
 #include "vc_imu_eval_mega.cuh"
 #include "vc_pnp.cuh"
@@ -220,7 +221,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -1189,6 +1190,18 @@ extern "C" int vcgpu_get_imu_mahalanobis_batch(vcgpu_handle* const* handles, int
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!dist) return batch_refuse(handles, n, 0, "null dist array", "vcgpu_get_imu_mahalanobis_batch");
   return run_imu_mahalanobis_batch(handles, n, dist, r, "vcgpu_get_imu_mahalanobis_batch");
+}
+
+// GetIntegrationPoses of every interval (vicalibrator.h:508-533): run_integration_poses_batch of this handle alone
+extern "C" int vcgpu_get_integration_poses(vcgpu_handle* h, int64_t* start, double* poses_or_null) {
+  if (!h) return VCGPU_ERR_INVALID;
+  return run_integration_poses_batch(&h, 1, &start, &poses_or_null, "vcgpu_get_integration_poses");
+}
+extern "C" int vcgpu_get_integration_poses_batch(vcgpu_handle* const* handles, int n, int64_t* const* start,
+                                                 double* const* poses) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!start) return batch_refuse(handles, n, 0, "null start array", "vcgpu_get_integration_poses_batch");
+  return run_integration_poses_batch(handles, n, start, poses, "vcgpu_get_integration_poses_batch");
 }
 
 extern "C" int vcgpu_comm_unique_id(uint8_t id[VCGPU_UNIQUE_ID_BYTES]) {

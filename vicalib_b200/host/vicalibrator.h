@@ -519,6 +519,31 @@ class ViCalibrator {
     return dist;
   }
 
+  // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
+  // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
+  // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
+  // (not while IsRunning()); GetIntegrationPoses stays the host-side call a GUI can poll during the solve.
+  std::vector<std::vector<ImuPose>> GetAllIntegrationPoses() {
+    VICALIB_CHECK(!IsRunning(), "GetAllIntegrationPoses while running");
+    const size_t nf = NumFrames();
+    std::vector<std::vector<ImuPose>> out(nf > 1 ? nf - 1 : 0);
+    if (!(is_inertial_active_ && !optimize_rotation_only_) || nf < 2) return out;
+    std::vector<int64_t> start(nf);
+    Check(vcgpu_get_integration_poses(h_, start.data(), nullptr), "get_integration_poses");
+    std::vector<double> p(static_cast<size_t>(start[nf - 1]) * 14);
+    Check(vcgpu_get_integration_poses(h_, start.data(), p.data()), "get_integration_poses");
+    for (size_t k = 0; k + 1 < nf; ++k)
+      for (int64_t i = start[k]; i < start[k + 1]; ++i) {
+        const double* o = p.data() + 14 * i;
+        ImuPose y;
+        std::memcpy(y.t_wp_.d, o, 7 * sizeof(double));
+        for (int j = 0; j < 3; ++j) { y.v_w_[j] = o[7 + j]; y.w_w_[j] = o[10 + j]; }
+        y.time_ = o[13];
+        out[k].push_back(y);
+      }
+    return out;
+  }
+
   // Pose seeds for AddFrame: what VicalibTask::AddSuperFrame computes per frame and camera with
   // calibu::PosePnPRansac(camera, ellipses, target.Circles3D(), ellipse_target_map, 0, 0, &t_cw) and
   // t_wp = t_cw.inverse() * t_ck (src/vicalib-task.cc:322-325, 341-349) — here for ALL views in one device call.
