@@ -28,13 +28,17 @@ ns = g.phase_clocks().astype(float) / K / 1e3
 # the back-substitution slots count levels from the top (slot 12: the level just below the dense system); the last one
 # used is level 0, shared out among whichever CTAs are there (the ones still working the weights queue join later)
 names = {10: "schur reduce", 11: "dense", 22: "step stats", 23: "weights (solver CTAs)", 32: "eval tasks", 33: "imu accumulate", 34: "reduce", 35: "decide", 36: "weights"}
-cyc = {40: "chunk: wait prev", 41: "chunk: async copies + wait", 42: "chunk: scale / damp / add in place",
-       44: "chunk: couplings", 45: "chunk: forward sweep", 46: "chunk: backward sweep", 47: "chunk: Z store", 48: "chunk: Schur acc",
-       49: "chunk: separator update + stores", 53: "dense: LDL^T", 54: "dense: back-substitution", 55: "dense: write + top update"}
+# chunk phase clocks: level 1 on CTA 0 (slots 40..47), level 0 on CTA 0's first group (slots 56..63); above level 0 the
+# couplings are written in the pass that adds the Schur terms from the left
+chunk = ("wait prev", "async copies + wait", "scale / damp / add in place", "couplings", "forward sweep (+ Z, last node)",
+         "backward sweep (+ Z)", "Schur acc", "separator update + stores")
+cyc = {53: "dense: LDL^T", 54: "dense: back-substitution", 55: "dense: write + top update"}
+for base, lv in ((40, 1), (56, 0)):
+    cyc.update({base + k: f"level {lv} chunk: {nm}" for k, nm in enumerate(chunk)})
 for k in range(64):
     if k in cyc:
         if ns[k] > 0:
-            print(f"  [{k:2d}] {cyc[k]:40s} {ns[k] * 1e3 / 1980.0:8.2f} us (cycles / 1980 MHz, the H100 SXM maximum SM clock)")
+            print(f"  [{k:2d}] {cyc[k]:46s} {ns[k] * 1e3 / 1980.0:8.2f} us (cycles / 1980 MHz, the H100 SXM maximum SM clock)")
         continue
     if ns[k] > 0:
         nm = names.get(k, f"eliminate level {k}" if k < 10 else f"backsub, level {k - 11} from the top")

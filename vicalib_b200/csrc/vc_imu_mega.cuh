@@ -87,11 +87,19 @@ struct ChainSolveArgs {
 // the Schur accumulator of a group: lower triangle of S packed row by row (row r at r (r + 1) / 2), then the right-hand
 // side — half the square, which is what lets two groups of chunk length 8 fit an SM at G = 67
 __host__ __device__ inline int chain_sacc_doubles(int G) { return G * (G + 1) / 2 + G; }
-// a group's workspace (chain_eliminate_chunk): Sacc | Al El gl | Ap | Uc | Ur | V | Eo
+// Above level 0 a chunk's Schur terms from the left (add*: A and g of its c nodes, E of its separator) are staged in the
+// coupling columns [0, 3 FD) of V's rows until the couplings step; what does not fit there (G > 109) goes past Eo
+__host__ __device__ inline int chain_stage_overflow(int G) {
+  constexpr int FD = 9, c = kCsChunk;
+  const int over = c * (FD * FD + FD) + FD * G - (c - 1) * FD * 3 * FD;
+  return over > 0 ? over : 0;
+}
+// a group's workspace (chain_eliminate_chunk): Sacc | Al El gl | Ap | Uc | Ur | V | Eo | staging overflow
 __host__ __device__ inline size_t chain_group_doubles(int G) {
   constexpr int FD = 9, c = kCsChunk;
   const size_t VW = FD + 2 * FD + G + 1;
-  return chain_sacc_doubles(G) + FD * FD + FD * G + FD + (2 * (c - 1) + 1) * FD * FD + (c - 1) * FD * VW + (c - 1) * FD * G;
+  return chain_sacc_doubles(G) + FD * FD + FD * G + FD + (2 * (c - 1) + 1) * FD * FD + (c - 1) * FD * VW + (c - 1) * FD * G +
+         chain_stage_overflow(G);
 }
 // tiles of the register version that fits N (0: none does — shared-memory version), and the layout of S that goes with it
 __host__ __device__ inline int dense_tiles(int N) {
@@ -137,39 +145,70 @@ __device__ __forceinline__ void cp_async8(double* dst, const double* src) {
 }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
 
-// *dst(e) += add[e] for e in [0, n), eight loads in flight per thread (element e by thread e mod NT)
-template <int NT, class Dst>
-__device__ __forceinline__ void add_in_place(const double* add, int n, int tid, Dst dst) {
-  constexpr int B = 8;
-  for (int e0 = tid; e0 < n; e0 += B * NT) {
-    double v[B];
-#pragma unroll
-    for (int u = 0; u < B; ++u) v[u] = e0 + u * NT < n ? __ldcg(add + e0 + u * NT) : 0.0;
-#pragma unroll
-    for (int u = 0; u < B; ++u)
-      if (e0 + u * NT < n) {
-        double* d = dst(e0 + u * NT);
-        *d = *d + v[u];
-      }
-  }
-}
-
-// Forward + backward sweep of one chunk (separator s = j*c, interior nodes s+1..s+m) by one group of 128 threads, in
-// chain_solve and, one chunk per CTA, in the multi-launch engine's chain_eliminate_kernel.  The chunk's blocks arrive by
-// asynchronous copies straight into their places in shared memory, all in flight before the first one is used (no
-// register staging: nothing grows with the chunk length), the 9 x 9 pivots are factored right-looking with rsqrt, and
-// the group's Schur accumulator Sacc lives on across chunks and levels.
-// NT: threads working on the chunk — a group of 128 (two chunks per CTA in flight: the wide levels) or the whole CTA of
-// 256 (levels with fewer chunks than CTAs, where the other group would idle); either covers a V row, one column each
 template <int NT>
 __device__ __forceinline__ void gsync(int grp) {
   if (NT == kCsThreads) __syncthreads();
   else group_sync(grp);
 }
+// A chunk's Schur terms: S += sum_i E_i^T X_i[E] (packed lower triangle, Sacc[0, GT)) and rhs += sum_i E_i^T X_i[g]
+// (Sacc[GT, GT + G)) over its m interior nodes; E_i row k at Eo + (i FD + k) G, X_i row k at X + (i FD + k) VW (column
+// G: g).  Each entry is one FMA chain from 0.0, i then k ascending, added to its accumulator once.  A thread takes a
+// 2 x 2 tile of the lower triangle (rows 2 br, 2 br + 1; columns 2 bc, 2 bc + 1; bc <= br) or two rows of the right-hand
+// side, so every value it loads from shared memory serves two entries.  Not inlined: in chain_solve_kernel the tiles
+// would otherwise cost the kernel more spills.
+template <int FD, int NT>
+__device__ __noinline__ void chain_schur_acc(double* Sacc, const double* Eo, const double* X, int m, int G, int VW, int tid) {
+  const int RB = (G + 1) / 2, nT = RB * (RB + 1) / 2, GT = G * (G + 1) / 2;
+  for (int t = tid; t < nT + RB; t += NT) {
+    int br = t - nT, c0 = G;  // t >= nT: rows 2 br, 2 br + 1 of the right-hand side
+    if (t < nT) {
+      int bc = t;
+      br = 0;
+      while (bc > br) { bc -= br + 1; ++br; }
+      c0 = 2 * bc;
+    }
+    const int r0 = 2 * br, r1 = min(r0 + 1, G - 1), c1 = min(c0 + 1, G);  // (clamped loads of a tile's missing row/column)
+    double s00 = 0.0, s01 = 0.0, s10 = 0.0, s11 = 0.0;
+    for (int i = 0; i < m; ++i) {
+      const double* Ei = Eo + i * FD * G;
+      const double* Xi = X + i * FD * VW;
+#pragma unroll
+      for (int k = 0; k < FD; ++k) {
+        const double e0 = Ei[k * G + r0], e1 = Ei[k * G + r1], x0 = Xi[k * VW + c0], x1 = Xi[k * VW + c1];
+        s00 += e0 * x0;
+        s01 += e0 * x1;
+        s10 += e1 * x0;
+        s11 += e1 * x1;
+      }
+    }
+    const bool two = r0 + 1 < G;
+    if (c0 == G) {
+      Sacc[GT + r0] += s00;
+      if (two) Sacc[GT + r0 + 1] += s10;
+    } else {
+      const int k0 = r0 * (r0 + 1) / 2 + c0, k1 = k0 + r0 + 1;  // (r0, c0), (r0 + 1, c0)
+      Sacc[k0] += s00;
+      if (c0 + 1 <= r0) Sacc[k0 + 1] += s01;
+      if (two) {
+        Sacc[k1] += s10;
+        Sacc[k1 + 1] += s11;
+      }
+    }
+  }
+}
+
+// Forward + backward sweep of one chunk (separator s = j*c, interior nodes s+1..s+m) by one group of 128 threads, in
+// chain_solve and, one chunk per CTA, in the multi-launch engine's chain_eliminate_kernel.  The chunk's blocks (and
+// above level 0 the Schur terms from the chunk on its left) arrive by asynchronous copies straight into shared memory,
+// all in flight before the first one is used (no register staging: nothing grows with the chunk length), the 9 x 9
+// pivots are factored right-looking with rsqrt, each element of an interior node's solution goes to Z as the sweep
+// finishes it, and the group's Schur accumulator Sacc lives on across chunks and levels.
+// NT: threads working on the chunk — a group of 128 (two chunks per CTA in flight: the wide levels) or the whole CTA of
+// 256 (levels with fewer chunks than CTAs, where the other group would idle); either covers a V row, one column each
 template <int FD, int NT>
 __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const ChainLevel L, const ChainLevel nxt, int G, int j, double* sm,
                                              int tid, int grp, int* bad, unsigned long long* dbg = nullptr) {
-  // dbg: cycle counts of the chunk's phases (measurement hook: phase clocks [40..51], one group)
+  // dbg: cycle counts of the chunk's phases (measurement hook: eight phase clock slots from dbg, one group)
   long long dbg_t = dbg ? clock64() : 0;
   auto tick = [&](int slot) {
     if (dbg && tid == 0) {
@@ -179,9 +218,9 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
     }
   };
   constexpr int c = kCsChunk;
-  const int NS = chain_sacc_doubles(G), GT = G * (G + 1) / 2;
+  const int NS = chain_sacc_doubles(G);
   const int w = 2 * FD + G + 1, VW = FD + w;
-  const int oL = FD, oR = 2 * FD, oE = 3 * FD, og = 3 * FD + G;  // column offsets inside a V row
+  const int oE = 3 * FD, og = 3 * FD + G;  // column offsets inside a V row [U | L | R | E | g]
   double* Sacc = sm;                       // [NS] packed (chain_sacc_doubles)
   double* Al = Sacc + NS;                  // [FD*FD]
   double* El = Al + FD * FD;               // [FD*G]
@@ -206,11 +245,30 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
   const int rw0 = tid / w, qw0 = tid - rw0 * w;      // ... of an FD x w block
   const int rV0 = tid / VW, qV0 = tid - rV0 * VW;    // ... of an FD x VW block
   const bool lvl0 = src.L == nullptr;
-  // level 0: the Jacobi scales of nodes s-1 .. rIdx ([(c+2)][FD], entries [0, kSG)) and of the globals (entries kSG + q)
-  // are parked in the coupling columns [0, 3 FD) of V's rows, which nothing else touches before the couplings step
-  constexpr int kSG = (c + 2) * FD;
-  auto scl = [&](int e) -> double* { return V + (e / (3 * FD)) * VW + e % (3 * FD); };
-  // ---- the chunk's blocks as stored (level 0: the unscaled normal equations and the scales), one round of copies
+  // The coupling columns [0, 3 FD) of V's rows, which nothing else touches before the couplings step, hold what the
+  // in-place step reads (entry t at row t / (3 FD)):
+  // level 0: the Jacobi scales of nodes s-1 .. rIdx ([(c+2)][FD], entries [0, kSG)) and of the globals (entries kSG + q);
+  // above: the Schur terms of the chunk on the left, addA [nn][FD*FD] | addg [nn][FD] | the separator's addE [FD*G]
+  // (entries past kPark in the staging overflow after Eo); the interior nodes' addE goes to Eo
+  constexpr int kSG = (c + 2) * FD, kPark = (c - 1) * FD * 3 * FD;
+  auto scl = [&](int e) -> double* { return V + (e / (3 * FD)) * VW + e % (3 * FD); };  // e < kPark
+  auto stg = [&](int e) -> double* { return e < kPark ? scl(e) : Eo + (c - 1) * FD * G + (e - kPark); };
+  const bool add = !lvl0 && L.addA != nullptr;  // (the host sets the three add* together)
+  const int oSg = nn * FD * FD, oSE = nn * (FD * FD + FD);
+  // couplings of the interior nodes' right-hand sides from the staged U blocks: entry t < m * 3 FD * FD of the coupling
+  // columns (interior node t / (3 FD * FD): H[p, p+1] | H[p0, s] = U[p0]^T | H[pl, rIdx])
+  auto coupling = [&](int t) -> double {
+    const int i = t / (3 * FD * FD), rc = t - i * 3 * FD * FD, r = rc / (3 * FD), col = rc - r * 3 * FD;
+    const int blk = col / FD, q = col - blk * FD;
+    const bool lastI = i == m - 1;
+    const double* Unext = lastI ? Ur : Uc + (i + 1) * FD * FD;  // H[p, p+1]
+    const double unext = (!lastI || hasR) ? Unext[r * FD + q] : 0.0;
+    if (blk == 0) return lastI ? 0.0 : unext;
+    if (blk == 1) return i == 0 ? Uc[q * FD + r] : 0.0;
+    return (lastI && hasR) ? unext : 0.0;
+  };
+  // ---- the chunk's blocks as stored (level 0: the unscaled normal equations and the scales; above: the Schur terms of
+  // the chunk on the left as well), one round of copies
   {
     const double* gA = (lvl0 ? src.b.B : L.A) + static_cast<int64_t>(s) * FD * FD;
     const double* gU = (lvl0 ? src.b.U : L.U) + static_cast<int64_t>(s + 1) * FD * FD;
@@ -229,11 +287,18 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
       }
       for (int e = tid; e < G; e += NT) cp_async8(scl(kSG + e), src.scale + static_cast<int64_t>(src.nf) * FD + e);
     }
+    if (add) {  // (8-byte copies, so .ca: cp.async.cg copies 16 bytes only; the level barrier's acquire orders them, as the blocks)
+      const int64_t o = static_cast<int64_t>(s);
+      for (int e = tid; e < nn * FD * FD; e += NT) cp_async8(stg(e), L.addA + o * FD * FD + e);
+      for (int e = tid; e < nn * FD; e += NT) cp_async8(stg(oSg + e), L.addg + o * FD + e);
+      for (int e = tid; e < nn * FD * G; e += NT) cp_async8(e < FD * G ? stg(oSE + e) : Eo + (e - FD * G), L.addE + o * FD * G + e);
+    }
     cp_async_wait_all();
   }
   gsync<NT>(grp);
   tick(1);
-  // ---- in place: level 0 scales and damps, deeper levels add the Schur terms of the chunk on the left (add*)
+  // ---- in place: level 0 scales and damps, deeper levels add the Schur terms of the chunk on the left (block + add)
+  const int nC = m * 3 * FD * FD;
   if (lvl0) {
     for (int e = tid; e < nn * FD * FD; e += NT) {
       const int nd = e / (FD * FD), el = e - nd * FD * FD, r = el / FD, q = el - r * FD;
@@ -258,41 +323,41 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
       double* d = e < FD ? gl + e : V + (e - FD) * VW + og;
       *d = *d * *scl(FD + e);
     }
+    // the interior nodes' E also goes to Eo as the sweeps will see it, kept for the Schur product
     for (int e = tid, R = rG0, q = qG0; e < nn * FD * G; e += NT, adv2(R, q, G, NT)) {
       double* d = R < FD ? El + e : V + (R - FD) * VW + oE + q;
-      *d = *d * *scl(FD + R) * *scl(kSG + q);
+      const double v = *d * *scl(FD + R) * *scl(kSG + q);
+      *d = v;
+      if (R >= FD) Eo[e - FD * G] = v;
     }
+    gsync<NT>(grp);
+    tick(2);
+    for (int t = tid; t < nC; t += NT) *scl(t) = coupling(t);
+    gsync<NT>(grp);
+    tick(3);
   } else {
-    const int64_t o = static_cast<int64_t>(s);
-    if (L.addA) add_in_place<NT>(L.addA + o * FD * FD, nn * FD * FD, tid, [&](int e) { return e < FD * FD ? Al + e : Ap + (e - FD * FD); });
-    if (L.addg) add_in_place<NT>(L.addg + o * FD, nn * FD, tid, [&](int e) { return e < FD ? gl + e : V + (e - FD) * VW + og; });
-    if (L.addE)
-      add_in_place<NT>(L.addE + o * FD * G, nn * FD * G, tid, [&](int e) {
-        const int R = e / G;
-        return R < FD ? El + e : V + (R - FD) * VW + oE + (e - R * G);
-      });
-  }
-  // the interior nodes' E as the sweeps will see it, kept for the Schur product (every thread copies the elements it
-  // finished itself: no barrier needed)
-  for (int e = tid, R = rG0, q = qG0; e < nn * FD * G; e += NT, adv2(R, q, G, NT))
-    if (R >= FD) Eo[e - FD * G] = V[(R - FD) * VW + oE + q];
-  gsync<NT>(grp);
-  tick(2);
-  // couplings of the interior nodes' right-hand sides, from the staged U blocks
-  for (int i = 0; i < m; ++i) {
-    double* Vi = V + static_cast<int64_t>(i) * FD * VW;
-    const bool lastI = i == m - 1;
-    const double* Unext = lastI ? Ur : Uc + (i + 1) * FD * FD;  // H[p, p+1]
-    for (int e = tid; e < FD * FD; e += NT) {
-      const int r = e / FD, q = e - r * FD;
-      Vi[r * VW + oL + q] = i == 0 ? Uc[q * FD + r] : 0.0;  // H[p0, s] = U[p0]^T
-      const double unext = (!lastI || hasR) ? Unext[e] : 0.0;
-      Vi[r * VW + q] = lastI ? 0.0 : unext;
-      Vi[r * VW + oR + q] = (lastI && hasR) ? unext : 0.0;
+    // entry t of the coupling columns is read (staged add) and then written (coupling) by the same thread
+    const int nS = add ? oSE + FD * G : 0;
+    for (int t = tid; t < max(nS, nC); t += NT) {
+      double* st = stg(t);
+      if (t < nS) {
+        double* d = t < oSg ? (t < FD * FD ? Al + t : Ap + (t - FD * FD))
+                  : t < oSE ? (t - oSg < FD ? gl + (t - oSg) : V + (t - oSg - FD) * VW + og)
+                            : El + (t - oSE);
+        *d = *d + *st;
+      }
+      if (t < nC) *st = coupling(t);
     }
+    // the interior nodes' E: staged add in Eo, where the sum stays for the Schur product
+    for (int e = FD * G + tid, R = FD + rG0, q = qG0; e < nn * FD * G; e += NT, adv2(R, q, G, NT)) {
+      double* d = V + (R - FD) * VW + oE + q;
+      const double v = add ? *d + Eo[e - FD * G] : *d;
+      *d = v;
+      Eo[e - FD * G] = v;
+    }
+    gsync<NT>(grp);
+    tick(2);
   }
-  gsync<NT>(grp);
-  tick(4);
   // ---- forward sweep
   for (int i = 0; i < m; ++i) {
     double* Vi = V + static_cast<int64_t>(i) * FD * VW;
@@ -351,69 +416,35 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
       }
 #pragma unroll
       for (int ii = 0; ii < FD; ++ii) Vi[ii * VW + q] = x[ii];
+      if (i == m - 1 && q >= FD) {  // the last interior node's solution is final here: its Z row, columns [L | R | E | g]
+        double* Z = L.Z + (static_cast<int64_t>(s) + 1 + i) * FD * w + (q - FD);
+#pragma unroll
+        for (int ii = 0; ii < FD; ++ii) Z[ii * w] = x[ii];
+      }
     }
     gsync<NT>(grp);
   }
-  tick(5);
-  // ---- backward sweep: X_i = V_R(i) - V_U(i) X_{i+1}
+  tick(4);
+  // ---- backward sweep: X_i = V_R(i) - V_U(i) X_{i+1}, each element stored to Z as it is finished
   for (int i = m - 2; i >= 0; --i) {
     double* Vi = V + static_cast<int64_t>(i) * FD * VW;
     const double* Vn = V + static_cast<int64_t>(i + 1) * FD * VW;
+    double* Z = L.Z + (static_cast<int64_t>(s) + 1 + i) * FD * w;
     for (int e = tid, r = rw0, qq = qw0; e < FD * w; e += NT, adv2(r, qq, w, NT)) {
       const int q = FD + qq;
       double sum = 0.0;
 #pragma unroll
       for (int k = 0; k < FD; ++k) sum += Vi[r * VW + k] * Vn[k * VW + q];
-      Vi[r * VW + q] -= sum;
+      const double x = Vi[r * VW + q] - sum;
+      Vi[r * VW + q] = x;
+      Z[e] = x;
     }
     gsync<NT>(grp);
   }
+  tick(5);
+  // ---- the Schur terms: S += E_i^T X_i[E], rhs += E_i^T X_i[g]
+  chain_schur_acc<FD, NT>(Sacc, Eo, V + oE, m, G, VW, tid);
   tick(6);
-  // ---- store Z, accumulate the Schur terms: S += E_i^T X_i[E], rhs += E_i^T X_i[g]
-  for (int i = 0; i < m; ++i) {
-    const int64_t p = s + 1 + i;
-    const double* Vi = V + static_cast<int64_t>(i) * FD * VW;
-    for (int e = tid, r = rw0, q = qw0; e < FD * w; e += NT, adv2(r, q, w, NT)) L.Z[p * FD * w + e] = Vi[r * VW + FD + q];
-  }
-  tick(7);
-  {  // lower triangle of S (row ra has ra + 1 entries), then the right-hand side; four entries in flight per thread
-    int ra = 0, cb = tid;
-    while (cb > ra) { cb -= ra + 1; ++ra; }
-    while (ra < G) {
-      int r4[4], c4[4];
-      double sum[4] = {0.0, 0.0, 0.0, 0.0};
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        r4[u] = ra; c4[u] = cb;
-        cb += NT;
-        while (cb > ra && ra < G) { cb -= ra + 1; ++ra; }
-      }
-      for (int i = 0; i < m; ++i) {
-        const double* Vi = V + static_cast<int64_t>(i) * FD * VW + oE;
-        const double* Ei = Eo + i * FD * G;
-#pragma unroll
-        for (int k = 0; k < FD; ++k) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (r4[u] < G) sum[u] += Ei[k * G + r4[u]] * Vi[k * VW + c4[u]];
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-        if (r4[u] < G) Sacc[r4[u] * (r4[u] + 1) / 2 + c4[u]] += sum[u];
-    }
-    for (int r = tid; r < G; r += NT) {
-      double sum = 0.0;
-      for (int i = 0; i < m; ++i) {
-        const double* Vi = V + static_cast<int64_t>(i) * FD * VW;
-        const double* Ei = Eo + i * FD * G;
-#pragma unroll
-        for (int k = 0; k < FD; ++k) sum += Ei[k * G + r] * Vi[k * VW + og];
-      }
-      Sacc[GT + r] += sum;
-    }
-  }
-  tick(8);
   if (m > 0) {
     const double* X0 = V;                                          // node s+1
     const double* Xl = V + static_cast<int64_t>(m - 1) * FD * VW;  // last interior node
@@ -469,7 +500,7 @@ __device__ __forceinline__ void chain_eliminate_chunk(const NodeSrc& src, const 
     if (j == 0) nxt.addg[e] = 0.0;
   }
   if (tid == 0) nxt.orig[j] = src.L ? L.orig[s] : s;
-  tick(9);
+  tick(7);
 }
 
 // Back-substitution of one level: x_p = -Z_g - Z_L x_left - Z_R x_right - Z_E dc for every interior node p, one warp each.
@@ -1122,11 +1153,12 @@ __device__ __forceinline__ void chain_solve(const ChainSolveArgs& a, Scope scope
     src.sepdiag = a.sepdiag; src.rank = a.dp.rank; src.ghost = a.dp.ghost;
     const int nsep = a.lev[l + 1].n - a.dp.ghost;
     const ChainLevel Lc = a.lev[l], Ln = a.lev[l + 1];
+    // chunk phase clocks (measurement hook): level 0 on CTA 0's group 0 in slots [56, 64), level 1 on CTA 0 in [40, 48)
+    unsigned long long* dbg = a.prof && bid == 0 && l < 2 ? a.prof + (l == 0 ? 56 : 40) : nullptr;
     if (nsep > nb || !a.narrow_ok) {  // wide level: two chunks per CTA in flight
       for (int j = gid; j < nsep; j += n_groups)
-        chain_eliminate_chunk<FD, kCsGroup>(src, Lc, Ln, G, j, gsm, gtid, grp, &bad_s[grp], nullptr);
+        chain_eliminate_chunk<FD, kCsGroup>(src, Lc, Ln, G, j, gsm, gtid, grp, &bad_s[grp], grp == 0 ? dbg : nullptr);
     } else {          // narrow level: the whole CTA on one chunk (group 0's workspace and Schur accumulator)
-      unsigned long long* dbg = (a.prof && bid == 0 && l == 1) ? a.prof + 40 : nullptr;
       for (int j = bid; j < nsep; j += nb) chain_eliminate_chunk<FD, kCsThreads>(src, Lc, Ln, G, j, smem, tid, 0, &bad_s[0], dbg);
       __syncthreads();
     }
