@@ -427,6 +427,64 @@ int vcgpu_get_frame_cross_covariance(vcgpu_handle* h, double* cov_fg /* n_frames
 int vcgpu_get_frame_cross_covariance_batch(vcgpu_handle* const* handles, int n, double* const* cov_fg /* n pointers, or NULL */,
                                            double* const* cov_fn /* n pointers, or NULL */, int* status /* n, or NULL */);
 
+/* The pixel uncertainty the calibration leaves at projected points.  Point i: camera c = cam_id[i], pixel z = pix[i],
+ * depth d = depth[i] >= 0 (NULL: every d = 0) and a frame:
+ *   ray      unproject_c(z), the unit vector whose projection at the current intrinsics is z (ray_or_null).
+ *            linear: closed form.  FOV: closed form in the model's own branches (w^2 <= 1e-5; the small-rad branch
+ *            where its undistorted radius has r^2 < 1e-5, else r = tan(r_d w) / m, m = 2 tan(w / 2), r_d |w| < pi / 2).
+ *            poly2 / poly3: r f(r) = r_d on [0, r_fold), r_fold the first zero of d(r f(r))/dr.  KB4: theta d(theta) =
+ *            r_d on [0, theta_max), theta_max = min(pi, the first zero of its derivative); rays beyond 90 degrees point
+ *            behind the image plane.  Both by Newton from r_d, at most 50 steps, converged where |r f(r) - r_d| <=
+ *            1e-15 r_d or after a step |dr| <= 1e-14 r;
+ *            every derivative it divides by must be positive and every iterate must stay inside the domain.
+ *   point    d > 0: P_c = d * ray (d is the distance along the ray, not z-depth).  d == 0: the point at infinity.
+ *   J        2 x (6 + K): the derivatives of the projection of that fixed point with respect to the camera's globals,
+ *            in vcgpu_get_covariance's tangent (w_ck 3 | p_ck 3 | intrinsics K), vcgpu_eval_reproj's columns.
+ *            VCGPU_PROJ_CAMERA: the point is fixed in the camera frame; only the intrinsics' columns are nonzero.
+ *            VCGPU_PROJ_RIG: it is fixed in the rig (IMU) frame, P_k = R_ck^T (P_c - p_ck); at d == 0 the p_ck columns
+ *            are exactly 0.0, the limit as d goes to infinity.
+ *   cov      Sigma_z = J Sigma_c J^T as (S_uu, S_uv, S_vv), Sigma_c camera c's (6+K)^2 diagonal block of the globals'
+ *            covariance; products in a fixed order, one triangle, so Sigma_z is exactly symmetric.  Like Sigma_c it
+ *            assumes unit observation variance: scale it by the residual variance (e.g. 2 cost / (n - G)).  Constant
+ *            or unused blocks are exactly 0.0 in Sigma_c and give exact zeros here (fix_intrinsics in CAMERA frame, a
+ *            camera no observation sees).
+ * A pixel outside its model's domain, or where Newton does not converge, gets NaN in every output. */
+enum { VCGPU_PROJ_CAMERA = 0, VCGPU_PROJ_RIG = 1 };
+typedef struct {
+  int64_t n;               /* points */
+  const int32_t* cam_id;   /* n */
+  const double* pix;       /* n * 2 */
+  const double* depth;     /* n, or NULL: every point at infinity */
+  int frame;               /* VCGPU_PROJ_* */
+  double* cov;             /* n * 3: S_uu, S_uv, S_vv */
+  double* ray_or_null;     /* n * 3 unit rays, or NULL */
+} vcgpu_proj_points;
+/* globals_cov_or_null: NULL computes the matrix as vcgpu_get_covariance does, keeping that call's device memory; or a
+ * G x G matrix in its layout (e.g. from vcgpu_get_covariance_batch), uploaded in place of the elimination.  A given
+ * matrix gives the same bits on either path.  Evaluated at the handle's current accepted state; one kernel launch, one
+ * thread per point.  Nothing on the handle changes: state, IMU weights, the weight update's stored eigenvectors and what
+ * a later vcgpu_solve or batch computes stay as they were.
+ * VCGPU_ERR_NUMERIC: as vcgpu_get_covariance (nothing is written).  VCGPU_ERR_INVALID, before anything is launched and
+ * naming the point: a null pts or cov, n < 0, null cam_id or pix with n > 0, a cam_id outside the handle's cameras, a
+ * negative or non-finite depth, an unknown frame, frame shards (one GPU only).
+ * Device memory, held by the handle and grown to the largest call, never freed per call: G^2 doubles, and per point 28
+ * bytes of inputs (20 without depths) and 24 bytes of outputs (48 with rays); plus vcgpu_get_covariance's when it computes
+ * the matrix. */
+int vcgpu_get_projection_covariance(vcgpu_handle* h, const double* globals_cov_or_null /* G x G */,
+                                    const vcgpu_proj_points* pts);
+/* vcgpu_get_projection_covariance of n rigs in one call: pts[i] are rig i's points.  The matrices are
+ * vcgpu_get_covariance_batch's (its cluster kernels), then one point launch covers every rig: tiles of 256 consecutive
+ * points of one rig, so a rig's outputs do not depend, bit for bit, on the rest of the batch or its order, and equal its
+ * single call to rounding (as the covariance calls do).  A rig with n = 0 gets nothing written.
+ * status, VCGPU_ERR_NUMERIC: as vcgpu_get_covariance_batch; a failing rig's outputs are not written, every other rig's are.
+ * VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in vcgpu_last_error
+ * of every non-null handle: n <= 0, a null pts, a rig vcgpu_get_projection_covariance refuses (naming the point), and
+ * everything vcgpu_get_covariance_batch refuses.
+ * Device memory: vcgpu_get_covariance_batch's, and held by handle 0 per rig G^2 doubles and 152 bytes of kernel
+ * arguments, and per point what vcgpu_get_projection_covariance takes. */
+int vcgpu_get_projection_covariance_batch(vcgpu_handle* const* handles, int n, const vcgpu_proj_points* pts,
+                                          int* status /* n, or NULL */);
+
 /* Each IMU interval's Mahalanobis distance, as UpdateImuWeights computes it and logs it against chi2inv(0.95, 9) =
  * 16.9190 (vicalibrator.h:786-794): per interval k (n_frames - 1 of them),
  *   r = [SE3::log(T_end * T_w,k+1^-1) (upsilon 3, omega 3); v_end - v_w[k+1]]   (the reference's `residuals`)

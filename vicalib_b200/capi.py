@@ -30,6 +30,7 @@ EXPORTS = [
     "vcgpu_get_frame_cross_covariance", "vcgpu_get_frame_cross_covariance_batch",
     "vcgpu_get_imu_mahalanobis", "vcgpu_get_imu_mahalanobis_batch",
     "vcgpu_get_integration_poses", "vcgpu_get_integration_poses_batch",
+    "vcgpu_get_projection_covariance", "vcgpu_get_projection_covariance_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -65,6 +66,36 @@ class PnpViews(C.Structure):
     _fields_ = [("n_views", C.c_int), ("cam_id", C.c_void_p), ("start", C.c_void_p), ("count", C.c_void_p),
                 ("pix", C.c_void_p), ("pw", C.c_void_p), ("T_cw", C.c_void_p), ("rmse_or_null", C.c_void_p),
                 ("n_used_or_null", C.c_void_p)]
+
+
+class ProjPoints(C.Structure):
+    """vcgpu_proj_points: one rig's points and outputs of vcgpu_get_projection_covariance(_batch)"""
+    _fields_ = [("n", C.c_int64), ("cam_id", C.c_void_p), ("pix", C.c_void_p), ("depth", C.c_void_p), ("frame", C.c_int),
+                ("cov", C.c_void_p), ("ray_or_null", C.c_void_p)]
+
+
+# vcgpu_proj_points::frame
+PROJ_FRAMES = {"camera": 0, "rig": 1}
+
+
+def _proj_points(cam_id, pix, depth, frame, rays):
+    """the arrays of one rig's points and a ProjPoints over them (the arrays must outlive the call)"""
+    if frame not in PROJ_FRAMES:
+        raise ValueError(f"frame must be one of {sorted(PROJ_FRAMES)}, not {frame!r}")
+    cam = _c(np.atleast_1d(cam_id), np.int32)
+    n = len(cam)
+    px = _c(pix).reshape(n, 2)
+    d = None if depth is None else _c(np.broadcast_to(np.asarray(depth, dtype=np.float64), (n,)))
+    cov = np.zeros((max(n, 1), 3))
+    ray = np.zeros((max(n, 1), 3)) if rays else None
+    pts = ProjPoints(n, cam.ctypes.data, px.ctypes.data, None if d is None else d.ctypes.data, PROJ_FRAMES[frame],
+                     cov.ctypes.data, None if ray is None else ray.ctypes.data)
+    return (cam, px, d, cov, ray), pts
+
+
+def _proj_result(keep, n):
+    cov, ray = keep[3][:n], keep[4]
+    return cov if ray is None else (cov, ray[:n])
 
 
 class Flow(C.Structure):
@@ -397,6 +428,18 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_integration_poses(self.h, _p(start), _p(poses)))
         return _split_poses(start, poses)
 
+    def projection_covariance(self, cam_id, pix, depth=None, frame="camera", cov=None, rays=False):
+        """The pixel covariance the calibration leaves at projected points (vcgpu_get_projection_covariance): point i is
+        pixel pix[i] (n, 2) of camera cam_id[i] at distance depth[i] along its ray (None or 0: at infinity), fixed in
+        the camera frame ("camera": only the intrinsics move it) or in the rig frame ("rig": q_ck and p_ck too).
+        Returns (n, 3) rows S_uu, S_uv, S_vv for unit observation variance (scale by the residual variance), NaN
+        outside the lens model's domain; rays=True also returns the (n, 3) unit rays.  cov: the G x G matrix of
+        covariance() to use instead of computing it.  Nothing on the handle changes."""
+        keep, pts = _proj_points(cam_id, pix, depth, frame, rays)
+        S = None if cov is None else _c(cov).reshape(self.G, self.G)
+        self._chk(self.L.vcgpu_get_projection_covariance(self.h, _p(S), C.byref(pts)))
+        return _proj_result(keep, pts.n)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -525,6 +568,32 @@ def imu_mahalanobis_batch(calibrators, residuals=False):
     if residuals:
         return [(d[i][: ni[i]], r[i][: ni[i]]) for i in range(n)]
     return [d[i][: ni[i]] for i in range(n)]
+
+
+def projection_covariance_batch(calibrators, points):
+    """vcgpu_get_projection_covariance_batch: Calibrator.projection_covariance() of every Calibrator of the list, the
+    matrices by covariance_batch's cluster kernels and one point launch for all.  points: one dict per calibrator with
+    cam_id, pix and optionally depth, frame ("camera") and rays (False).  Returns one result per calibrator, in order,
+    as projection_covariance() returns it.  Raises VcgpuError as covariance_batch does; its `covariances` then holds
+    the results of the rigs that were written and None for the others."""
+    n = len(calibrators)
+    L = lib()
+    keeps, arr = [], (ProjPoints * max(n, 1))()
+    for i, p in enumerate(points):
+        keep, arr[i] = _proj_points(p["cam_id"], p["pix"], p.get("depth"), p.get("frame", "camera"), p.get("rays", False))
+        keeps.append(keep)
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    st = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_projection_covariance_batch(hs, C.c_int(n), arr, st)
+    out = [_proj_result(keeps[i], arr[i].n) for i in range(n)]
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:
+            e.status = [st[i] for i in range(n)]
+            e.covariances = [out[i] if st[i] == 0 else None for i in range(n)]
+        raise e
+    return out
 
 
 def _split_poses(start, poses):

@@ -519,6 +519,21 @@ class ViCalibrator {
     return dist;
   }
 
+  // The pixel covariance the calibration leaves at points of camera `cam`: pixels (u, v) interleaved, depth one distance
+  // along each pixel's ray (empty: every point at infinity), the point fixed in the rig frame (rig_frame) or the camera
+  // frame.  Three values per point, S_uu S_uv S_vv, for unit observation variance (scale by the residual variance); NaN
+  // where a pixel lies outside the lens model's domain.  Call after the solve has finished (not while IsRunning()).
+  std::vector<double> GetProjectionCovariance(int cam, const std::vector<double>& pixels, const std::vector<double>& depth,
+                                              bool rig_frame) {
+    const int64_t n = static_cast<int64_t>(pixels.size() / 2);
+    std::vector<int32_t> cam_id(n, cam);
+    std::vector<double> cov(3 * n, 0.0);
+    const vcgpu_proj_points pts{n, cam_id.data(), pixels.data(), depth.empty() ? nullptr : depth.data(),
+                                rig_frame ? VCGPU_PROJ_RIG : VCGPU_PROJ_CAMERA, cov.data(), nullptr};
+    Check(vcgpu_get_projection_covariance(h_, nullptr, &pts), "get_projection_covariance");
+    return cov;
+  }
+
   // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
   // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
   // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
