@@ -485,6 +485,78 @@ int vcgpu_get_projection_covariance(vcgpu_handle* h, const double* globals_cov_o
 int vcgpu_get_projection_covariance_batch(vcgpu_handle* const* handles, int n, const vcgpu_proj_points* pts,
                                           int* status /* n, or NULL */);
 
+/* The information candidate views of the target would add to the globals, to choose the next view to capture.  A
+ * candidate is a rig pose T_wp (vcgpu_set_frames' storage, q | t) from which the target's points p_w (world frame, as
+ * vcgpu_set_observations' p_w) may be seen.  At the handle's current accepted state, corner j is seen by camera c of
+ * candidate i when
+ *   domain   KB4: theta < theta_max; every other model: z > 0 in the camera frame; poly2 / poly3: the undistorted
+ *            radius is below r_fold; FOV: r_d |w| < pi / 2 past its small-rad branch.  These are the limits
+ *            vcgpu_get_projection_covariance documents, from the same device routines;
+ *   image    its projection lies in [0, width[c]) x [0, height[c]);
+ *   facing   with facing != NULL (the target's front normal n, world frame): (c_w - p_w) . n > 0, c_w the camera centre.
+ * A seen corner is an observation at its own projection (residual 0, SoftLOne weight 1) weighted by the flags'
+ * visual_mult, as the solve weights a frame.  The view couples only its own pose and the globals; eliminating the pose
+ * leaves S = C_v - E_v^T B_v^-1 E_v (G x G), and the posterior of the globals is Sigma' = (Sigma^-1 + S)^-1.  F: the rows
+ * of Sigma whose diagonal is not exactly 0.0 (constant globals, a camera no active observation sees).  Corners of a
+ * camera no active observation sees count in n_seen but add nothing; constant globals are masked as the solve masks
+ * them.  Per candidate i:
+ *   n_seen[i][c]  the corners camera c sees;
+ *   gain[i]       1/2 log det(Sigma_F Sigma'_F^-1) = 1/2 log det(I + Sigma_F S_F), the entropy in nats the view removes
+ *                 from the globals, >= 0 (rounding below 0 is clamped to 0.0);
+ *   var[i]        (G, or NULL) diag(Sigma'), exactly 0.0 outside F, bitwise the diagonal of post;
+ *   post[i]       (G x G, or NULL) Sigma', one triangle computed and mirrored (exactly symmetric), 0.0 outside F.
+ * Pass post as globals_cov_or_null of the next call to plan greedily (score, take the best, score it alone with post,
+ * chain), and to vcgpu_get_projection_covariance to map the pixel uncertainty after that view.
+ * A candidate that sees no corner of a used camera gets gain 0.0 and var / post copied from Sigma's bits.  One that sees
+ * 1 to 3 such corners, or whose B_v fails the frame elimination's positive-definiteness test (a Cholesky pivot that is
+ * not positive), gets NaN in gain, var and post: the view does not fix its pose.  n_seen is written either way.
+ * Assumptions: a candidate is a free-pose view.  On an inertial rig it gets no IMU interval, so its gain is what its
+ * images alone add, a lower bound on what an IMU-tied frame would add.  Like Sigma, the result assumes unit observation
+ * variance.
+ * Computation (vc_view_info.cuh): Sigma_F is Jacobi-scaled and factored once per rig; one CTA per candidate projects the
+ * target, builds the view's blocks with the solve's frame build, forms I + L^T S~ L and factors and inverts it in shared
+ * memory.  Nothing on the handle changes: state, IMU weights, the weight update's stored eigenvectors and what a later
+ * vcgpu_solve or batch computes stay as they were. */
+typedef struct {
+  int64_t n_cand;            /* candidates */
+  const double* T_wp;        /* n_cand * 7: q (4) | t (3), |q| within 1e-6 of 1 */
+  int n_pts;                 /* target points, 1 .. 400 (a candidate's corners of 8 cameras fit the CTA's workspace) */
+  const double* p_w;         /* n_pts * 3 */
+  const double* facing;      /* 3, or NULL: every side is the front */
+  const int32_t* width;      /* n_cams image widths, pixels */
+  const int32_t* height;     /* n_cams image heights */
+  int32_t* n_seen;           /* n_cand * n_cams */
+  double* gain;              /* n_cand */
+  double* var_or_null;       /* n_cand * G, or NULL */
+  double* post_or_null;      /* n_cand * G * G, or NULL */
+} vcgpu_view_candidates;
+/* globals_cov_or_null: NULL computes Sigma as vcgpu_get_covariance does; or a G x G matrix in its layout (e.g. a post of
+ * an earlier call), uploaded in place of the elimination.  A given matrix gives the same bits on either path.
+ * VCGPU_ERR_NUMERIC: Sigma_F is not positive definite (as vcgpu_get_covariance's own); nothing is written.
+ * VCGPU_ERR_INVALID, before anything is launched and naming the candidate, point or camera: a null v, n_cand < 0 or
+ * above 2^31 - 1 (one CTA per candidate), with
+ * candidates a null T_wp, p_w, width, height, n_seen or gain, n_pts <= 0 or above 400, a width or height <= 0, a
+ * non-finite p_w, facing or pose entry, a quaternion whose norm is not within 1e-6 of 1, frame shards (one GPU only).
+ * n_cand = 0 writes nothing.
+ * Device memory, held by the handle and grown to the largest call, never freed per call: G^2 + G_F^2 doubles, 56 bytes
+ * per candidate and 24 per point of inputs, per candidate 4 n_cams + 8 bytes of outputs (+ 8 G with var, + 8 G^2 with
+ * post); plus vcgpu_get_covariance's when it computes the matrix. */
+int vcgpu_get_view_information(vcgpu_handle* h, const double* globals_cov_or_null /* G x G */, const vcgpu_view_candidates* v);
+/* vcgpu_get_view_information of n rigs in one call: v[i] are rig i's candidates.  The matrices are
+ * vcgpu_get_covariance_batch's (its cluster kernels), then one prior launch and one candidate launch cover every rig, one
+ * CTA per candidate, so a rig's outputs do not depend, bit for bit, on the rest of the batch or its order, and equal its
+ * single call to rounding.  A rig with n_cand = 0 gets nothing written.
+ * status, VCGPU_ERR_NUMERIC: as vcgpu_get_covariance_batch (and a rig whose Sigma_F is not positive definite); a failing
+ * rig's outputs are not written, every other rig's are.
+ * VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in vcgpu_last_error
+ * of every non-null handle: n <= 0, a null v, a rig vcgpu_get_view_information refuses, more than 2^31 - 1 candidates
+ * in all, and everything
+ * vcgpu_get_covariance_batch refuses.
+ * Device memory: vcgpu_get_covariance_batch's, and held by handle 0 per rig what vcgpu_get_view_information takes and
+ * its kernel arguments. */
+int vcgpu_get_view_information_batch(vcgpu_handle* const* handles, int n, const vcgpu_view_candidates* v,
+                                     int* status /* n, or NULL */);
+
 /* Each IMU interval's Mahalanobis distance, as UpdateImuWeights computes it and logs it against chi2inv(0.95, 9) =
  * 16.9190 (vicalibrator.h:786-794): per interval k (n_frames - 1 of them),
  *   r = [SE3::log(T_end * T_w,k+1^-1) (upsilon 3, omega 3); v_end - v_w[k+1]]   (the reference's `residuals`)

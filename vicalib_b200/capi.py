@@ -31,6 +31,7 @@ EXPORTS = [
     "vcgpu_get_imu_mahalanobis", "vcgpu_get_imu_mahalanobis_batch",
     "vcgpu_get_integration_poses", "vcgpu_get_integration_poses_batch",
     "vcgpu_get_projection_covariance", "vcgpu_get_projection_covariance_batch",
+    "vcgpu_get_view_information", "vcgpu_get_view_information_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -96,6 +97,41 @@ def _proj_points(cam_id, pix, depth, frame, rays):
 def _proj_result(keep, n):
     cov, ray = keep[3][:n], keep[4]
     return cov if ray is None else (cov, ray[:n])
+
+
+class ViewCandidates(C.Structure):
+    """vcgpu_view_candidates: one rig's candidate views, target and outputs of vcgpu_get_view_information(_batch)"""
+    _fields_ = [("n_cand", C.c_int64), ("T_wp", C.c_void_p), ("n_pts", C.c_int), ("p_w", C.c_void_p),
+                ("facing", C.c_void_p), ("width", C.c_void_p), ("height", C.c_void_p), ("n_seen", C.c_void_p),
+                ("gain", C.c_void_p), ("var_or_null", C.c_void_p), ("post_or_null", C.c_void_p)]
+
+
+def _view_candidates(T_wp, p_w, width, height, facing, var, post, n_cams, G):
+    """the arrays of one rig's candidates and a ViewCandidates over them (the arrays must outlive the call)"""
+    T = _c(T_wp).reshape(-1, 7)
+    pw = _c(p_w).reshape(-1, 3)
+    n = len(T)
+    wd = _c(np.broadcast_to(np.asarray(width), (n_cams,)), np.int32)
+    ht = _c(np.broadcast_to(np.asarray(height), (n_cams,)), np.int32)
+    fc = None if facing is None else _c(facing).reshape(3)
+    seen = np.zeros((max(n, 1), n_cams), np.int32)
+    gain = np.zeros(max(n, 1))
+    vr = np.zeros((max(n, 1), G)) if var else None
+    ps = np.zeros((max(n, 1), G, G)) if post else None
+    v = ViewCandidates(n, T.ctypes.data, len(pw), pw.ctypes.data, None if fc is None else fc.ctypes.data, wd.ctypes.data,
+                       ht.ctypes.data, seen.ctypes.data, gain.ctypes.data, None if vr is None else vr.ctypes.data,
+                       None if ps is None else ps.ctypes.data)
+    return (T, pw, wd, ht, fc, seen, gain, vr, ps), v
+
+
+def _view_result(keep, n):
+    """dict(gain, n_seen[, var][, post]) of one rig's call"""
+    out = dict(gain=keep[6][:n], n_seen=keep[5][:n])
+    if keep[7] is not None:
+        out["var"] = keep[7][:n]
+    if keep[8] is not None:
+        out["post"] = keep[8][:n]
+    return out
 
 
 class Flow(C.Structure):
@@ -440,6 +476,19 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_projection_covariance(self.h, _p(S), C.byref(pts)))
         return _proj_result(keep, pts.n)
 
+    def view_information(self, T_wp, p_w, width, height, facing=None, cov=None, var=False, post=False):
+        """The information candidate views of the target would add to the globals (vcgpu_get_view_information):
+        T_wp (n, 7) candidate rig poses (q | t), p_w (m, 3) the target's points in the world frame, width / height
+        each camera's image size (a scalar for all), facing the target's front normal or None.  Returns a dict:
+        gain (n,) the entropy in nats the view removes from the globals (NaN: the view does not fix its pose),
+        n_seen (n, n_cams), and with var=True the posterior variances (n, G), with post=True the posterior matrices
+        (n, G, G).  cov: the G x G prior to use instead of covariance(), e.g. an earlier post.  Nothing on the handle
+        changes."""
+        keep, v = _view_candidates(T_wp, p_w, width, height, facing, var, post, self.n_cams, self.G)
+        S = None if cov is None else _c(cov).reshape(self.G, self.G)
+        self._chk(self.L.vcgpu_get_view_information(self.h, _p(S), C.byref(v)))
+        return _view_result(keep, v.n_cand)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -592,6 +641,36 @@ def projection_covariance_batch(calibrators, points):
         if rc == -3:
             e.status = [st[i] for i in range(n)]
             e.covariances = [out[i] if st[i] == 0 else None for i in range(n)]
+        raise e
+    return out
+
+
+def view_information_batch(calibrators, views):
+    """vcgpu_get_view_information_batch: Calibrator.view_information() of every Calibrator of the list, the priors by
+    covariance_batch's cluster kernels and one candidate launch for all.  views: one dict per calibrator with T_wp,
+    p_w, width, height and optionally facing, var and post.  Returns one dict per calibrator, in order, as
+    view_information() returns it.  Raises VcgpuError as covariance_batch does; its `results` then holds the results
+    of the rigs that were written and None for the others."""
+    n = len(calibrators)
+    if len(views) != n:
+        raise ValueError(f"{len(views)} views for {n} calibrators")
+    L = lib()
+    keeps, arr = [], (ViewCandidates * max(n, 1))()
+    for i, v in enumerate(views):
+        g = calibrators[i]
+        keep, arr[i] = _view_candidates(v["T_wp"], v["p_w"], v["width"], v["height"], v.get("facing"), v.get("var", False),
+                                        v.get("post", False), g.n_cams if g is not None else 1, g.G if g is not None else 1)
+        keeps.append(keep)
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    st = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_view_information_batch(hs, C.c_int(n), arr, st)
+    out = [_view_result(keeps[i], arr[i].n_cand) for i in range(n)]
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:
+            e.status = [st[i] for i in range(n)]
+            e.results = [out[i] if st[i] == 0 else None for i in range(n)]
         raise e
     return out
 

@@ -209,6 +209,9 @@ struct vcgpu_handle {
   // vcgpu_get_projection_covariance(_batch) with this handle as handle 0: every rig's matrix and points, then every
   // rig's outputs (vc_batch.inl: run_proj_cov)
   unsigned char* d_proj = nullptr;
+  // vcgpu_get_view_information(_batch) with this handle as handle 0: every rig's inputs, its factored prior and every
+  // rig's outputs (vc_batch.inl: run_view_info)
+  unsigned char* d_view = nullptr;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

@@ -33,6 +33,7 @@
 #include "vc_pnp.cuh"
 #include "vc_eval_batch.cuh"
 #include "vc_proj_cov.cuh"
+#include "vc_view_info.cuh"
 
 using namespace vc;
 
@@ -222,7 +223,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_view); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -1156,6 +1157,35 @@ extern "C" int vcgpu_get_projection_covariance_batch(vcgpu_handle* const* handle
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!pts) return batch_refuse(handles, n, 0, "null pts array", "vcgpu_get_projection_covariance_batch");
   return run_proj_cov_batch(handles, n, pts, status);
+}
+
+// The information candidate views would add (vc_view_info.cuh): the matrix of vcgpu_get_covariance (run_cov) or the
+// caller's, then run_view_info of this handle alone.  Both paths hand the kernels a host matrix, so a given matrix
+// gives the same bits on either.
+extern "C" int vcgpu_get_view_information(vcgpu_handle* h, const double* globals_cov, const vcgpu_view_candidates* v) {
+  if (!h) return VCGPU_ERR_INVALID;
+  const std::string why = view_refusal(h, v);
+  if (!why.empty()) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_view_information: " + why);
+  if (v->n_cand == 0) return VCGPU_OK;
+  std::vector<double> own;
+  if (!globals_cov) {
+    int G = 0;
+    vcgpu_num_globals(h, &G);
+    own.resize(static_cast<size_t>(G) * G);
+    VC_TRY(run_cov(h, own.data(), kCovGlobals));
+    globals_cov = own.data();
+  } else {
+    VC_TRY(prepare(h));
+  }
+  int st = VCGPU_OK;
+  VC_TRY(run_view_info(&h, 1, &globals_cov, v, &st));
+  if (st != VCGPU_OK) return fail(h, st, "vcgpu_get_view_information: Sigma_F is not positive definite");
+  return VCGPU_OK;
+}
+extern "C" int vcgpu_get_view_information_batch(vcgpu_handle* const* handles, int n, const vcgpu_view_candidates* v, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!v) return batch_refuse(handles, n, 0, "null candidates array", "vcgpu_get_view_information_batch");
+  return run_view_info_batch(handles, n, v, status);
 }
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp

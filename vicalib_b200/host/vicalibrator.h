@@ -534,6 +534,35 @@ class ViCalibrator {
     return cov;
   }
 
+  // The information each candidate view of the target would add to the calibration (vcgpu_get_view_information):
+  // T_wp holds 7 doubles (q | t) per candidate rig pose, p_w 3 per target point in the world frame, facing the target's
+  // front normal (empty: every side is the front).  Each camera's image is its CameraInterface's Width() x Height().
+  // Returns one gain per candidate, the entropy in nats the view removes from the globals (NaN where the view does not
+  // fix its own pose); var (if not null) gets NumGlobals() posterior variances per candidate and n_seen (if not null)
+  // the corners each camera sees.  Call after the solve has finished (not while IsRunning()).
+  std::vector<double> GetViewInformation(const std::vector<double>& T_wp, const std::vector<double>& p_w,
+                                         const std::vector<double>& facing = {}, std::vector<double>* var = nullptr,
+                                         std::vector<int32_t>* n_seen = nullptr) {
+    VICALIB_CHECK(!IsRunning(), "GetViewInformation while running");
+    VICALIB_CHECK(facing.empty() || facing.size() == 3, "GetViewInformation: facing needs 3 values");
+    const int64_t n = static_cast<int64_t>(T_wp.size() / 7);
+    int G = 0;
+    Check(vcgpu_num_globals(h_, &G), "num_globals");
+    std::vector<int32_t> width, height, seen(static_cast<size_t>(n) * cameras_.size());
+    for (const auto& c : cameras_) {
+      width.push_back(c->camera->Width());
+      height.push_back(c->camera->Height());
+    }
+    std::vector<double> gain(n);
+    if (var) var->assign(static_cast<size_t>(n) * G, 0.0);
+    const vcgpu_view_candidates v{n, T_wp.data(), static_cast<int>(p_w.size() / 3), p_w.data(),
+                                  facing.empty() ? nullptr : facing.data(), width.data(), height.data(), seen.data(),
+                                  gain.data(), var ? var->data() : nullptr, nullptr};
+    Check(vcgpu_get_view_information(h_, nullptr, &v), "get_view_information");
+    if (n_seen) *n_seen = seen;
+    return gain;
+  }
+
   // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
   // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
   // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
