@@ -557,6 +557,65 @@ int vcgpu_get_view_information(vcgpu_handle* h, const double* globals_cov_or_nul
 int vcgpu_get_view_information_batch(vcgpu_handle* const* handles, int n, const vcgpu_view_candidates* v,
                                      int* status /* n, or NULL */);
 
+/* Regression diagnostics of every reprojection observation: which corners the calibration rests on, which pull it away
+ * from the rest of the data, and whether a large residual is a bad detection or a corner the model cannot fit.
+ * Observation i has camera c and frame f.  P = (frame f's 6 pose tangents | camera c's 6 + K globals in
+ * vcgpu_get_covariance's layout, w_ck 3 | p_ck 3 | intrinsics K), p = 12 + K.  At the handle's current accepted state:
+ *   J_i, r_i   the loss-free 2 x p Jacobian and residual of vcgpu_eval_reproj, restricted to P; constant globals'
+ *              columns masked as the solve masks them;
+ *   w_i        visual_mult * rho'(|r_i|^2), the solve's SoftLOne weight;  J~ = sqrt(w_i) J_i,  r~ = sqrt(w_i) r_i;
+ *   Sigma_PP   the P x P block of the inverse vcgpu_get_covariance takes (from Sigma_ff, Sigma_fc and Sigma_cc);
+ *   Sigma_F    the globals' covariance on F, the globals whose variance is not exactly 0.0.
+ * Per observation, active or removed by vcgpu_remove_outliers, in caller order (as vcgpu_get_obs_active):
+ *   h[i]     (H_uu, H_uv, H_vv) of the leverage H_i = J~ Sigma_PP J~^T;
+ *   stud[i]  active: r~^T (I - H_i)^-1 r~, the deleted (studentized) residual; removed: r~^T (I + H_i)^-1 r~, the
+ *            predictive residual of a point outside the fit;
+ *   infl[i]  Dg^T Sigma_F^-1 Dg, Dg = Sigma_gP J~^T (I -+ H_i)^-1 r~ (minus: active, plus: removed): the shift of the
+ *            globals that deleting (or re-admitting) the observation causes in the linearised problem at a stationary
+ *            point, measured in the calibration's own uncertainty.
+ * Like every covariance call these assume unit observation variance: divide stud and infl by sigma^2 (e.g. 2 cost /
+ * (n - dim)) before reading either against a chi-square quantile (chi2inv(0.99, 2) = 9.2103 for stud).  h is
+ * scale-free.  On a vision rig the sum of tr(H_i) over the active observations is the number of free tangents: 6 per
+ * used frame plus |F|.
+ * NaN in all three: an observation of a camera no active observation sees, or of a vision frame no active observation
+ * sees (its prediction is not determined).  A frame of an inertial rig stays determined by its IMU intervals.  An active
+ * observation whose I - H_i is not positive definite as computed ((0,0) entry or determinant not > 0): h is written,
+ * stud and infl are NaN.
+ * Computation (vc_obs_infl.cuh): Sigma_gg, Sigma_ff and Sigma_fg from one elimination and selected inversion, as
+ * vcgpu_get_frame_covariance and vcgpu_get_frame_cross_covariance form them, kept on the device; Sigma_F factored once (as
+ * vcgpu_get_view_information's prior); Q_f = Sigma_fF Sigma_F^-1 Sigma_Ff per frame; then one thread per observation
+ * in tiles of at most 64 of one (frame, camera), so infl = a^T M_P a with a = J~^T u and M_P = Sigma_PP with Q_f in
+ * its pose block.  Nothing on the handle changes: state, IMU weights, the weight update's stored eigenvectors and what a
+ * later vcgpu_solve or batch computes stay as they were.
+ * VCGPU_ERR_NUMERIC: where vcgpu_get_covariance returns it, or Sigma_F is not positive definite; nothing is written.
+ * VCGPU_ERR_INVALID: a null handle or out, all three outputs null, frame shards (one GPU only).  Accepts every rig
+ * vcgpu_get_frame_cross_covariance accepts, inertial G >= 68 included.
+ * Device memory, held by the handle and grown to the largest call, never freed per call: vcgpu_get_frame_cross_covariance's
+ * plus n_frames fd^2 doubles for Sigma_ff; G^2 + G_F^2 + 36 n_frames doubles; per observation 49 bytes of inputs (the
+ * observations sorted by (camera, frame), uploaded once and kept until the problem changes) and 24 (h), 8 (stud) and 8
+ * (infl) of outputs; 24 bytes per tile and a few hundred per rig of kernel arguments. */
+typedef struct {
+  double* h;     /* n_obs * 3, or NULL */
+  double* stud;  /* n_obs, or NULL */
+  double* infl;  /* n_obs, or NULL */
+} vcgpu_obs_influence;
+int vcgpu_get_observation_influence(vcgpu_handle* h, vcgpu_obs_influence* out);
+/* vcgpu_get_observation_influence of n rigs in one call: out[i] receives rig i's values.  Sigma_gg, Sigma_ff and
+ * Sigma_fg come from one elimination per rig by the frame cross-covariance batch's cluster kernels in a mode that also
+ * writes the diagonal blocks (one cluster per rig, of the size its batch solve takes), and stay on the device; then one
+ * launch of each influence kernel covers every rig.  A rig's values are the same bits
+ * whatever else is in the batch and in whatever order, and equal its single call to rounding; vision and inertial rigs
+ * may be mixed.
+ * status, VCGPU_ERR_NUMERIC: as vcgpu_get_frame_cross_covariance_batch (and a rig whose Sigma_F is not positive definite);
+ * a failing rig's outputs are not written, every other rig's are.
+ * VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in vcgpu_last_error
+ * of every non-null handle: n <= 0, a null out, a rig vcgpu_get_observation_influence refuses, and everything
+ * vcgpu_get_frame_cross_covariance_batch refuses (a rig with no active observation, inertial G >= 68 on an H100).
+ * Device memory: per handle what vcgpu_get_observation_influence keeps and vcgpu_get_covariance_batch's workspace; held by
+ * handle 0 per rig G^2 + G_F^2 + 36 n_frames doubles, the outputs and the kernel arguments. */
+int vcgpu_get_observation_influence_batch(vcgpu_handle* const* handles, int n, const vcgpu_obs_influence* out,
+                                          int* status /* n, or NULL */);
+
 /* Each IMU interval's Mahalanobis distance, as UpdateImuWeights computes it and logs it against chi2inv(0.95, 9) =
  * 16.9190 (vicalibrator.h:786-794): per interval k (n_frames - 1 of them),
  *   r = [SE3::log(T_end * T_w,k+1^-1) (upsilon 3, omega 3); v_end - v_w[k+1]]   (the reference's `residuals`)

@@ -32,6 +32,7 @@ EXPORTS = [
     "vcgpu_get_integration_poses", "vcgpu_get_integration_poses_batch",
     "vcgpu_get_projection_covariance", "vcgpu_get_projection_covariance_batch",
     "vcgpu_get_view_information", "vcgpu_get_view_information_batch",
+    "vcgpu_get_observation_influence", "vcgpu_get_observation_influence_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -132,6 +133,23 @@ def _view_result(keep, n):
     if keep[8] is not None:
         out["post"] = keep[8][:n]
     return out
+
+
+class ObsInfluence(C.Structure):
+    """vcgpu_obs_influence: one rig's outputs of vcgpu_get_observation_influence(_batch), any of them NULL"""
+    _fields_ = [("h", C.c_void_p), ("stud", C.c_void_p), ("infl", C.c_void_p)]
+
+
+def _obs_influence(n_obs, h, stud, infl):
+    """the output arrays of one rig and an ObsInfluence over them (the arrays must outlive the call)"""
+    m = max(n_obs, 1)
+    keep = (np.zeros((m, 3)) if h else None, np.zeros(m) if stud else None, np.zeros(m) if infl else None)
+    return keep, ObsInfluence(*[None if a is None else a.ctypes.data for a in keep])
+
+
+def _obs_influence_result(keep, n_obs):
+    """dict(h[, stud][, infl]) of one rig's call"""
+    return {k: a[:n_obs] for k, a in zip(("h", "stud", "infl"), keep) if a is not None}
 
 
 class Flow(C.Structure):
@@ -489,6 +507,18 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_view_information(self.h, _p(S), C.byref(v)))
         return _view_result(keep, v.n_cand)
 
+    def observation_influence(self, h=True, stud=True, infl=True):
+        """Regression diagnostics of every reprojection observation, active or removed, in upload order
+        (vcgpu_get_observation_influence): h (n, 3) the leverage H_uu, H_uv, H_vv; stud (n,) the studentized (deleted)
+        residual, or for a removed observation its predictive residual; infl (n,) the shift of the globals its deletion
+        (or re-admission) causes, measured in the globals' covariance.  stud and infl assume unit observation variance:
+        divide by the residual variance before reading them against chi-square quantiles.  NaN where the observation's
+        camera or vision frame is not determined.  Only the outputs asked for are returned.  Nothing on the handle
+        changes."""
+        keep, o = _obs_influence(self.n_obs, h, stud, infl)
+        self._chk(self.L.vcgpu_get_observation_influence(self.h, C.byref(o)))
+        return _obs_influence_result(keep, self.n_obs)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -665,6 +695,31 @@ def view_information_batch(calibrators, views):
     st = (C.c_int * max(n, 1))()
     rc = L.vcgpu_get_view_information_batch(hs, C.c_int(n), arr, st)
     out = [_view_result(keeps[i], arr[i].n_cand) for i in range(n)]
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:
+            e.status = [st[i] for i in range(n)]
+            e.results = [out[i] if st[i] == 0 else None for i in range(n)]
+        raise e
+    return out
+
+
+def observation_influence_batch(calibrators, h=True, stud=True, infl=True):
+    """vcgpu_get_observation_influence_batch: Calibrator.observation_influence() of every Calibrator of the list (vision
+    and inertial rigs may be mixed), the covariance blocks from one elimination per rig by the cluster kernels and one launch of
+    each influence kernel for all.  Returns one dict per calibrator, in order.  Raises VcgpuError as covariance_batch
+    does; its `results` then holds the results of the rigs that were written and None for the others."""
+    n = len(calibrators)
+    L = lib()
+    keeps, arr = [], (ObsInfluence * max(n, 1))()
+    for i, g in enumerate(calibrators):
+        keep, arr[i] = _obs_influence(g.n_obs if g is not None else 0, h, stud, infl)
+        keeps.append(keep)
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    st = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_observation_influence_batch(hs, C.c_int(n), arr, st)
+    out = [_obs_influence_result(keeps[i], calibrators[i].n_obs if calibrators[i] is not None else 0) for i in range(n)]
     if rc != 0:
         msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
         e = VcgpuError(f"vcgpu error {rc}: {msg}")

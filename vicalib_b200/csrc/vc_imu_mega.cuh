@@ -1635,6 +1635,8 @@ struct ChainCovArgs {
   // cross mode (chain_frame_cross_cov_batch_kernel): frame mode's, with out Σ_fg [nf][9][G] and out_next Σ_f,f+1
   // [nf - 1][81]
   double* out_next;
+  // diagonal and cross mode (chain_frame_diag_cross_cov_batch_kernel): cross mode's, and out_ff Σ_ff [nf][81]
+  double* out_ff;
 };
 // A batch of inertial rigs, one thread-block cluster each: cluster k writes the covariance of args[k] (vcgpu_get_covariance_batch).
 __global__ void __launch_bounds__(kCsThreads, 1) chain_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
@@ -1743,6 +1745,20 @@ __global__ void __launch_bounds__(kCsThreads, 1) chain_frame_cross_cov_batch_ker
     const int G = a.s.dp.G;
     for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < frame_cross_cov_entries<FD>(nf, G); e += static_cast<int64_t>(nb) * kCsThreads)
       frame_cross_cov_out_entry<FD>(e, nf, G, a.live, a.sig[0], a.s.scale, a.mask, a.out, a.out_next);
+  });
+}
+// ... both: level 0's Σ_kk, Σ_kg and Σ_k,k+1 unscaled, from one walk (vcgpu_get_observation_influence_batch)
+__global__ void __launch_bounds__(kCsThreads, 1) chain_frame_diag_cross_cov_batch_kernel(const ChainCovArgs* __restrict__ args) {
+  constexpr int FD = 9;
+  ClusterScope scope;
+  const ChainCovArgs& a = args[blockIdx.x / scope.nb()];
+  chain_frame_cov_walk(a, scope, [&](int tid, int bid, int nb, int nf) {
+    const int G = a.s.dp.G;
+    const int64_t nd = static_cast<int64_t>(nf) * FD * FD, nc = frame_cross_cov_entries<FD>(nf, G);
+    for (int64_t e = static_cast<int64_t>(bid) * kCsThreads + tid; e < nd + nc; e += static_cast<int64_t>(nb) * kCsThreads) {
+      if (e < nd) a.out_ff[e] = frame_cov_out_entry<FD>(e, a.live, a.sig[0].kk, a.s.scale);
+      else frame_cross_cov_out_entry<FD>(e - nd, nf, G, a.live, a.sig[0], a.s.scale, a.mask, a.out, a.out_next);
+    }
   });
 }
 

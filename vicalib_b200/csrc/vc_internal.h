@@ -27,6 +27,12 @@ constexpr int kImuProfSlots = 64;   // phase clock slots of the persistent inert
 
 constexpr int kFreeCam = 3, kFreeImu = kFreeCam * kMaxCams;  // DevProblem::free_blocks
 
+// one tile of infl_obs_kernel (vc_obs_infl.cuh): sorted observations [start, start + count) of camera cam in frame f
+struct InflTile {
+  int64_t start;
+  int rig, cam, frame, count;
+};
+
 struct CamInfo {
   int model, K;
   int goff;         // offset of [w_ck p_ck intr] in the global tangent vector
@@ -212,6 +218,14 @@ struct vcgpu_handle {
   // vcgpu_get_view_information(_batch) with this handle as handle 0: every rig's inputs, its factored prior and every
   // rig's outputs (vc_batch.inl: run_view_info)
   unsigned char* d_view = nullptr;
+  // vcgpu_get_observation_influence(_batch) with this handle as handle 0: the argument tables, every rig's covariance
+  // blocks and sorted observations, its factored prior and Q_f, then the flags and every rig's outputs (run_obs_infl)
+  unsigned char* d_infl = nullptr;
+  // vcgpu_get_observation_influence(_batch): every observation of this handle, removed ones included, sorted by (camera,
+  // frame) with its caller index and active flag, and its tiles; valid until prepare() rebuilds the problem
+  unsigned char* d_infl_obs = nullptr;
+  std::vector<vc::InflTile> infl_tiles;
+  bool infl_obs_valid = false;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

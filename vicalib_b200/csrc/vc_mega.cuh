@@ -938,6 +938,8 @@ struct CovArgs {
   // cross mode (cov_frame_cross_mega_batch_kernel): frame mode's D2x and frame_used; fcov Σ_fg [nf][6][G], fcov_next
   // Σ_f,f+1 [nf - 1][36]
   double* fcov_next;
+  // diagonal and cross mode (cov_frame_diag_cross_mega_batch_kernel): cross mode's, and fcov_diag Σ_ff [nf][36]
+  double* fcov_diag;
 };
 // dynamic shared memory of cov_mega_batch_kernel: per warp its frame's scaled [E | g] and X, the reduced system, pivots
 __host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
@@ -949,8 +951,9 @@ __host__ __device__ inline size_t cov_mega_smem_doubles(int G, int n_warps) {
 // warps share the right-hand sides.  kCovGlobals: the covariance of the globals.  kCovFrames: all G unit right-hand
 // sides give Σ_gg; after a cluster barrier one warp per frame refactors B_f, forms X_f = B_f^-1 E_f again and writes
 // B_f^-1 + X_f Σ_gg X_f^T (frame_cov_block).  kCovCross: as kCovFrames, but the warp forms X_f and X_f+1 and writes
-// -X_f Σ_gg and X_f Σ_gg X_f+1^T (frame_cross_cov_block).
-enum CovMode { kCovGlobals, kCovFrames, kCovCross };
+// -X_f Σ_gg and X_f Σ_gg X_f+1^T (frame_cross_cov_block).  kCovDiagCross: kCovFrames' pass into fcov_diag, then
+// kCovCross' pass: one elimination leaves Σ_gg, Σ_ff and Σ_fg on the device (vcgpu_get_observation_influence_batch).
+enum CovMode { kCovGlobals, kCovFrames, kCovCross, kCovDiagCross };
 template <CovMode kMode>
 __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
   extern __shared__ double smem[];
@@ -1071,10 +1074,12 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
         if (32 * q + lane < G) a.cov[static_cast<int64_t>(32 * q + lane) * G + j] = x[q];
     }
     scope.sync();
-    if constexpr (kMode == kCovFrames) {
+    if constexpr (kMode == kCovFrames || kMode == kCovDiagCross) {
+      // kCovDiagCross: the diagonal blocks first, in their own pass (X_f formed again: held across both products, the
+      // two blocks' registers spill)
       for (int k = warp; k < nk; k += nwarps) {
         const int f = bid + k * nb;
-        double* out = a.fcov + static_cast<int64_t>(f) * FD * FD;
+        double* out = (kMode == kCovFrames ? a.fcov : a.fcov_diag) + static_cast<int64_t>(f) * FD * FD;
         if (!a.frame_used[f]) {
           for (int e = lane; e < FD * FD; e += 32) out[e] = 0.0;
           continue;
@@ -1086,7 +1091,8 @@ __device__ __forceinline__ void cov_mega(const CovArgs& a, ClusterScope scope) {
         frame_cov_block<FD>(a.b, a.D2x, f, a.scale + static_cast<int64_t>(f) * FD, Xw, M, a.cov, G, lane, out);
         __syncwarp();
       }
-    } else {
+    }
+    if constexpr (kMode == kCovCross || kMode == kCovDiagCross) {
       // X_f into the warp's second slot, X_f+1 (its owner's bits: the same routine on the same inputs) into its first
       for (int k = warp; k < nk; k += nwarps) {
         const int f = bid + k * nb;
@@ -1126,6 +1132,11 @@ __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_mega_batch_kerne
 __global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_cross_mega_batch_kernel(const CovArgs* __restrict__ args) {
   ClusterScope scope;
   cov_mega<kCovCross>(args[blockIdx.x / scope.nb()], scope);
+}
+// ... the frame blocks on and off the diagonal of args[k] from one elimination (vcgpu_get_observation_influence_batch)
+__global__ void __launch_bounds__(kMegaMaxThreads, 1) cov_frame_diag_cross_mega_batch_kernel(const CovArgs* __restrict__ args) {
+  ClusterScope scope;
+  cov_mega<kCovDiagCross>(args[blockIdx.x / scope.nb()], scope);
 }
 
 }  // namespace vc

@@ -34,6 +34,7 @@
 #include "vc_eval_batch.cuh"
 #include "vc_proj_cov.cuh"
 #include "vc_view_info.cuh"
+#include "vc_obs_infl.cuh"
 
 using namespace vc;
 
@@ -223,7 +224,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_view); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_view); dev_free(&h->d_infl); dev_free(&h->d_infl_obs); h->infl_obs_valid = false; dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -522,6 +523,7 @@ static int prepare(vcgpu_handle* h) {
   CUDA_TRY(h, cudaSetDevice(h->device));
   if (h->n_cams <= 0 || h->n_frames <= 0) return fail(h, VCGPU_ERR_INVALID, "cameras and frames must be set first");
   if (h->dirty) {
+    h->infl_obs_valid = false;  // vcgpu_get_observation_influence's sorted copy of the observations
     DevProblem& dp = h->dp;
     std::memset(&dp, 0, sizeof dp);
     dp.n_cams = h->n_cams;
@@ -997,6 +999,11 @@ static int cov_vision(vcgpu_handle* h, const double* D2x, CovMode mode, const Co
     if (mode == kCovFrames) vc::frame_cov_vision_kernel<6><<<grid, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
     else vc::frame_cross_cov_vision_kernel<6><<<grid, 32 * vc::kFrameCovWarps, 0, h->stream>>>({fa, h->d_mask, w.out_next});
     ++h->launches;
+    if (mode == kCovDiagCross) {  // the diagonal blocks too, from the same X_f and Σ_gg
+      fa.out = w.out_ff;
+      vc::frame_cov_vision_kernel<6><<<grid, 32 * vc::kFrameCovWarps, 0, h->stream>>>(fa);
+      ++h->launches;
+    }
   }
   CUDA_TRY(h, cudaGetLastError());
   return VCGPU_OK;
@@ -1024,10 +1031,12 @@ static int cov_inertial(vcgpu_handle* h, const double* D2x, CovMode mode, int li
     vc::chain_selinv_kernel<FD><<<d->levels[l + 1].n, vc::kChainThreads, sm, h->stream>>>(sa);
     ++h->launches;
   }
-  if (mode == kCovFrames) {
+  if (mode == kCovFrames || mode == kCovDiagCross) {
     const int64_t ne = static_cast<int64_t>(dp.n_frames) * FD * FD;
-    vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, w.sig[0].kk, h->d_scale, w.out);
-  } else {
+    vc::frame_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, live, w.sig[0].kk, h->d_scale, w.out_ff);
+  }
+  if (mode == kCovDiagCross) ++h->launches;
+  if (mode != kCovFrames) {
     const int64_t ne = vc::frame_cross_cov_entries<FD>(dp.n_frames, G);
     vc::frame_cross_cov_out_kernel<FD><<<static_cast<int>((ne + 255) / 256), 256, 0, h->stream>>>(dp.n_frames, G, live, w.sig[0], h->d_scale,
                                                                                                   h->d_mask, w.out, w.out_next);
@@ -1041,7 +1050,9 @@ static int cov_inertial(vcgpu_handle* h, const double* D2x, CovMode mode, int li
 // (kCovCross) of one handle, the per-handle counterpart of run_cov_batch: cov_prelude, the frames' elimination and one
 // inversion of the system it leaves; the globals' block of that inverse, or the frames' blocks from it.  kCovCross:
 // Σ_fg into cov and Σ_f,f+1 into cov_next, either of them null.  Writes no state buffer.
-static int run_cov(vcgpu_handle* h, double* cov, CovMode mode, double* cov_next = nullptr) {
+// kCovDiagCross: cov is not read; the workspace, with Σ_gg (scaled, in inv), Σ_fg (out) and Σ_ff (out_ff) on the device,
+// goes to *keep.
+static int run_cov(vcgpu_handle* h, double* cov, CovMode mode, double* cov_next = nullptr, CovSpace* keep = nullptr) {
   VC_TRY(prepare(h));
   const bool frames = mode != kCovGlobals;
   std::vector<double> D2;
@@ -1064,8 +1075,13 @@ static int run_cov(vcgpu_handle* h, double* cov, CovMode mode, double* cov_next 
   }
   VC_TRY(read_scalars(h));
   if (h->h_scalars[kScNotPD] > 0)
-    return fail(h, VCGPU_ERR_NUMERIC, std::string(mode == kCovCross ? "frame cross covariance" : frames ? "frame covariance" : "covariance") +
+    return fail(h, VCGPU_ERR_NUMERIC, std::string(mode == kCovCross ? "frame cross covariance" : mode == kCovDiagCross ? "observation influence"
+                                                  : frames ? "frame covariance" : "covariance") +
                                           ": J^T J is singular at the current state");
+  if (mode == kCovDiagCross) {
+    *keep = w;
+    return VCGPU_OK;
+  }
   if (mode == kCovFrames) {
     CUDA_TRY(h, cudaMemcpy(cov, w.out, nfp * dp.fd * sizeof(double), cudaMemcpyDeviceToHost));
     return VCGPU_OK;
@@ -1187,6 +1203,28 @@ extern "C" int vcgpu_get_view_information_batch(vcgpu_handle* const* handles, in
   if (!v) return batch_refuse(handles, n, 0, "null candidates array", "vcgpu_get_view_information_batch");
   return run_view_info_batch(handles, n, v, status);
 }
+
+// The regression diagnostics of every reprojection observation (vc_obs_infl.cuh): Σ_gg, Σ_ff and Σ_fg from one
+// elimination and selected inversion of this handle (run_cov, kCovDiagCross; Σ_ff and Σ_fg stay on the device), then
+// run_obs_infl of this handle alone.
+extern "C" int vcgpu_get_observation_influence(vcgpu_handle* h, vcgpu_obs_influence* out) {
+  if (!h) return VCGPU_ERR_INVALID;
+  const std::string why = infl_refusal(h, out);
+  if (!why.empty()) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_observation_influence: " + why);
+  CovSpace w;
+  VC_TRY(run_cov(h, nullptr, kCovDiagCross, nullptr, &w));
+  const InflSrc src{w.inv, w.N, w.out_ff, w.out};
+  int st = VCGPU_OK;
+  VC_TRY(run_obs_infl(&h, 1, &src, out, &st));
+  if (st != VCGPU_OK) return fail(h, st, "vcgpu_get_observation_influence: Sigma_F is not positive definite");
+  return VCGPU_OK;
+}
+extern "C" int vcgpu_get_observation_influence_batch(vcgpu_handle* const* handles, int n, const vcgpu_obs_influence* out, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!out) return batch_refuse(handles, n, 0, "null out array", "vcgpu_get_observation_influence_batch");
+  return run_obs_infl_batch(handles, n, out, status);
+}
+
 
 // Batched PosePnPRansac (vicalib-task.cc:322-325): pose of the planar target in every (frame, camera) view, one warp
 // per view (vc_pnp.cuh): run_pnp_batch of this handle alone.  Cameras (model, intrinsics) are the ones given to

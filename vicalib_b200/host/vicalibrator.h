@@ -563,6 +563,23 @@ class ViCalibrator {
     return gain;
   }
 
+  // The regression diagnostics of every observation, active or removed, in upload order
+  // (vcgpu_get_observation_influence): h 3 doubles per observation (H_uu, H_uv, H_vv of the leverage), stud the
+  // studentized residual (a removed observation's predictive residual), infl the shift of the calibration its deletion
+  // causes, measured in the calibration's covariance.  stud and infl assume unit observation variance.  Any output may
+  // be null, not all three.  The outputs cover the observations the solve was given (the last upload), which after a
+  // Clear() may differ from those added since.
+  void GetObservationInfluence(std::vector<double>* h, std::vector<double>* stud, std::vector<double>* infl) {
+    VICALIB_CHECK(!IsRunning(), "GetObservationInfluence while running");
+    VICALIB_CHECK(h || stud || infl, "GetObservationInfluence: every output is null");
+    const size_t n = n_uploaded_obs_;
+    if (h) h->assign(3 * n, 0.0);
+    if (stud) stud->assign(n, 0.0);
+    if (infl) infl->assign(n, 0.0);
+    vcgpu_obs_influence out{h ? h->data() : nullptr, stud ? stud->data() : nullptr, infl ? infl->data() : nullptr};
+    Check(vcgpu_get_observation_influence(h_, &out), "get_observation_influence");
+  }
+
   // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
   // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
   // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
@@ -693,6 +710,7 @@ class ViCalibrator {
     if (!problem_uploaded_) {  // residual blocks are added once; later stages only change masks / multiplicities
       Check(vcgpu_set_observations(h_, static_cast<int64_t>(obs_frame_.size()), obs_frame_.data(), obs_cam_.data(),
                                    obs_pw_.data(), obs_pc_.data()), "set_observations");
+      n_uploaded_obs_ = obs_frame_.size();
       std::vector<double> t(imu_.size()), w(3 * imu_.size()), a(3 * imu_.size());
       for (size_t i = 0; i < imu_.size(); ++i) {
         t[i] = imu_[i].time;
@@ -940,6 +958,7 @@ class ViCalibrator {
   bool thread_valid_ = false;
   volatile bool should_run_ = false, is_running_ = false, stopped_by_user_ = false;
   bool fix_intrinsics_ = false, problem_uploaded_ = false, emulate_block_duplication_ = true;
+  size_t n_uploaded_obs_ = 0;  // observations the handle holds (GetObservationInfluence's output size); Clear() keeps it
   int visual_adds_ = 0, imu_adds_ = 0;
   std::vector<std::shared_ptr<VicalibFrame> > t_wk_;
   std::vector<std::unique_ptr<CameraAndPose> > cameras_;
