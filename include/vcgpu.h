@@ -616,6 +616,74 @@ int vcgpu_get_observation_influence(vcgpu_handle* h, vcgpu_obs_influence* out);
 int vcgpu_get_observation_influence_batch(vcgpu_handle* const* handles, int n, const vcgpu_obs_influence* out,
                                           int* status /* n, or NULL */);
 
+/* Regression diagnostics of every IMU interval: which intervals the calibration rests on and which pull the gravity,
+ * biases, scale factors or time offset towards themselves.  Interval k = 0 .. n_frames - 2 (the indexing of
+ * vcgpu_get_imu_mahalanobis and vcgpu_eval_imu) touches P = (frame k: pose 6, v 3 | frame k+1: pose 6, v 3 | IMU
+ * globals g 2, b 6, sf 6, ts 1), p = 33; the frame rows follow vcgpu_normal_equations' B, the IMU globals are
+ * vcgpu_get_covariance's columns at the IMU offset.  At the handle's current accepted state, with its current IMU weights:
+ *   r_w, J_w   the interval's residual (r^T W)^T and its 9 x 33 tangent Jacobian, loss-free, as vcgpu_eval_imu returns
+ *              them (rows 0-2 and 6-8 zero in rotation-only stages); constant IMU globals' columns masked as the solve
+ *              masks them;
+ *   w          imu_mult * rho'(|r_w|^2), CauchyLoss(100) (rho' = 1 / (1 + s / 1e4)), the solve's weight;
+ *              J~ = sqrt(w) J_w,  r~ = sqrt(w) r_w;
+ *   Sigma_PP   the 33 x 33 block of the inverse vcgpu_get_covariance takes (from Sigma_kk, Sigma_k+1,k+1, Sigma_k,k+1,
+ *              Sigma_kg, Sigma_k+1,g and Sigma_gg);
+ *   Sigma_F    the globals' covariance on F, the globals whose variance is not exactly 0.0.
+ * Per interval:
+ *   h[k]     81 doubles, H_k = J~ Sigma_PP J~^T row-major in the rows of r_w; one triangle formed and mirrored, so it is
+ *            exactly symmetric;
+ *   stud[k]  r~^T (I - H_k)^-1 r~, the deleted (studentized) residual;
+ *   infl[k]  Dg^T Sigma_F^-1 Dg, Dg = Sigma_FP J~^T (I - H_k)^-1 r~: the shift of the globals that deleting the interval
+ *            causes in the linearised problem at a stationary point, measured in the calibration's own uncertainty; the
+ *            observation call's metric, so intervals and corners can be ranked together.
+ * vcgpu_get_imu_mahalanobis measures an interval's residual against the integration covariance, the noise model
+ * UpdateImuWeights builds; stud measures it against what the fit leaves when the interval is taken out.  An interval
+ * that pulls the fit towards itself keeps a small residual and a small Mahalanobis distance, but not a small stud.
+ * Like every covariance call these assume unit observation variance: divide stud and infl by sigma^2 before reading stud
+ * against a chi-square quantile with 9 degrees of freedom (chi2inv(0.99, 9) = 21.666), or 3 in rotation-only stages,
+ * which keep the attitude rows 3-5 only.  h is scale-free.  On an inertial rig, sum tr(H_obs) over the active observations
+ * plus sum tr(H_k) is the number of free tangents: 9 per frame (6 rotation-only) plus |F|.
+ * Exact cases: an interval with no measurements gets NaN in all three (the solve gives it a zero residual and Jacobian,
+ * and vcgpu_get_imu_mahalanobis returns NaN there).  In rotation-only runs rows and columns 0-2 and 6-8 of H_k are exactly
+ * 0.0.  Where I - H_k fails a pivot test of its Cholesky factorisation (a pivot not > 0), h is written, stud and infl are
+ * NaN; typically an interval that alone fixes a direction: the last interval of a last frame no active observation sees
+ * has H_k = I, and the interval before it three unit leverages (it alone fixes the velocity of the frame between).  Near
+ * that boundary the test follows H_k's rounding, which on inertial rigs can reach 1e-4 where H_k cancels large terms.
+ * obs_or_null: vcgpu_get_observation_influence's outputs, the same bits, from the same elimination: a caller who screens
+ * both kinds of residual pays for one elimination.
+ * Computation (vc_imu_infl.cuh): the covariance blocks as vcgpu_get_observation_influence forms them, Sigma_f,f+1 too;
+ * the intervals' weighted rows by the solve's IMU evaluation into the call's own buffers; then one CTA per interval:
+ * Sigma_PP and J~ in shared memory, H, a 9 x 9 Cholesky of I - H, a = J~^T u, Dg = Sigma_FP a and a triangular solve with
+ * the factor of Sigma_F.  Nothing on the handle changes: state, IMU weights, the weight update's stored eigenvectors and
+ * what a later vcgpu_solve or batch computes stay as they were.
+ * VCGPU_ERR_NUMERIC: where vcgpu_get_covariance returns it, or Sigma_F is not positive definite; nothing is written.
+ * VCGPU_ERR_INVALID, before anything is launched and with nothing written: a null handle or imu, all three IMU outputs
+ * null, inertial terms off, fewer than two frames, frame shards (one GPU only), or obs_or_null refused as
+ * vcgpu_get_observation_influence refuses it.  Accepts inertial G >= 68.
+ * Device memory, held by the handle and grown to the largest call, never freed per call: vcgpu_get_observation_influence's
+ * (its per-observation part only with obs_or_null); per interval 2456 bytes of weighted rows, and 648 (h), 8 (stud) and
+ * 8 (infl) of outputs; a few hundred bytes per rig of kernel arguments. */
+typedef struct {
+  double* h;     /* (n_frames - 1) * 81, or NULL */
+  double* stud;  /* n_frames - 1, or NULL */
+  double* infl;  /* n_frames - 1, or NULL */
+} vcgpu_imu_influence;
+int vcgpu_get_imu_influence(vcgpu_handle* h, vcgpu_imu_influence* imu, vcgpu_obs_influence* obs_or_null);
+/* vcgpu_get_imu_influence of n rigs in one call: imu[i] (and obs_or_null[i]) receive rig i's values.  The covariance
+ * blocks come from the frame cross-covariance batch's cluster kernels, as vcgpu_get_observation_influence_batch takes
+ * them; then one IMU evaluation per rig and one launch of each influence kernel covers every rig.  A rig's values are
+ * the same bits whatever else is in the batch and in whatever order, and equal its single call to rounding; obs
+ * outputs are the bits vcgpu_get_observation_influence_batch returns.
+ * status, VCGPU_ERR_NUMERIC: as vcgpu_get_observation_influence_batch; a failing rig's outputs are not written, every
+ * other rig's are.
+ * VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in vcgpu_last_error
+ * of every non-null handle: n <= 0, a null imu, a rig vcgpu_get_imu_influence refuses (a vision rig among them), and
+ * everything vcgpu_get_frame_cross_covariance_batch refuses (inertial G >= 68 on an H100).
+ * Device memory: per handle vcgpu_get_covariance_batch's workspace and what vcgpu_get_imu_influence keeps; held by
+ * handle 0 what vcgpu_get_imu_influence takes for every rig. */
+int vcgpu_get_imu_influence_batch(vcgpu_handle* const* handles, int n, const vcgpu_imu_influence* imu,
+                                  const vcgpu_obs_influence* obs_or_null /* n, or NULL */, int* status /* n, or NULL */);
+
 /* Each IMU interval's Mahalanobis distance, as UpdateImuWeights computes it and logs it against chi2inv(0.95, 9) =
  * 16.9190 (vicalibrator.h:786-794): per interval k (n_frames - 1 of them),
  *   r = [SE3::log(T_end * T_w,k+1^-1) (upsilon 3, omega 3); v_end - v_w[k+1]]   (the reference's `residuals`)

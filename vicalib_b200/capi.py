@@ -33,6 +33,7 @@ EXPORTS = [
     "vcgpu_get_projection_covariance", "vcgpu_get_projection_covariance_batch",
     "vcgpu_get_view_information", "vcgpu_get_view_information_batch",
     "vcgpu_get_observation_influence", "vcgpu_get_observation_influence_batch",
+    "vcgpu_get_imu_influence", "vcgpu_get_imu_influence_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -150,6 +151,26 @@ def _obs_influence(n_obs, h, stud, infl):
 def _obs_influence_result(keep, n_obs):
     """dict(h[, stud][, infl]) of one rig's call"""
     return {k: a[:n_obs] for k, a in zip(("h", "stud", "infl"), keep) if a is not None}
+
+
+class ImuInfluence(C.Structure):
+    """vcgpu_imu_influence: one rig's outputs of vcgpu_get_imu_influence(_batch), any of them NULL"""
+    _fields_ = [("h", C.c_void_p), ("stud", C.c_void_p), ("infl", C.c_void_p)]
+
+
+def _imu_influence(ni, h, stud, infl):
+    """the output arrays of one rig's intervals and an ImuInfluence over them (the arrays must outlive the call)"""
+    m = max(ni, 1)
+    keep = (np.zeros((m, 9, 9)) if h else None, np.zeros(m) if stud else None, np.zeros(m) if infl else None)
+    return keep, ImuInfluence(*[None if a is None else a.ctypes.data for a in keep])
+
+
+def _imu_influence_result(keep, ni, obs_keep, n_obs):
+    """dict(h[, stud][, infl][, observations]) of one rig's call"""
+    out = {k: a[:ni] for k, a in zip(("h", "stud", "infl"), keep) if a is not None}
+    if obs_keep is not None:
+        out["observations"] = _obs_influence_result(obs_keep, n_obs)
+    return out
 
 
 class Flow(C.Structure):
@@ -519,6 +540,19 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_observation_influence(self.h, C.byref(o)))
         return _obs_influence_result(keep, self.n_obs)
 
+    def imu_influence(self, h=True, stud=True, infl=True, observations=False):
+        """Regression diagnostics of every IMU interval k = 0 .. n_frames - 2 (vcgpu_get_imu_influence): h (n, 9, 9) the
+        leverage H_k; stud (n,) the studentized (deleted) residual; infl (n,) the shift of the globals the interval's
+        deletion causes, measured in the globals' covariance (the observation call's metric).  stud and infl assume unit
+        observation variance.  NaN in all three for an interval with no measurements; stud and infl NaN where I - H_k is
+        not positive definite.  observations=True adds "observations", observation_influence()'s dict from the same
+        elimination.  Only the outputs asked for are returned.  Nothing on the handle changes."""
+        ni = max(self.n_frames - 1, 0)
+        keep, o = _imu_influence(ni, h, stud, infl)
+        okeep, oo = _obs_influence(self.n_obs, True, True, True) if observations else (None, None)
+        self._chk(self.L.vcgpu_get_imu_influence(self.h, C.byref(o), C.byref(oo) if observations else None))
+        return _imu_influence_result(keep, ni, okeep, self.n_obs)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -720,6 +754,38 @@ def observation_influence_batch(calibrators, h=True, stud=True, infl=True):
     st = (C.c_int * max(n, 1))()
     rc = L.vcgpu_get_observation_influence_batch(hs, C.c_int(n), arr, st)
     out = [_obs_influence_result(keeps[i], calibrators[i].n_obs if calibrators[i] is not None else 0) for i in range(n)]
+    if rc != 0:
+        msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
+        e = VcgpuError(f"vcgpu error {rc}: {msg}")
+        if rc == -3:
+            e.status = [st[i] for i in range(n)]
+            e.results = [out[i] if st[i] == 0 else None for i in range(n)]
+        raise e
+    return out
+
+
+def imu_influence_batch(calibrators, h=True, stud=True, infl=True, observations=False):
+    """vcgpu_get_imu_influence_batch: Calibrator.imu_influence() of every Calibrator of the list (inertial rigs), the
+    covariance blocks from one elimination per rig by the cluster kernels and one launch of each influence kernel for
+    all.  Returns one dict per calibrator, in order.  Raises VcgpuError as covariance_batch does; its `results` then
+    holds the results of the rigs that were written and None for the others."""
+    n = len(calibrators)
+    L = lib()
+    ni = [max(g.n_frames - 1, 0) if g is not None else 0 for g in calibrators]
+    no = [g.n_obs if g is not None else 0 for g in calibrators]
+    keeps, okeeps = [], []
+    arr, oarr = (ImuInfluence * max(n, 1))(), (ObsInfluence * max(n, 1))()
+    for i in range(n):
+        keep, arr[i] = _imu_influence(ni[i], h, stud, infl)
+        keeps.append(keep)
+        okeep = None
+        if observations:
+            okeep, oarr[i] = _obs_influence(no[i], True, True, True)
+        okeeps.append(okeep)
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    st = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_get_imu_influence_batch(hs, C.c_int(n), arr, oarr if observations else None, st)
+    out = [_imu_influence_result(keeps[i], ni[i], okeeps[i], no[i]) for i in range(n)]
     if rc != 0:
         msg = next((L.vcgpu_last_error(g.h).decode() for g in calibrators if g is not None and g.h.value), "")
         e = VcgpuError(f"vcgpu error {rc}: {msg}")

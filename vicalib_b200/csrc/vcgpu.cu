@@ -35,6 +35,7 @@
 #include "vc_proj_cov.cuh"
 #include "vc_view_info.cuh"
 #include "vc_obs_infl.cuh"
+#include "vc_imu_infl.cuh"
 
 using namespace vc;
 
@@ -1213,7 +1214,7 @@ extern "C" int vcgpu_get_observation_influence(vcgpu_handle* h, vcgpu_obs_influe
   if (!why.empty()) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_observation_influence: " + why);
   CovSpace w;
   VC_TRY(run_cov(h, nullptr, kCovDiagCross, nullptr, &w));
-  const InflSrc src{w.inv, w.N, w.out_ff, w.out};
+  const InflSrc src{w.inv, w.N, w.out_ff, w.out, w.out_next};
   int st = VCGPU_OK;
   VC_TRY(run_obs_infl(&h, 1, &src, out, &st));
   if (st != VCGPU_OK) return fail(h, st, "vcgpu_get_observation_influence: Sigma_F is not positive definite");
@@ -1223,6 +1224,29 @@ extern "C" int vcgpu_get_observation_influence_batch(vcgpu_handle* const* handle
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!out) return batch_refuse(handles, n, 0, "null out array", "vcgpu_get_observation_influence_batch");
   return run_obs_infl_batch(handles, n, out, status);
+}
+
+// The regression diagnostics of every IMU interval (vc_imu_infl.cuh), and of every observation where obs is given, from
+// one elimination and selected inversion of this handle (run_cov, kCovDiagCross), then run_imu_infl of this handle alone.
+extern "C" int vcgpu_get_imu_influence(vcgpu_handle* h, vcgpu_imu_influence* imu, vcgpu_obs_influence* obs) {
+  if (!h) return VCGPU_ERR_INVALID;
+  const std::string why = imu_infl_refusal(h, imu, obs);
+  if (!why.empty()) return fail(h, VCGPU_ERR_INVALID, "vcgpu_get_imu_influence: " + why);
+  CovSpace w;
+  const int rc = run_cov(h, nullptr, kCovDiagCross, nullptr, &w);
+  if (rc == VCGPU_ERR_NUMERIC) return fail(h, rc, "vcgpu_get_imu_influence: J^T J is singular at the current state");
+  VC_TRY(rc);
+  const InflSrc src{w.inv, w.N, w.out_ff, w.out, w.out_next};
+  int st = VCGPU_OK;
+  VC_TRY(run_imu_infl(&h, 1, &src, imu, obs, &st));
+  if (st != VCGPU_OK) return fail(h, st, "vcgpu_get_imu_influence: Sigma_F is not positive definite");
+  return VCGPU_OK;
+}
+extern "C" int vcgpu_get_imu_influence_batch(vcgpu_handle* const* handles, int n, const vcgpu_imu_influence* imu,
+                                             const vcgpu_obs_influence* obs, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!imu) return batch_refuse(handles, n, 0, "null imu array", "vcgpu_get_imu_influence_batch");
+  return run_imu_infl_batch(handles, n, imu, obs, status);
 }
 
 

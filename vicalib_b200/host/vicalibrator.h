@@ -580,6 +580,23 @@ class ViCalibrator {
     Check(vcgpu_get_observation_influence(h_, &out), "get_observation_influence");
   }
 
+  // The regression diagnostics of every IMU interval k < NumFrames() - 1 (vcgpu_get_imu_influence): h 81 doubles per
+  // interval (its 9 x 9 leverage, row-major), stud the studentized residual, infl the shift of the calibration its
+  // deletion causes, measured in the calibration's covariance.  stud and infl assume unit observation variance; NaN in
+  // all three for an interval with no measurements.  Any output may be null, not all three.  The inertial terms must be
+  // active in the handle's last solve.  Call after the solve has finished (not while IsRunning()).
+  void GetImuInfluence(std::vector<double>* h, std::vector<double>* stud, std::vector<double>* infl) {
+    VICALIB_CHECK(!IsRunning(), "GetImuInfluence while running");
+    VICALIB_CHECK(h || stud || infl, "GetImuInfluence: every output is null");
+    VICALIB_CHECK(FLAGS_.calibrate_imu && is_inertial_active_, "GetImuInfluence: the inertial terms are not active");
+    const size_t nf = NumFrames(), ni = nf > 1 ? nf - 1 : 0;
+    if (h) h->assign(81 * ni, 0.0);
+    if (stud) stud->assign(ni, 0.0);
+    if (infl) infl->assign(ni, 0.0);
+    vcgpu_imu_influence out{h ? h->data() : nullptr, stud ? stud->data() : nullptr, infl ? infl->data() : nullptr};
+    Check(vcgpu_get_imu_influence(h_, &out, nullptr), "get_imu_influence");
+  }
+
   // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
   // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
   // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
