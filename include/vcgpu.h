@@ -749,6 +749,79 @@ int vcgpu_get_integration_poses(vcgpu_handle* h, int64_t* start, double* poses_o
 int vcgpu_get_integration_poses_batch(vcgpu_handle* const* handles, int n, int64_t* const* start,
                                       double* const* poses /* n pointers, or NULL; an entry may be NULL */);
 
+/* Hand-eye alignment of the gyro stream with the vision poses: the rotation Q from the IMU's axes to the rig's, the time
+ * offset ts and the gyro bias b_g, which every inertial solve starts from and the library cannot otherwise produce.  The
+ * intended call sits between a vision-only flow and the inertial one (INTEGRATION.md).  At the handle's current accepted
+ * state, over interval f = 0 .. n_frames - 2 (frames f, f+1):
+ *   a_f        log(R_f^T R_f+1), R_f the rotation of T_wp[f]: the rig's turn in its current axes;
+ *   b_f(s, b_g) log(dR_f), dR_f the attitude the solve's RK4 reaches from the identity over GetRange(t_f, t_f+1, s) with
+ *              the handle's gyro scale factors sf[0..2] and bias b_g (the accelerometer terms do not reach it);
+ *   usable     both frames are seen by an active observation, and [t_f, t_f+1] lies inside [t_first + s, t_last + s]
+ *              (t_first, t_last: the first and last IMU sample) for every s tried: [ts_lo, ts_hi], or the handle's ts
+ *              without find_time_offset.  n is their number; every sum below is over them.
+ *   grid       n_ts candidates s_c = ts_lo + c (ts_hi - ts_lo) / (n_ts - 1), the last exactly ts_hi (one candidate: ts_lo);
+ *              M(s) = sum a_f b_f^T, and cost(s) = (sum |a|^2 + sum |b|^2 - 2 lambda_max(N(M))) / n, N Horn's 4 x 4
+ *              matrix: the least mean |a_f - Q b_f|^2 over rotations Q, reached at Horn's Q.
+ *   start      the candidate of least cost (lowest index among equals), its Horn Q and the handle's b_g.
+ *   refinement up to max_iters Gauss-Newton iterations on (dtheta, s, b_g) with residual a_f - Exp(dtheta) Q b_f(s, b_g):
+ *              the s and b_g columns by one-direction duals through the interpolation and the RK4 chain (ts flows through
+ *              GetRange as in the solve's ts column).  A step is taken only if it lowers the cost, else it is halved, at
+ *              most 10 times; s is clamped to [ts_lo, ts_hi]; Q is renormalised after each step.  The fit stops when no
+ *              halving lowers the cost.
+ *   find_time_offset = 0 (the reference's flag name): no grid, s stays the handle's ts bit for bit, and only Q and b_g are
+ *              fitted; ts_lo, ts_hi and n_ts are checked but play no other part, and curve is not written.
+ * Outputs (vcgpu_imu_alignment): Q (IMU axes to the current rig axes, x y z w, w >= 0), ts, b_g, rms = sqrt(mean
+ * |a_f - Q b_f|^2) at the result in radians, excitation = the ascending eigenvalues of (1/n) sum b_f b_f^T at the result
+ * (two near zero: rotation about one axis, which leaves Q unobservable), n_intervals, iterations (steps taken), and, with
+ * find_time_offset, curve_or_null[n_ts] = cost(s_c) if the pointer is not NULL.
+ * apply = 0: nothing on the handle changes.  apply != 0 and VCGPU_OK: for every camera c and frame f q_ck[c] <- q_ck[c] (x)
+ * Q and T_wp[f].q <- T_wp[f].q (x) Q (Hamilton products, not renormalised), ts and b_g take the result; every camera pose
+ * T_wk T_ck^-1 is unchanged, and translations, p_ck, velocities, intrinsics, gravity, accelerometer bias and scale factors
+ * keep their bits.  The handle is left as vcgpu_set_cameras + vcgpu_set_frames + vcgpu_set_imu_params with those values
+ * leave it.
+ * The inertial flag is not required: without it the IMU samples of vcgpu_set_imu are uploaded by the call.
+ * VCGPU_ERR_NUMERIC, nothing applied: fewer than 3 usable intervals, or a Gauss-Newton normal matrix that fails its
+ * Cholesky factorisation.  curve, excitation, n_intervals and iterations are still written, Q, ts, b_g and rms are NaN.
+ * VCGPU_ERR_INVALID, before anything is launched and with nothing written: a null handle, opts or out; n_ts < 1 or above
+ * 65536; ts_lo > ts_hi or a bound that is not finite; max_iters < 0; fewer than two frames; no IMU samples; frame shards
+ * (one GPU only).  Runs as vcgpu_align_imu_batch of this handle alone: the same memory. */
+typedef struct {
+  double ts_lo, ts_hi;   /* seconds: the candidate time offsets' range, both ends included */
+  int n_ts;              /* candidates, 1 .. 65536 */
+  int find_time_offset;  /* 0: s stays the handle's ts */
+  int max_iters;         /* Gauss-Newton iterations at most, >= 0 */
+  int apply;             /* nonzero: the result goes on the handle */
+} vcgpu_imu_align_opts;
+typedef struct {
+  double Q[4];           /* x y z w, w >= 0 */
+  double ts;
+  double b_g[3];
+  double rms;            /* radians */
+  double excitation[3];  /* ascending */
+  int n_intervals, iterations;
+  double* curve_or_null; /* caller's n_ts doubles, or NULL */
+} vcgpu_imu_alignment;
+int vcgpu_align_imu(vcgpu_handle* h, const vcgpu_imu_align_opts* opts, vcgpu_imu_alignment* out);
+/* vcgpu_align_imu of n rigs in one call: opts[i] and out[i] are rig i's.  Per handle, on its own stream, prepare(), the
+ * accepted state read back and (inertial terms off) the IMU samples uploaded; then on handle 0's stream one upload of
+ * every rig's usable intervals and four launches over every rig: a_f (one thread per interval), the grid (one CTA per
+ * rig, candidate and tile of 128 intervals; each thread integrates its interval's attitude and the CTA reduces the 11
+ * sums in a fixed order into the tile's partial), the costs (one thread per candidate: the tiles in order, Horn's
+ * matrix and its cyclic Jacobi eigen-solve) and the refinement (one CTA per rig: the argmin, Gauss-Newton with fixed-order
+ * 7 x 7 reductions and a one-thread Cholesky, the excitation).  Every reduction order is a function of the rig alone, so a
+ * rig's outputs are the bits of its own call whatever else is in the batch and in whatever order.
+ * status: n codes or NULL.  VCGPU_ERR_NUMERIC: as vcgpu_align_imu for one or more rigs; their status is
+ * VCGPU_ERR_NUMERIC and nothing is applied to them, every other rig is written (and applied) with status VCGPU_OK, and
+ * the message names the first failing index.
+ * VCGPU_ERR_INVALID before anything is launched and writes nothing, with a message naming the index in vcgpu_last_error
+ * of every non-null handle: n <= 0, a null opts or out, a null or repeated handle, handles on different devices, a rig
+ * vcgpu_align_imu refuses, and more than 2^31 - 1 grid CTAs in all.
+ * Device memory, held by handle 0 and grown to the largest batch, never freed per call: per usable interval 48 bytes, per
+ * candidate 40 bytes and 88 per tile of 128 intervals (the partials: 401 candidates of 2000 intervals take 0.6 MB), 128
+ * bytes per rig of results and the kernel arguments; per handle without inertial terms its IMU samples, 56 bytes each. */
+int vcgpu_align_imu_batch(vcgpu_handle* const* handles, int n, const vcgpu_imu_align_opts* opts /* n */,
+                          vcgpu_imu_alignment* out /* n */, int* status /* n, or NULL */);
+
 /* ---- inspection hooks used by the parity tests (what AutoDiffCostFunction::Evaluate and the
  * normal-equation build produce inside Ceres) ------------------------------------------------ */
 /* loss-free residuals and tangent-space Jacobians per observation, caller order.

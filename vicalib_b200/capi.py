@@ -34,6 +34,7 @@ EXPORTS = [
     "vcgpu_get_view_information", "vcgpu_get_view_information_batch",
     "vcgpu_get_observation_influence", "vcgpu_get_observation_influence_batch",
     "vcgpu_get_imu_influence", "vcgpu_get_imu_influence_batch",
+    "vcgpu_align_imu", "vcgpu_align_imu_batch",
 ]
 
 CHI2_95_9 = 16.9190  # chi2inv(0.95, 9): the bound UpdateImuWeights logs each interval's distance against
@@ -170,6 +171,35 @@ def _imu_influence_result(keep, ni, obs_keep, n_obs):
     out = {k: a[:ni] for k, a in zip(("h", "stud", "infl"), keep) if a is not None}
     if obs_keep is not None:
         out["observations"] = _obs_influence_result(obs_keep, n_obs)
+    return out
+
+
+class ImuAlignOpts(C.Structure):
+    """vcgpu_imu_align_opts"""
+    _fields_ = [("ts_lo", C.c_double), ("ts_hi", C.c_double), ("n_ts", C.c_int), ("find_time_offset", C.c_int),
+                ("max_iters", C.c_int), ("apply", C.c_int)]
+
+
+class ImuAlignment(C.Structure):
+    """vcgpu_imu_alignment"""
+    _fields_ = [("Q", C.c_double * 4), ("ts", C.c_double), ("b_g", C.c_double * 3), ("rms", C.c_double),
+                ("excitation", C.c_double * 3), ("n_intervals", C.c_int), ("iterations", C.c_int),
+                ("curve_or_null", C.c_void_p)]
+
+
+def _align_args(ts_lo, ts_hi, n_ts, find_time_offset, max_iters, apply, curve):
+    """the opts, the output struct and the curve array of one rig (the array must outlive the call)"""
+    c = np.full(max(int(n_ts), 1), np.nan) if curve else None
+    o = ImuAlignOpts(float(ts_lo), float(ts_hi), int(n_ts), int(bool(find_time_offset)), int(max_iters), int(bool(apply)))
+    return o, ImuAlignment(curve_or_null=None if c is None else c.ctypes.data), c
+
+
+def _align_result(a, c, status):
+    """dict(Q, ts, b_g, rms, excitation, n_intervals, iterations, status[, curve]) of one rig"""
+    out = dict(Q=np.array(a.Q[:]), ts=a.ts, b_g=np.array(a.b_g[:]), rms=a.rms, excitation=np.array(a.excitation[:]),
+               n_intervals=a.n_intervals, iterations=a.iterations, status=int(status))
+    if c is not None:
+        out["curve"] = c
     return out
 
 
@@ -553,6 +583,19 @@ class Calibrator:
         self._chk(self.L.vcgpu_get_imu_influence(self.h, C.byref(o), C.byref(oo) if observations else None))
         return _imu_influence_result(keep, ni, okeep, self.n_obs)
 
+    def align_imu(self, ts_lo=-0.1, ts_hi=0.1, n_ts=401, find_time_offset=True, max_iters=20, apply=False, curve=False):
+        """vcgpu_align_imu: the rotation Q (IMU axes to the current rig axes, x y z w with w >= 0), time offset ts and
+        gyro bias b_g that align the gyro stream with the frame poses' turns, from a grid of n_ts offsets in
+        [ts_lo, ts_hi] and a Gauss-Newton refinement.  Returns dict(Q, ts, b_g, rms, excitation, n_intervals, iterations,
+        status[, curve]); status is 0, or -3 (VCGPU_ERR_NUMERIC: fewer than 3 usable intervals or a singular fit; Q, ts,
+        b_g and rms are then NaN and nothing is applied).  apply=True puts the result on the handle: q_ck and every
+        frame's rotation right-multiplied by Q, ts and b_g replaced.  The inertial flag is not required."""
+        o, a, c = _align_args(ts_lo, ts_hi, n_ts, find_time_offset, max_iters, apply, curve)
+        rc = self.L.vcgpu_align_imu(self.h, C.byref(o), C.byref(a))
+        if rc not in (0, -3):
+            self._chk(rc)
+        return _align_result(a, c, rc)
+
     def phase_clocks(self):
         """raw phase clocks (ns) of the persistent inertial kernels, see vcgpu_get_phase_clocks"""
         ns = np.zeros(64, dtype=np.uint64)
@@ -794,6 +837,25 @@ def imu_influence_batch(calibrators, h=True, stud=True, infl=True, observations=
             e.results = [out[i] if st[i] == 0 else None for i in range(n)]
         raise e
     return out
+
+
+def align_imu_batch(calibrators, ts_lo=-0.1, ts_hi=0.1, n_ts=401, find_time_offset=True, max_iters=20, apply=False,
+                    curve=False):
+    """vcgpu_align_imu_batch: Calibrator.align_imu() of every Calibrator of the list in one call, each rig's result the
+    bits its own call returns.  Any option may be one value or a list with one value per calibrator.  Returns one dict
+    per calibrator, in order, as align_imu() returns it (status -3 marks a rig whose fit failed)."""
+    n = len(calibrators)
+    L = lib()
+    per = [v if isinstance(v, (list, tuple)) else [v] * n for v in (ts_lo, ts_hi, n_ts, find_time_offset, max_iters, apply, curve)]
+    args = [_align_args(*(v[i] for v in per)) for i in range(n)]
+    hs = (C.c_void_p * max(n, 1))(*[None if g is None else g.h for g in calibrators])
+    opts = (ImuAlignOpts * max(n, 1))(*[a[0] for a in args])
+    outs = (ImuAlignment * max(n, 1))(*[a[1] for a in args])
+    status = (C.c_int * max(n, 1))()
+    rc = L.vcgpu_align_imu_batch(hs, C.c_int(n), opts, outs, status)
+    if rc not in (0, -3):
+        _batch_check(L, rc, calibrators)
+    return [_align_result(outs[i], args[i][2], status[i]) for i in range(n)]
 
 
 def _split_poses(start, poses):

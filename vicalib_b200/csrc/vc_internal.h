@@ -226,6 +226,9 @@ struct vcgpu_handle {
   unsigned char* d_infl_obs = nullptr;
   std::vector<vc::InflTile> infl_tiles;
   bool infl_obs_valid = false;
+  // vcgpu_align_imu(_batch) with this handle as handle 0: every rig's usable intervals, a_j, grid partials, curve,
+  // candidate rotations and results (vc_batch.inl: run_align_imu_batch)
+  double* d_align = nullptr;
   // vcgpu_get_covariance_batch: this handle's [G*G] matrix | [kScCount] flags | vision: [8][G*G+G] CTA partials | [G*G+G] total
   double* d_cov = nullptr;
   // persistent inertial kernels (vc_imu_mega.cuh, vc_imu_eval_mega.cuh)

@@ -36,6 +36,7 @@
 #include "vc_view_info.cuh"
 #include "vc_obs_infl.cuh"
 #include "vc_imu_infl.cuh"
+#include "vc_imu_align.cuh"
 
 using namespace vc;
 
@@ -225,7 +226,7 @@ extern "C" int vcgpu_destroy(vcgpu_handle* h) {
   dev_free(&h->d_blk_mem[0]); dev_free(&h->d_blk_mem[1]);
   dev_free(&h->d_scale); dev_free(&h->d_X); dev_free(&h->d_Spart); dev_free(&h->d_delta);
   dev_free(&h->d_red); dev_free(&h->d_scalars); dev_free(&h->d_Ssum); dev_free(&h->d_red_part); dev_free(&h->d_counter);
-  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_view); dev_free(&h->d_infl); dev_free(&h->d_infl_obs); h->infl_obs_valid = false; dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
+  dev_free(&h->d_dl); dev_free(&h->d_dl_part); dev_free(&h->d_partS); dev_free(&h->d_partC); dev_free(&h->d_batch_args); dev_free(&h->d_eval); dev_free(&h->d_pnp); dev_free(&h->d_mahal); dev_free(&h->d_pstart); dev_free(&h->d_poses); dev_free(&h->d_proj); dev_free(&h->d_view); dev_free(&h->d_infl); dev_free(&h->d_infl_obs); h->infl_obs_valid = false; dev_free(&h->d_align); dev_free(&h->d_rank); dev_free(&h->d_cov); dev_free(&h->d_fcov); dev_free(&h->d_prof); dev_free(&h->d_prof2); dev_free(&h->d_csync);
   dev_free(&h->d_imu); dev_free(&h->d_wsqrt); h->d_wvec = nullptr; dev_free(&h->d_imu_r); dev_free(&h->d_imu_J);
   imu_free(h);
   dev_free(&h->d_mg); dev_free(&h->d_sep); dev_free(&h->d_dense); dev_free(&h->d_dsys);
@@ -1320,6 +1321,20 @@ extern "C" int vcgpu_get_integration_poses_batch(vcgpu_handle* const* handles, i
   if (!handles || n <= 0) return VCGPU_ERR_INVALID;
   if (!start) return batch_refuse(handles, n, 0, "null start array", "vcgpu_get_integration_poses_batch");
   return run_integration_poses_batch(handles, n, start, poses, "vcgpu_get_integration_poses_batch");
+}
+
+// hand-eye alignment of the gyro stream with the vision poses: run_align_imu_batch of this handle alone
+extern "C" int vcgpu_align_imu(vcgpu_handle* h, const vcgpu_imu_align_opts* opts, vcgpu_imu_alignment* out) {
+  if (!h) return VCGPU_ERR_INVALID;
+  if (!opts || !out) return fail(h, VCGPU_ERR_INVALID, "vcgpu_align_imu: null opts or out");
+  return run_align_imu_batch(&h, 1, opts, out, nullptr, "vcgpu_align_imu");
+}
+extern "C" int vcgpu_align_imu_batch(vcgpu_handle* const* handles, int n, const vcgpu_imu_align_opts* opts,
+                                     vcgpu_imu_alignment* out, int* status) {
+  if (!handles || n <= 0) return VCGPU_ERR_INVALID;
+  if (!opts) return batch_refuse(handles, n, 0, "null opts array", "vcgpu_align_imu_batch");
+  if (!out) return batch_refuse(handles, n, 0, "null out array", "vcgpu_align_imu_batch");
+  return run_align_imu_batch(handles, n, opts, out, status, "vcgpu_align_imu_batch");
 }
 
 extern "C" int vcgpu_comm_unique_id(uint8_t id[VCGPU_UNIQUE_ID_BYTES]) {

@@ -597,6 +597,23 @@ class ViCalibrator {
     Check(vcgpu_get_imu_influence(h_, &out, nullptr), "get_imu_influence");
   }
 
+  // The hand-eye alignment of the gyro stream with the frame poses (vcgpu_align_imu, applied): the rotation Q from the
+  // IMU's axes to the rig's, the time offset and the gyro bias, from n_ts candidate offsets in [ts_lo, ts_hi] (without
+  // find_time_offset the current offset is kept) and a Gauss-Newton refinement of at most max_iters steps.  On success
+  // every camera's T_ck and every frame's rotation are right-multiplied by Q, and time_offset() and the gyro part of
+  // GetBiases() take the result; camera poses T_wk T_ck^-1 do not change.  Returns the call's outputs; a fit that fails
+  // (fewer than 3 usable intervals, a singular system) aborts as every other device error does.  Call between the
+  // vision-only solve and the inertial stages, after the solve has finished (not while IsRunning()).
+  vcgpu_imu_alignment AlignImu(double ts_lo, double ts_hi, int n_ts, bool find_time_offset, int max_iters = 20) {
+    VICALIB_CHECK(!IsRunning(), "AlignImu while running");
+    VICALIB_CHECK(problem_uploaded_, "AlignImu before the problem is on the device (run the vision solve first)");
+    const vcgpu_imu_align_opts o{ts_lo, ts_hi, n_ts, find_time_offset ? 1 : 0, max_iters, 1};
+    vcgpu_imu_alignment r{};
+    Check(vcgpu_align_imu(h_, &o, &r), "align_imu");
+    ReadBackState();
+    return r;
+  }
+
   // GetIntegrationPoses(k) for every k < NumFrames() - 1, computed on the device from the current solution: one vector
   // per interval, empty where the interval has no IMU measurements, and all empty unless the inertial terms are active
   // and the stage is not rotation-only (the reference's gate, vicalibrator.h:510).  Call after the solve has finished
